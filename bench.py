@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - H-Codec-2.0 encode + RVQ + decode throughput on B200 (BASELINE.json configs[1]).
+"""bench.py - H-Codec-2.0 encode + RVQ + decode throughput on H100 (BASELINE.json configs[1]).
 
 A "step" = one pass of the hot path (Codec.encode -> Codec.decode) over one synthetic batch of
 B=64 clips x 10 s at the shipped 48 kHz configuration (480 000 samples / clip, 125 tokens / stream),
@@ -9,8 +9,9 @@ weights / datasets exist offline, hence `data: synthetic`.
   python bench.py --gpus 1 --steps 5 --warmup 3            # our arm (CUDA kernels via the C ABI)
   python bench.py --impl reference --steps 2 --warmup 1     # the reference's CPU path (oracle port)
   torchrun ... bench.py --gpus N ...                        # one rank per GPU, weak scaling
+  python bench.py --steps 5 --dump-outputs out/             # + what the last timed step computed, as .npy
 
-Prints ONE JSON line (see README / DESIGN.md "Measurement").
+Prints ONE JSON line (see README).
 """
 from __future__ import annotations
 
@@ -53,7 +54,8 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sus=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sus=1400.0, src="fallback")
+    # H100 SXM data sheet (700 W): HBM3 bandwidth and dense bf16 rate - an upper bound, not a measured figure
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sus=989.0, src="H100 SXM data sheet")
 
 
 def random_init_(model, seed: int):
@@ -89,7 +91,7 @@ def random_init_(model, seed: int):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     def __init__(self, gpu_index: int):
         self.gpu, self.rows, self.proc = gpu_index, [], None
@@ -157,7 +159,7 @@ class Ctx:
         self.dev = torch.device("cuda", self.local)
         self.dist = None
         self.t0 = time.perf_counter()
-        # wall-clock budget for the optional legs (the driver's per-N limit in the scaling run is 870 s): a leg that would start
+        # wall-clock budget for the optional legs: a leg that would start
         # after the budget is recorded as skipped instead of endangering the headline line
         self.budget_s = float(os.environ.get("QB_BENCH_BUDGET_S", "540"))
         if self.world > 1:
@@ -376,7 +378,7 @@ def bench_lm_generate(args, ctx, m, task, B_local, total_batch=None, with_cpu=Fa
                                     f"steps, KV <= {P + 283}", batch=B_all, batch_per_gpu=B_local, semantic_length=T,
                            parallelism=f"dp{world} (sequences sharded, one NCCL all_gather of ids)",
                            chunks=f"{chunks_local} chunk(s) of <= {m.chunk} sequences per GPU on {min(m.lanes, chunks_local)} concurrent lane(s) "
-                                  "(own stream / KV cache / captured graphs each; profiles/r02_lm_lanes_ab.md)",
+                                  "(own stream / KV cache / captured graphs each)",
                            launches="decode steps replay captured CUDA graphs (8 steps x 62 kernels each); gpu_launches counts the eager launches "
                                     "(prefill, adapter) per generation"),
                e2e=dict(value=B_all * 283 / (ms_e2e * 1e-3), unit="tokens/s", ms_per_step=ms_e2e,
@@ -718,6 +720,26 @@ def bench_h15(args, ctx):
                               flops_per_step=flops[0]))
 
 
+DUMP_WAV_SAMPLES = 1 << 22      # 16 MB of float32: a fixed sample of the decoded batch (the whole of it is 123 MB at B = 64 x 10 s)
+
+
+def dump_codec_outputs(out_dir, ac, sc, rec):
+    """What the caller of Codec.encode -> Codec.decode receives from the last timed step, as .npy: the acoustic and semantic codes
+    (exact in float64) and the waveform at DUMP_WAV_SAMPLES positions drawn once from a fixed seed (all of it when it is smaller),
+    with those flat positions, so that two builds can be compared output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, "acoustic_codes.npy"), ac.detach().cpu().double().numpy())
+    np.save(os.path.join(out_dir, "semantic_codes.npy"), sc.detach().cpu().double().numpy())
+    flat = rec.detach().float().reshape(-1)
+    if flat.numel() > DUMP_WAV_SAMPLES:
+        idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_WAV_SAMPLES].sort().values
+        np.save(os.path.join(out_dir, "waveform_sample_index.npy"), idx.double().numpy())
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(out_dir, "waveform_sample.npy"), flat.cpu().numpy())
+
+
 def run_codec(args, cfg, ctx, collect_secondary, first_legs=None):
     from unified_audio_b200 import ops
     from unified_audio_b200.parallel import gather_tokens
@@ -739,6 +761,7 @@ def run_codec(args, cfg, ctx, collect_secondary, first_legs=None):
             torch.cuda.synchronize()
     gbuf = {}
     tok_stack = torch.zeros(B, 2, 16, T // 3840, dtype=torch.int64, device=dev)
+    last = {}
 
     def step_device():
         if graphed is not None:
@@ -750,6 +773,7 @@ def run_codec(args, cfg, ctx, collect_secondary, first_legs=None):
             tok_stack[:, 0].copy_(ac)
             tok_stack[:, 1].copy_(sc)
             gather_tokens(tok_stack, world * B, buffers=gbuf)
+        last["out"] = (ac, sc, rec)
         return ac, sc, rec
 
     codes_h = torch.empty(2, B, 16, T // 3840, dtype=torch.int64).pin_memory()
@@ -785,6 +809,8 @@ def run_codec(args, cfg, ctx, collect_secondary, first_legs=None):
         for _ in range(args.warmup):
             step_device()
         ms = ctx.timed(step_device, args.steps)
+        if rank == 0 and args.dump_outputs:
+            dump_codec_outputs(args.dump_outputs, *last["out"])
         if rank == 0:
             print(json.dumps(dict(quick=True, ms_per_step=ms, value=world * B * T / (ms * 1e-3))))
         return None
@@ -795,6 +821,8 @@ def run_codec(args, cfg, ctx, collect_secondary, first_legs=None):
         sampler.start()
     ops.launch_count_reset()
     ms = ctx.timed(step_device, args.steps)
+    if rank == 0 and args.dump_outputs:
+        dump_codec_outputs(args.dump_outputs, *last["out"])
     launches = ops.launch_count() + (graphed.launches_per_replay * args.steps if graphed is not None else 0)
     clocks = sampler.stop() if rank == 0 else None
     for _ in range(2):
@@ -826,7 +854,7 @@ def run_codec(args, cfg, ctx, collect_secondary, first_legs=None):
     e2e_split = dict(h2d_ms=ev[0].elapsed_time(ev[1]), compute_ms=ev[1].elapsed_time(ev[2]), d2h_ms=ev[2].elapsed_time(ev[3]),
                      note="one extra step, serial on the launching stream (no overlap between copies and kernels)")
 
-    # ---- roofline of the dominant kernel: the ConvNeXt pointwise GEMM (tcgen05), timed alone on operands of the step's shapes
+    # ---- roofline of the dominant kernel: the ConvNeXt pointwise GEMM (wgmma), timed alone on operands of the step's shapes
     M, C, I = B * F_, 1536, 4608
     sd_ = model.state_dict()
     w1 = ops.Planes.from_f32(sd_["encoder.prior_net.0.pwconv1.linear.weight"], False)
@@ -862,7 +890,7 @@ def run_codec(args, cfg, ctx, collect_secondary, first_legs=None):
         data="synthetic",
         config=dict(workload=f"HCodec-2.0 batch={B} x {args.seconds:g} s (48 kHz shipped config, {T} samples/clip) encode+RVQ+decode",
                     batch_per_gpu=B, samples_per_clip=T, tokens_per_stream=T // 3840, precision_policy=args.precision,
-                    l2="working set per step (~3 GB activations + 4.6 GB weights) exceeds the 126 MB L2; no flush needed",
+                    l2="working set per step (~3 GB activations + 4.6 GB weights) exceeds the 50 MB L2; no flush needed",
                     parallelism=f"dp{world} (clips sharded, one NCCL all_gather_into_tensor of tokens)",
                     launch="one CUDA graph replay per step (Codec.graphed('roundtrip')); gpu_launches = library kernels in the "
                            "graph x steps" if graphed is not None else "kernel by kernel"),
@@ -1096,7 +1124,7 @@ def run_bicodec(args):
         dtype="f16x3 split tensor-core (fp32-grade), f32 accumulate", data="synthetic",
         config=dict(workload="BiCodec detokenize (UniSE's decoder): 32 clips x 250 semantic + 32 global tokens -> 5 s @ 16 kHz",
                     batch_per_gpu=B, tokens=T, precision_policy="accurate",
-                    l2="activations per step (~10 GB) exceed the 126 MB L2; no flush needed",
+                    l2="activations per step (~10 GB) exceed the 50 MB L2; no flush needed",
                     parallelism=f"dp{world} (clips sharded, no collective)"),
         e2e=dict(value=samples / (ms_e2e * 1e-3), unit="samples/s", ms_per_step=ms_e2e,
                  h2d_bytes_per_step=int(sem_h.numel() * 8 + glob_h.numel() * 8) * world,
@@ -1123,10 +1151,14 @@ def main():
     ap.add_argument("--ref-clips", type=int, default=2)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--workload", default="all", choices=["all", "codec", "lm", "lm_tse", "lm_forward", "bicodec", "h15"],
-                    help="all (default, the driver's line) = the codec line (BASELINE configs[1]) with the UniSE AR-LM legs (configs[2], [3], "
+                    help="all (default) = the codec line (BASELINE configs[1]) with the UniSE AR-LM legs (configs[2], [3], "
                          "[4]) under `secondary`; codec / lm / lm_tse / lm_forward / bicodec = that line alone")
     ap.add_argument("--quick", action="store_true", help="profiling aid: W warm-up + K steps only, no e2e/roofline/cpu legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the codec line's last timed step computed (codes, a fixed sample of the waveform) to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload not in ("all", "codec")):
+        ap.error("--dump-outputs writes the outputs of the codec line: use it with --impl ours and --workload all or codec")
     args.warmup = max(args.warmup, 0)
     cfg = H2_FULL
     if args.workload == "bicodec":

@@ -1,5 +1,5 @@
 /*
- * libquark_b200 - C ABI of the B200-native QuarkAudio audio-token hot path.
+ * libquark_b200 - C ABI of the H100-native QuarkAudio audio-token hot path.
  *
  * The reference (alibaba/unified-audio) is pure Python/PyTorch and has no FFI layer; its boundary
  * for this path is the nn.Module method surface (SURVEY.md 8b).  The entry points below are what a
@@ -93,7 +93,7 @@ typedef struct {
                              * (HuBERT / WavLM positional conv: k = 128, 16 groups, transformers modeling_hubert.py) */
 } qb_gemm_desc;
 
-/* tcgen05 / TMA / TMEM persistent GEMM (the product path). */
+/* wgmma / TMA persistent GEMM (the product path). */
 int qb_gemm(const qb_gemm_desc* d, void* stream);
 /* Name of the kernel variant qb_gemm runs for this shape (m_per_batch output rows per batch, n columns, split != 0 for the
  * 3-term mode) - static string, used by bench.py's roofline label. */
@@ -200,7 +200,7 @@ int qb_attention_hd(const float* qkv, int64_t B, int64_t T, int32_t heads, int32
 int64_t qb_attention_tc_workspace_bytes(int64_t B, int64_t T, int32_t heads);
 int qb_attention_tc(const float* qkv, int64_t B, int64_t T, int32_t heads, const float* rope_cos,
                     const float* rope_sin, qb_half* out_hi, qb_half* out_lo, void* workspace, void* stream);
-/* The same attention on the 5th-gen tensor cores (tcgen05.mma, accumulators in TMEM, TMA-fed operands; csrc/attention_umma.cu):
+/* The same attention on the Hopper tensor cores (wgmma, accumulators in registers, TMA-fed operands; csrc/attention_umma.cu):
  * head_dim 64 or 128, any L; split = 0: single-pass fp16 operands, split = 1: fp16 hi + lo operands for both contractions (3 passes,
  * fp32-grade); causal = 1: query t attends keys <= t (the AR-LM's teacher-forced / prefill attention, U/model/llm/llm.py:195-216).
  * q is scaled by head_dim^-0.5; rope tables [L, head_dim] in the rotate-half layout.  workspace: 128-byte aligned,
@@ -216,7 +216,7 @@ int64_t qb_lstm_workspace_bytes(int64_t B, int64_t H);
 int qb_lstm(const float* xp, const qb_half* whh_hi, const qb_half* whh_lo, int64_t B, int64_t T, int64_t H,
             qb_half* out_hi, qb_half* out_lo, void* workspace, void* stream);
 
-/* Same recurrence on tcgen05 / TMEM / TMA (the product path; lstm.cu's mma.sync version is kept as a
+/* Same recurrence on wgmma / TMA (the product path; lstm.cu's mma.sync version is kept as a
  * cross-check).  whh_perm: fp16 [H/U][4U][H] with row (4j+g) of slice c = gate g of hidden unit c*U+j,
  * U = qb_lstm_tc_units(H).  B <= 256 per call.  workspace: qb_lstm_tc_workspace_bytes(B,H). */
 int32_t qb_lstm_tc_units(int64_t H);

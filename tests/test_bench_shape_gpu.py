@@ -1,7 +1,7 @@
 """Parity AT THE BENCHMARKED SHAPES (VERDICT r01 "what's weak" 1-5): the shipped H-Codec-2.0 configuration on 10 s clips
 (T = 500 STFT frames, 125 tokens / stream) against the CPU oracle, both precision policies and both weight
 initialisations (oracle.weights and bench.py::random_init_); end-to-end RVQ index identity asserted with the
-Lipschitz audit of oracle/parity.py; the tcgen05 LSTM against torch's own fp64 / fp32 nn.LSTM at H = 1536, T = 500,
+Lipschitz audit of oracle/parity.py; the wgmma LSTM against torch's own fp64 / fp32 nn.LSTM at H = 1536, T = 500,
 B = 64; the UniSE LM at the SR (prefix 252, B = 32) and TSE (prefix 503, B = 16) shapes over all 283 cached steps.
 
 Sizes: QB_PARITY_CLIPS (default 64 = one full bench batch = 8000 tokens / stream) sets the audit batch."""
@@ -151,7 +151,7 @@ def test_h2_index_identity_full_batch(lib):
 
 
 def test_lstm_vs_torch_lstm_bench_shape(lib):
-    """tcgen05 LSTM (fp16 W_hh / h operands, fp32 accumulate and cell state) against torch.nn.LSTM in fp64 (truth) and in
+    """wgmma LSTM (fp16 W_hh / h operands, fp32 accumulate and cell state) against torch.nn.LSTM in fp64 (truth) and in
     fp32 (what the reference runs, encoder_modules/transformer.py:115,133) at the benchmarked shape H=1536, T=500, B=64."""
     from unified_audio_b200 import ops
     B, T, H = 64, 500, 1536

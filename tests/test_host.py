@@ -179,6 +179,8 @@ def test_precision_policies_cover_every_gemm_group():
 
 # ----------------------------------------------------------------------------- C ABI
 def test_library_builds_loads_and_exports_every_declared_symbol(lib):
+    import torch
+    launched = lib.qb_launch_count()           # GPU tests earlier in the same session may have launched kernels
     hdr = open(os.path.join(ROOT, "include", "quark_b200.h")).read()
     declared = set(re.findall(r"\b(qb_[a-z0-9_]+)\s*\(", hdr))
     declared -= {"qb_gemm_desc", "qb_rowmap", "qb_half"}
@@ -187,7 +189,9 @@ def test_library_builds_loads_and_exports_every_declared_symbol(lib):
     for name in declared:
         assert getattr(lib, name) is not None
     assert lib.qb_version() >= 100
-    assert lib.qb_launch_count() == 0          # nothing computed on the CPU box
+    assert lib.qb_launch_count() == launched   # resolving and querying the symbols launches nothing
+    if not torch.cuda.is_available():
+        assert launched == 0                   # nothing computed on a machine without a GPU
 
 
 def test_gemm_desc_struct_layout_matches_header():

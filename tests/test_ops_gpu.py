@@ -187,7 +187,7 @@ def test_attention(lib):
 @pytest.mark.parametrize("D,split", [(64, True), (64, False), (128, True), (128, False)])
 @pytest.mark.parametrize("B,T,H", [(2, 37, 3), (1, 64, 2), (3, 250, 8), (2, 382, 4), (1, 515, 2)])
 def test_attention_umma(lib, D, split, B, T, H):
-    """tcgen05 attention (csrc/attention_umma.cu) against fp64 softmax attention; ragged lengths exercise the TMA zero fill of the
+    """wgmma attention (csrc/attention_umma.cu) against fp64 softmax attention; ragged lengths exercise the TMA zero fill of the
     last query / key tiles, 515 the 9-tile K/V ring; and against the fp32 SIMT kernel it replaces"""
     from unified_audio_b200 import ops
     qkv = _mk((B, T, 3 * H * D), 31 + T)
@@ -250,7 +250,7 @@ def test_lstm(lib, B, T, H):
     ref = torch.stack(outs, 1)
     e = relerr(planes_ref(out), ref)
     print(f"lstm B{B} T{T} H{H} relerr {e:.3e}")
-    # tcgen05 version (product path)
+    # wgmma version (product path)
     U = ops.lstm_tc_units(H)
     out2 = ops.Planes.zeros((B, T, H), True, DEV)
     ws2 = torch.zeros(ops.lstm_tc_workspace_bytes(B, H), dtype=torch.uint8, device=DEV)

@@ -1,4 +1,4 @@
-"""unified_audio_b200 - B200-native (sm_100a) implementation of QuarkAudio's audio-token hot path.
+"""unified_audio_b200 - H100-native (sm_90a) implementation of QuarkAudio's audio-token hot path.
 
 Public surface mirrors the reference (alibaba/unified-audio):
   Codec            <- QuarkAudio-HCodec/HCodec-2.0/vq/codec.py:17   (encode / decode)

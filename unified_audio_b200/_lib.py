@@ -1,6 +1,6 @@
 """ctypes binding of libquark_b200.so (the C ABI declared in include/quark_b200.h).
 
-The library is built in-tree by unified_audio_b200/build.py (nvcc, sm_100a).  There is NO fallback:
+The library is built in-tree by unified_audio_b200/build.py (nvcc, sm_90a).  There is NO fallback:
 if the shared library is missing or a call fails, a RuntimeError is raised.
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""Build libquark_b200.so in-tree with nvcc for sm_100a (no GPU needed: cross-compiles)."""
+"""Build libquark_b200.so in-tree with nvcc for sm_90a (no GPU needed: cross-compiles)."""
 from __future__ import annotations
 
 import os
@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libquark_b200.so")
 SOURCES = ["gemm.cu", "elementwise.cu", "attention.cu", "attention_umma.cu", "lstm.cu", "lstm_tc.cu", "rvq.cu", "llm.cu", "engine.cu", "ssl.cu", "llm_step.cu", "adaptive.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-I" + os.path.join(os.path.dirname(HERE), "include"), "-I" + CSRC]
 
 

@@ -301,7 +301,7 @@ class Codec(nn.Module):
         lstm_u = ops.lstm_tc_units(C) if use_tc else 0
         cos, sin = self._rope(F, hd)
         legacy = os.environ.get("QB_ATTENTION", "umma") == "legacy"
-        umma = (not legacy) and hd in (64, 128)          # tcgen05 attention (csrc/attention_umma.cu), both precision policies
+        umma = (not legacy) and hd in (64, 128)          # wgmma attention (csrc/attention_umma.cu), both precision policies
         tc_att = (not umma) and (not pa) and hd == 64
         att_ws = (self._buf("att5_ws", (ops.attention_umma_workspace_bytes(B, F, heads, hd, pa),), torch.uint8) if umma else
                   self._buf("att_ws", (ops.attention_tc_workspace_bytes(B, F, heads),), torch.uint8) if tc_att else None)

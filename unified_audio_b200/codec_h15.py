@@ -159,7 +159,7 @@ class CodecH15(CodecH1):
         hid = self._planes("mm_hid", (M, FF), split)
         qkv = self._buf("mm_qkv", (M, 3 * C))
         cos, sin = self._rope_mimi(L, hd)
-        umma = hd in (64, 128) and os.environ.get("QB_ATTENTION", "umma") != "legacy"      # tcgen05 attention (csrc/attention_umma.cu)
+        umma = hd in (64, 128) and os.environ.get("QB_ATTENTION", "umma") != "legacy"      # wgmma attention (csrc/attention_umma.cu)
         tc_att = (not umma) and (not split) and hd == 64
         att_ws = (self._buf("att5_ws", (ops.attention_umma_workspace_bytes(B, L, heads, hd, split),), torch.uint8) if umma else
                   self._buf("att_ws", (ops.attention_tc_workspace_bytes(B, L, heads),), torch.uint8) if tc_att else None)

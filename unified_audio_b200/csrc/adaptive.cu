@@ -151,7 +151,7 @@ agg_gather_kernel(const float* __restrict__ x, const int* __restrict__ qpos, con
 }
 static inline unsigned ad_grid(long long total) {
   long long g = (total + 255) / 256;
-  return (unsigned)(g < 1 ? 1 : (g > 148 * 16 ? 148 * 16 : g));
+  return (unsigned)(g < 1 ? 1 : (g > 132 * 16 ? 132 * 16 : g));
 }
 }  // namespace qb
 using namespace qb;

@@ -2,7 +2,7 @@
 // (reference: HCodec-2.0/vq/encoder_modules/transformer.py:134-215).
 // v1: fp32 SIMT flash-style kernel - one thread per query row (q, o in registers), K/V tiles of 32
 // keys staged in shared memory and read as warp-wide broadcasts.  Attention is ~0.5 % of the path's
-// FLOPs; the tensor-core version is a later optimisation (DESIGN.md).
+// FLOPs; the tensor-core version is attention_umma.cu.
 #include <atomic>
 #include <vector>
 

@@ -1,27 +1,20 @@
-// Non-causal multi-head self-attention on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), head_dim 64 / 128, with the library's
+// Non-causal multi-head self-attention on the Hopper tensor cores (wgmma + TMA + mbarrier), head_dim 64 / 128, with the library's
 // two precision policies: single-pass fp16 operands, or the fp16 hi + lo split (3 tensor-core passes, fp32-grade) for both
 // contractions.  Callers: the LSTM-transformers of the codecs (HCodec-2.0/vq/encoder_modules/transformer.py:134-215), the SSL front
-// ends, and the 96 mimi transformer layers of H-Codec-1.5 (HCodec-1.5/adaptive/model_blocks/mimi/transformer.py:377-424), where the
-// fp32 SIMT kernel of attention.cu was 54 % of the step (profiles/r02_h15_launches.md).
+// ends, and the 96 mimi transformer layers of H-Codec-1.5 (HCodec-1.5/adaptive/model_blocks/mimi/transformer.py:377-424).
 //
 // Two launches:
 //  1. fa5_prep_kernel: qkv fp32 [B*L, 3*H*D] (the in_proj GEMM's output) -> RoPE (rotate-half tables) + 1/sqrt(D) on q -> fp16 hi (+ lo)
 //     planes in the operand layouts the MMAs want, all K-major:  Q [plane*B*H + bh][L][D],  K likewise,  V TRANSPOSED [..][D][Lp]
 //     (P.V contracts over keys, so V is the B operand [N = D rows] x [K = keys]).
-//  2. fa5_kernel: one CTA = 128 queries of one (batch, head).  warp 0 lane 0 = TMA producer, warp 1 lane 0 = MMA issuer, warps 2-5 =
-//     softmax (thread = query row = TMEM lane).  Per 64-key tile j:
-//        S_j   = Q K_j^T            UMMA M128 N64  K=D   -> TMEM columns [(j & 1) * 64, +64)   (split: hi.hi + lo.hi + hi.lo per K step)
-//        P_j   = exp2(S_j - m)      softmax threads: tcgen05.ld, reference max, ex2.approx, fp16 hi (+ lo) written to shared memory in the
-//                                   128-byte-swizzled K-major tile layout TMA would have produced (A operand of the next MMA)
-//        O    += P_j V_j            UMMA M128 N=D  K=64  -> TMEM columns [128, 128 + D), accumulated over ALL key tiles.
-//     The reference maximum m of a row only moves when a tile exceeds it by 2^8; only then does the row's warp rescale its O lanes in
-//     TMEM (tcgen05.ld -> multiply -> tcgen05.st) before that tile's P.V is issued - in steady state the softmax threads never touch O
-//     and never wait for P.V except to reuse the single P slot.  S is double-buffered in TMEM and K in shared memory, so S_{j+1} is
-//     issued as soon as K_{j+1} has landed and runs under the softmax of tile j; the issuer polls (mbarrier.test_wait) "K_{j+1} landed" and
-//     "P_j written" and issues whichever is ready.  V has one slot (refilled under the next S / softmax).  causal = 1 skips the key tiles
-//     right of the diagonal and masks inside the diagonal ones (AR-LM prefill).
-//     Shared memory: head_dim 64 split = 113 KB exactly (two CTAs per SM); head_dim 128 split 193 KB (one).
-//     Per-tile cycle split of a softmax thread: QB_F5_PROF=1 (profiles/r02_attention_ab.md).
+//  2. fa5_kernel: one CTA = 128 queries of one (batch, head).  Warpgroup 0 (one thread) = TMA producer: Q once, K and V tiles of 64
+//     keys double-buffered.  Warpgroups 1 and 2 each own 64 query rows.  Per key tile j:
+//        S_j   = Q K_j^T            wgmma m64n64k16 from shared memory into registers (split: hi.hi + lo.hi + hi.lo per K step)
+//        P_j   = exp2(S_j - m)      in registers, fp16 hi (+ lo) packed directly into the A-operand fragments of the next MMA
+//        O    += P_j V_j            wgmma m64nDk16 with A from registers, accumulated in registers over ALL key tiles.
+//     The reference maximum m of a row only moves when a tile exceeds it by 2^8 (P stays < 2^8: exact in fp16 hi + lo); only then are
+//     that row's O accumulators and running sum rescaled.  causal = 1 skips the key tiles right of the diagonal and masks inside the
+//     diagonal ones (AR-LM prefill).  Shared memory: head_dim 128 split = 192 KB, one CTA per SM.
 #include <atomic>
 #include <cstdio>
 #include <cstdlib>
@@ -29,40 +22,19 @@
 
 #include "common.cuh"
 #include "quark_b200.h"
+#include "wgmma.cuh"
 
 namespace qb {
 extern std::atomic<long long> g_launches;
 
-constexpr int F5_BQ = 128, F5_BK = 64, F5_THREADS = 192;
+constexpr int F5_BQ = 128, F5_BK = 64, F5_THREADS = 3 * 128;
 constexpr float F5_RESCALE_LOG2 = 8.0f;      // the running reference max moves only when a tile exceeds it by 2^8 (P stays < 2^8: exact in fp16 hi + lo)
 
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]),
-        "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]),
-        "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-// non-blocking probe of an mbarrier phase (mbarrier.try_wait may suspend the thread for a while: wrong for polling two conditions)
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  return ok != 0;
-}
 __device__ __forceinline__ float f5_ex2(float x) {        // ex2.approx: 2^-22 relative, one MUFU instruction (exp2f adds a denormal-range fix-up)
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------- prep
 // grid (ceil(L / 32), H, B), 256 threads.  q16 / k16: [(plane * BH + bh) * L + t] * D + d;  vT: [(plane * BH + bh) * D + d] * Lp + t.
@@ -114,265 +86,191 @@ template <int D, bool SPLIT>
 struct F5Cfg {
   static constexpr int NPL = SPLIT ? 2 : 1, KBQ = D / 64;
   static constexpr uint32_t Q_KB = F5_BQ * 128, K_KB = F5_BK * 128;          // bytes of one 64-wide K-block of Q / of K
-  static constexpr uint32_t Q_PLANE = KBQ * Q_KB, K_PLANE = KBQ * K_KB, V_PLANE = D * 128, P_PLANE = F5_BQ * 128;
-  static constexpr uint32_t K_SLOT = NPL * K_PLANE;                            // K is double-buffered: S_{j+1} never waits for a TMA round trip
-  static constexpr uint32_t OFF_Q = 0, OFF_K = OFF_Q + NPL * Q_PLANE, OFF_V = OFF_K + 2 * K_SLOT, OFF_P = OFF_V + NPL * V_PLANE;
-  static constexpr uint32_t OFF_BAR = OFF_P + NPL * P_PLANE;
-  static constexpr uint32_t SMEM = OFF_BAR + 128 + 896;                       // + barriers + slack for a 128-byte-aligned base (head_dim 64 split:
-                                                                              // exactly 113 KB, so that two CTAs fit an SM)
-  static constexpr uint32_t TCOLS = 256;                                      // S double-buffered: 2 x 64 columns; O: D columns at 128
-  static constexpr int MIN_CTAS = SMEM <= 113 * 1024 ? 2 : 1;
+  static constexpr uint32_t Q_PLANE = KBQ * Q_KB, K_PLANE = KBQ * K_KB, V_PLANE = D * 128;
+  static constexpr uint32_t K_SLOT = NPL * K_PLANE, V_SLOT = NPL * V_PLANE;   // K and V double-buffered
+  static constexpr uint32_t OFF_Q = 0, OFF_K = OFF_Q + NPL * Q_PLANE, OFF_V = OFF_K + 2 * K_SLOT;
+  static constexpr uint32_t OFF_BAR = OFF_V + 2 * V_SLOT;
+  static constexpr uint32_t SMEM = OFF_BAR + 128 + 1024;                      // + barriers + slack for a 1024-byte-aligned base
+  static_assert(SMEM <= 227 * 1024, "attention tile exceeds the 227 KB of shared memory a block may use");
 };
 
 template <int D, bool SPLIT>
-__global__ void __launch_bounds__(F5_THREADS, F5Cfg<D, SPLIT>::MIN_CTAS)
+__global__ void __launch_bounds__(F5_THREADS, 1)
 fa5_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-           int L, int H, int BH, int causal, __half* __restrict__ out_hi, __half* __restrict__ out_lo, long long* prof) {
+           int L, int H, int BH, int causal, __half* __restrict__ out_hi, __half* __restrict__ out_lo) {
   using C = F5Cfg<D, SPLIT>;
   constexpr int NPL = C::NPL, KBQ = C::KBQ;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = (uint64_t*)(smem + C::OFF_BAR);
-  uint64_t *q_full = bars, *k_full = bars + 1 /* [2] */, *k_empty = bars + 3 /* [2] */, *v_full = bars + 5, *v_empty = bars + 6,
-           *s_full = bars + 7 /* [2] */, *p_full = bars + 9, *o_full = bars + 10;
-  uint32_t* tmem_slot = (uint32_t*)(bars + 11);
-  if ((smem_u32(smem) & 1023u) != 0 || smem + C::OFF_BAR + 128 > smem_raw + C::SMEM) __trap();      // layout assumption violated
+  uint64_t *q_full = bars, *k_full = bars + 1 /* [2] */, *k_empty = bars + 3 /* [2] */, *v_full = bars + 5 /* [2] */,
+           *v_empty = bars + 7 /* [2] */;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   const int q0 = blockIdx.x * F5_BQ, h = blockIdx.y, b = blockIdx.z;
   const int bh = b * H + h;
   // causal: query t sees keys <= t, so a query tile stops at the key tile that holds its last row
   const int n_tiles = causal ? min((L + F5_BK - 1) / F5_BK, (min(q0 + F5_BQ, L) + F5_BK - 1) / F5_BK) : (L + F5_BK - 1) / F5_BK;
 
   if (threadIdx.x == 0) {
-    mbar_init(q_full, 1); mbar_init(k_full, 1); mbar_init(k_full + 1, 1); mbar_init(k_empty, 1); mbar_init(k_empty + 1, 1);
-    mbar_init(v_full, 1); mbar_init(v_empty, 1);
-    mbar_init(s_full, 1); mbar_init(s_full + 1, 1); mbar_init(p_full, 4); mbar_init(o_full, 1);
+    mbar_init(q_full, 1);
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(k_full + s, 1); mbar_init(k_empty + s, 8); mbar_init(v_full + s, 1); mbar_init(v_empty + s, 8);
+    }
     fence_mbar_init();
+    prefetch_tmap(&tmQ); prefetch_tmap(&tmK); prefetch_tmap(&tmV);
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, C::TCOLS); tmem_relinquish(); }
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tmQ); prefetch_tmap(&tmK); prefetch_tmap(&tmV); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base, tmem_O = tmem_base + 128;       // S_j in columns [(j & 1) * 64, +64)
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(q_full, NPL * C::Q_PLANE);
       for (int pl = 0; pl < NPL; ++pl)
         for (int kb = 0; kb < KBQ; ++kb)
           tma_load_3d(smem + C::OFF_Q + pl * C::Q_PLANE + kb * C::Q_KB, &tmQ, q_full, kb * 64, q0, pl * BH + bh);
-      auto load_k = [&](int i) {             // K_i into slot i & 1 (free once S_{i-2} has completed)
-        const int sl = i & 1;
-        if (i >= 2) mbar_wait(k_empty + sl, ((i >> 1) - 1) & 1);
+      for (int j = 0; j < n_tiles; ++j) {
+        const int sl = j & 1;                     // slot sl is free once both consumer warpgroups are done with tile j - 2
+        if (j >= 2) mbar_wait(k_empty + sl, ((j >> 1) - 1) & 1);
         mbar_arrive_expect_tx(k_full + sl, C::K_SLOT);
         for (int pl = 0; pl < NPL; ++pl)
           for (int kb = 0; kb < KBQ; ++kb)
-            tma_load_3d(smem + C::OFF_K + sl * C::K_SLOT + pl * C::K_PLANE + kb * C::K_KB, &tmK, k_full + sl, kb * 64, i * F5_BK, pl * BH + bh);
-      };
-      load_k(0);
-      if (n_tiles > 1) load_k(1);
-      for (int j = 0; j < n_tiles; ++j) {
-        if (j > 0) mbar_wait(v_empty, (j - 1) & 1);
-        mbar_arrive_expect_tx(v_full, NPL * C::V_PLANE);
-        for (int pl = 0; pl < NPL; ++pl) tma_load_3d(smem + C::OFF_V + pl * C::V_PLANE, &tmV, v_full, j * F5_BK, 0, pl * BH + bh);
-        if (j + 2 < n_tiles) load_k(j + 2);
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_f16(F5_BQ, F5_BK), idesc_o = make_idesc_f16(F5_BQ, D);
-      const uint32_t sQ = smem_u32(smem + C::OFF_Q), sK = smem_u32(smem + C::OFF_K), sV = smem_u32(smem + C::OFF_V),
-                     sP = smem_u32(smem + C::OFF_P);
-      // Split mode issues the three terms of one K step back to back (hi.hi, lo.hi, hi.lo): consecutive MMAs then share an operand
-      // (B, then A), which the pair GEMM measured as 0.9 instead of 0.7 of the tensor peak (profiles/r02_gemm_issue_analysis.md).
-      auto issue_s = [&](int j) {          // K_j has landed (caller checked k_full)
-        tc_fence_after();
-        const uint32_t kbase = sK + (j & 1) * C::K_SLOT, d = tmem_S + (j & 1) * 64;
-        uint32_t acc = 0;
-#pragma unroll
-        for (int kb = 0; kb < KBQ; ++kb)
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint32_t qo = kb * C::Q_KB + k * 32, ko = kb * C::K_KB + k * 32;
-            umma_f16(d, make_sw128_kmajor_desc(sQ + qo), make_sw128_kmajor_desc(kbase + ko), idesc_s, acc);
-            if (SPLIT) {
-              umma_f16(d, make_sw128_kmajor_desc(sQ + C::Q_PLANE + qo), make_sw128_kmajor_desc(kbase + ko), idesc_s, 1u);
-              umma_f16(d, make_sw128_kmajor_desc(sQ + qo), make_sw128_kmajor_desc(kbase + C::K_PLANE + ko), idesc_s, 1u);
-            }
-            acc = 1;
-          }
-        umma_commit(k_empty + (j & 1));
-        umma_commit(s_full + (j & 1));
-      };
-      auto issue_pv = [&](int j) {         // P_j is in shared memory and V_j has landed; O accumulates over the key tiles in TMEM
-        tc_fence_after();
-        uint32_t acc = j > 0 ? 1u : 0u;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          umma_f16(tmem_O, make_sw128_kmajor_desc(sP + k * 32), make_sw128_kmajor_desc(sV + k * 32), idesc_o, acc);
-          if (SPLIT) {
-            umma_f16(tmem_O, make_sw128_kmajor_desc(sP + C::P_PLANE + k * 32), make_sw128_kmajor_desc(sV + k * 32), idesc_o, 1u);
-            umma_f16(tmem_O, make_sw128_kmajor_desc(sP + k * 32), make_sw128_kmajor_desc(sV + C::V_PLANE + k * 32), idesc_o, 1u);
-          }
-          acc = 1;
-        }
-        umma_commit(v_empty);
-        umma_commit(o_full);
-      };
-      mbar_wait(q_full, 0);
-      // Whichever is ready goes next: S_{i} into S buffer i & 1 (free once the softmax threads signalled p_full(i - 2), i.e. pv >= i - 1)
-      // as soon as K_i has landed - it then runs under the softmax of tile i - 1 - or P.V_j once P_j and V_j are there.
-      int si = 0, pv = 0;
-      unsigned spins = 0;
-      while (pv < n_tiles) {
-        if (++spins > (1u << 26)) __trap();      // a mis-programmed pipeline traps instead of hanging the GPU box (cf. mbar_wait)
-        if (si < n_tiles && si <= pv + 1 && mbar_test(k_full + (si & 1), (si >> 1) & 1)) { issue_s(si); ++si; spins = 0; }
-        if (pv < si && mbar_test(p_full, pv & 1) && mbar_test(v_full, pv & 1)) { issue_pv(pv); ++pv; spins = 0; }
+            tma_load_3d(smem + C::OFF_K + sl * C::K_SLOT + pl * C::K_PLANE + kb * C::K_KB, &tmK, k_full + sl, kb * 64, j * F5_BK, pl * BH + bh);
+        if (j >= 2) mbar_wait(v_empty + sl, ((j >> 1) - 1) & 1);
+        mbar_arrive_expect_tx(v_full + sl, C::V_SLOT);
+        for (int pl = 0; pl < NPL; ++pl)
+          tma_load_3d(smem + C::OFF_V + sl * C::V_SLOT + pl * C::V_PLANE, &tmV, v_full + sl, j * F5_BK, 0, pl * BH + bh);
       }
     }
   } else {
-    // ===================== softmax (thread = query row = TMEM lane) =====================
-    // O accumulates in TMEM across the key tiles.  P is taken relative to a reference maximum m that only moves when a tile exceeds it by
-    // more than 2^8: then the warp rescales its O rows in TMEM (tcgen05.ld -> multiply -> tcgen05.st) before P.V of that tile is issued.
-    // On a typical row that happens on the first one or two tiles; afterwards the softmax threads never touch O until the end, and the
-    // P.V MMAs run under the next tile's exp2 work.
-    const int quad = warp & 3, r = quad * 32 + lane;
-    const int kmax = causal ? min(L, q0 + r + 1) : L;          // keys [0, kmax) are visible to this row
-    const uint32_t lane_addr = (uint32_t)(quad * 32) << 16;
+    // ===================== consumers: warpgroup cw owns query rows [cw * 64, +64) of the tile =====================
+    // Thread layout of the wgmma accumulators: rows ra = 16 * (warp % 4) + lane / 4 and rb = ra + 8, columns 8j + 2 (lane % 4) + {0, 1};
+    // a row's 64 keys are spread over 4 lanes.  P is taken relative to a reference maximum m that only moves when a tile exceeds it
+    // by more than 2^8; then that row's O accumulators and running sum are rescaled in registers.
+    const int cw = wg - 1, wq = warp & 3, quad = lane & 3;
+    const int ra = cw * 64 + wq * 16 + (lane >> 2), tqa = q0 + ra, tqb = tqa + 8;
+    const int kmax_a = causal ? min(L, tqa + 1) : L, kmax_b = causal ? min(L, tqb + 1) : L;
     constexpr float LOG2E = 1.4426950408889634f;
-    float m = -INFINITY, l = 0.f;                              // m in log2 units (score * log2 e)
-    uint8_t* prow = smem + C::OFF_P + (r >> 3) * 1024 + (r & 7) * 128;
-    const bool pr = prof != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && r == 0;
-    long long pc[5] = {0, 0, 0, 0, 0}, t0 = pr ? clock64() : 0;
+    const uint32_t sQ = smem_u32(smem + C::OFF_Q) + cw * 64 * 128;
+    float o[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+    float m_a = -INFINITY, m_b = -INFINITY, l_a = 0.f, l_b = 0.f;   // m in log2 units (score * log2 e); l: this lane's partial sums
+    mbar_wait(q_full, 0);
     for (int j = 0; j < n_tiles; ++j) {
-      const int k0 = j * F5_BK;
-      mbar_wait(s_full + (j & 1), (j >> 1) & 1);
-      tc_fence_after();
-      if (pr) { const long long t = clock64(); pc[0] += t - t0; t0 = t; }
-      const uint32_t sa = tmem_S + (j & 1) * 64 + lane_addr;
-      float mx = -INFINITY;
-      {
-        uint32_t v0[32], v1[32];              // pass 1: row maximum (both loads in flight, one wait; the values are re-read below)
-        tmem_ld_32x32b_x32(sa, v0);
-        tmem_ld_32x32b_x32(sa + 32, v1);
-        tmem_ld_wait();
+      const int sl = j & 1, k0 = j * F5_BK;
+      const uint32_t par = (j >> 1) & 1;
+      const uint32_t sK = smem_u32(smem + C::OFF_K + sl * C::K_SLOT), sV = smem_u32(smem + C::OFF_V + sl * C::V_SLOT);
+      // S_j = Q K_j^T; split mode issues the three terms of one K step back to back (hi.hi, lo.hi, hi.lo)
+      float s[F5_BK / 2];
+      mbar_wait(k_full + sl, par);
+      wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          if (k0 + c < kmax) mx = fmaxf(mx, __uint_as_float(v0[c]));
-          if (k0 + 32 + c < kmax) mx = fmaxf(mx, __uint_as_float(v1[c]));
+      for (int kb = 0; kb < KBQ; ++kb)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint32_t qo = kb * C::Q_KB + k * 32, ko = kb * C::K_KB + k * 32;
+          Wgmma<F5_BK>::ss(s, make_wgmma_desc_sw128(sQ + qo), make_wgmma_desc_sw128(sK + ko), (kb | k) != 0 ? 1u : 0u);
+          if (SPLIT) {
+            Wgmma<F5_BK>::ss(s, make_wgmma_desc_sw128(sQ + C::Q_PLANE + qo), make_wgmma_desc_sw128(sK + ko), 1u);
+            Wgmma<F5_BK>::ss(s, make_wgmma_desc_sw128(sQ + qo), make_wgmma_desc_sw128(sK + C::K_PLANE + ko), 1u);
+          }
         }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      if (lane == 0) mbar_arrive(k_empty + sl);
+      // row maxima over the visible keys
+      float mx_a = -INFINITY, mx_b = -INFINITY;
+#pragma unroll
+      for (int c = 0; c < F5_BK / 8; ++c)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int key = k0 + 8 * c + 2 * quad + e;
+          if (key < kmax_a) mx_a = fmaxf(mx_a, s[4 * c + e]);
+          if (key < kmax_b) mx_b = fmaxf(mx_b, s[4 * c + 2 + e]);
+        }
+#pragma unroll
+      for (int x = 1; x <= 2; x <<= 1) {
+        mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, x));
+        mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, x));
       }
-      mx *= LOG2E;
-      if (pr) { const long long t = clock64(); pc[1] += t - t0; t0 = t; }
-      bool waited_o = false;
+      mx_a *= LOG2E; mx_b *= LOG2E;
       if (j == 0) {
-        m = mx;                                  // key 0 is visible to every row: finite
+        m_a = mx_a; m_b = mx_b;                  // key 0 is visible to every row: finite
       } else {
-        const bool need = mx > m + F5_RESCALE_LOG2;
-        if (__any_sync(0xffffffffu, need)) {     // tcgen05.ld / st are warp-collective: lanes that need no rescale multiply by 1
-          mbar_wait(o_full, (j - 1) & 1);        // P.V_{j-1} has finished accumulating into O
-          tc_fence_after();
-          waited_o = true;
-          const float f = need ? f5_ex2(m - mx) : 1.f;
-          if (need) { l *= f; m = mx; }
+        const bool need_a = mx_a > m_a + F5_RESCALE_LOG2, need_b = mx_b > m_b + F5_RESCALE_LOG2;
+        if (need_a || need_b) {
+          const float fa = need_a ? f5_ex2(m_a - mx_a) : 1.f, fb = need_b ? f5_ex2(m_b - mx_b) : 1.f;
+          if (need_a) { l_a *= fa; m_a = mx_a; }
+          if (need_b) { l_b *= fb; m_b = mx_b; }
 #pragma unroll
-          for (int c0 = 0; c0 < D; c0 += 32) {
-            uint32_t o[32];
-            tmem_ld_32x32b_x32(tmem_O + lane_addr + c0, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int c = 0; c < 32; ++c) o[c] = __float_as_uint(__uint_as_float(o[c]) * f);
-            tmem_st_32x32b_x32(tmem_O + lane_addr + c0, o);
-          }
-          tmem_st_wait();
+          for (int c = 0; c < D / 8; ++c) { o[4 * c] *= fa; o[4 * c + 1] *= fa; o[4 * c + 2] *= fb; o[4 * c + 3] *= fb; }
         }
       }
-      if (pr) { const long long t = clock64(); pc[2] += t - t0; t0 = t; }
-      // P = exp2(S * log2e - m) as fp16 hi (+ lo), packed in registers while P.V_{j-1} is still reading the P slot
-      float rs = 0.f;
-      const bool full = k0 + F5_BK <= kmax;        // no masked key in this tile for this row (all but the last / the diagonal tiles)
-      uint32_t ph[F5_BK / 2], pl[SPLIT ? F5_BK / 2 : 1];
+      // P = exp2(S * log2e - m) as fp16 hi (+ lo), packed as the register A operand of P.V (m16n8k16 A-fragment layout)
+      const bool full = k0 + F5_BK <= min(kmax_a, kmax_b);      // no masked key in this tile for either row
+      uint32_t ph[F5_BK / 16][4], plo[SPLIT ? F5_BK / 16 : 1][4];
 #pragma unroll
-      for (int c0 = 0; c0 < F5_BK; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(sa + c0, v);
-        tmem_ld_wait();
+      for (int c = 0; c < F5_BK / 8; ++c)
 #pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const int c = 2 * e;
-          float p0 = f5_ex2(fmaf(__uint_as_float(v[c]), LOG2E, -m)), p1 = f5_ex2(fmaf(__uint_as_float(v[c + 1]), LOG2E, -m));
+        for (int rr = 0; rr < 2; ++rr) {
+          const int key = k0 + 8 * c + 2 * quad;
+          const float mr = rr ? m_b : m_a;
+          const int km = rr ? kmax_b : kmax_a;
+          float p0 = f5_ex2(fmaf(s[4 * c + 2 * rr], LOG2E, -mr)), p1 = f5_ex2(fmaf(s[4 * c + 2 * rr + 1], LOG2E, -mr));
           if (!full) {
-            p0 = (k0 + c0 + c < kmax) ? p0 : 0.f;
-            p1 = (k0 + c0 + c + 1 < kmax) ? p1 : 0.f;
+            p0 = key < km ? p0 : 0.f;
+            p1 = key + 1 < km ? p1 : 0.f;
           }
-          rs += p0 + p1;
+          if (rr) l_b += p0 + p1; else l_a += p0 + p1;
           const __half2 hh = __floats2half2_rn(p0, p1);
-          ph[c0 / 2 + e] = *reinterpret_cast<const uint32_t*>(&hh);
+          ph[c >> 1][(c & 1) * 2 + rr] = *reinterpret_cast<const uint32_t*>(&hh);
           if (SPLIT) {
             const float2 back = __half22float2(hh);
             const __half2 ll = __floats2half2_rn(p0 - back.x, p1 - back.y);
-            pl[c0 / 2 + e] = *reinterpret_cast<const uint32_t*>(&ll);
+            plo[c >> 1][(c & 1) * 2 + rr] = *reinterpret_cast<const uint32_t*>(&ll);
           }
         }
-      }
-      // the P slot is free once P.V_{j-1} has read it
-      if (j > 0 && !waited_o) mbar_wait(o_full, (j - 1) & 1);
-      if (pr) { const long long t = clock64(); pc[3] += t - t0; t0 = t; }
+      // O += P_j V_j (V^T tile: D rows x 64 keys, K-major)
+      mbar_wait(v_full + sl, par);
+      wgmma_fence();
 #pragma unroll
-      for (int cc = 0; cc < F5_BK / 8; ++cc) {     // 16-byte chunk cc of row r sits at cc ^ (r % 8) (128-byte swizzle)
-        uint8_t* dst = prow + ((cc ^ (r & 7)) << 4);
-        *reinterpret_cast<uint4*>(dst) = make_uint4(ph[4 * cc], ph[4 * cc + 1], ph[4 * cc + 2], ph[4 * cc + 3]);
-        if (SPLIT) *reinterpret_cast<uint4*>(dst + C::P_PLANE) = make_uint4(pl[4 * cc], pl[4 * cc + 1], pl[4 * cc + 2], pl[4 * cc + 3]);
+      for (int k = 0; k < F5_BK / 16; ++k) {
+        Wgmma<D>::rs(o, ph[k], make_wgmma_desc_sw128(sV + k * 32));
+        if (SPLIT) {
+          Wgmma<D>::rs(o, plo[k], make_wgmma_desc_sw128(sV + k * 32));
+          Wgmma<D>::rs(o, ph[k], make_wgmma_desc_sw128(sV + C::V_PLANE + k * 32));
+        }
       }
-      l += rs;
-      tc_fence_before();
-      fence_proxy_async();                       // generic-proxy stores of P -> visible to the tensor core's async proxy
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);        // one arrival per softmax warp
-      if (pr) { const long long t = clock64(); pc[4] += t - t0; t0 = t; }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(o);
+      if (lane == 0) mbar_arrive(v_empty + sl);
     }
-    if (pr) { for (int i = 0; i < 5; ++i) prof[i] = pc[i]; prof[5] = n_tiles; }
-    mbar_wait(o_full, (n_tiles - 1) & 1);
-    tc_fence_after();
-    const int tq = q0 + r;
-    const float inv = 1.f / l;
-    const long long ob = ((long long)b * L + tq) * (long long)(H * D) + h * D;
 #pragma unroll
-    for (int c0 = 0; c0 < D; c0 += 32) {
-      uint32_t o[32];
-      tmem_ld_32x32b_x32(tmem_O + lane_addr + c0, o);
-      tmem_ld_wait();
-      if (tq < L) {
+    for (int x = 1; x <= 2; x <<= 1) {
+      l_a += __shfl_xor_sync(0xffffffffu, l_a, x);
+      l_b += __shfl_xor_sync(0xffffffffu, l_b, x);
+    }
+    const float inv_a = 1.f / l_a, inv_b = 1.f / l_b;
 #pragma unroll
-        for (int d0 = 0; d0 < 32; d0 += 8) {
-          uint32_t hi[4], lo[4];
+    for (int rr = 0; rr < 2; ++rr) {
+      const int tq = rr ? tqb : tqa;
+      if (tq >= L) continue;
+      const float inv = rr ? inv_b : inv_a;
+      const long long ob = ((long long)b * L + tq) * (long long)(H * D) + h * D + 2 * quad;
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float a = __uint_as_float(o[d0 + 2 * e]) * inv, c = __uint_as_float(o[d0 + 2 * e + 1]) * inv;
-            const __half2 hh = __floats2half2_rn(a, c);
-            hi[e] = *reinterpret_cast<const uint32_t*>(&hh);
-            const float2 back = __half22float2(hh);
-            const __half2 ll = __floats2half2_rn(a - back.x, c - back.y);
-            lo[e] = *reinterpret_cast<const uint32_t*>(&ll);
-          }
-          *reinterpret_cast<uint4*>(out_hi + ob + c0 + d0) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-          if (out_lo) *reinterpret_cast<uint4*>(out_lo + ob + c0 + d0) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+      for (int c = 0; c < D / 8; ++c) {
+        const float a = o[4 * c + 2 * rr] * inv, e = o[4 * c + 2 * rr + 1] * inv;
+        const __half2 hh = __floats2half2_rn(a, e);
+        *reinterpret_cast<__half2*>(out_hi + ob + 8 * c) = hh;
+        if (out_lo) {
+          const float2 back = __half22float2(hh);
+          *reinterpret_cast<__half2*>(out_lo + ob + 8 * c) = __floats2half2_rn(a - back.x, e - back.y);
         }
       }
     }
-    tc_fence_before();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C::TCOLS);
   }
 }
 
@@ -422,20 +320,10 @@ static int f5_launch(const float* qkv, int64_t B, int64_t L, int32_t H, const fl
   if (int e = f5_map(&tmK, k16, D, L, NPL * BH, D, 64, F5_BK)) return e;
   if (int e = f5_map(&tmV, vT, L, D, NPL * BH, Lp, F5_BK, D)) return e;
   QB_CHECK_CUDA(cudaFuncSetAttribute(fa5_kernel<D, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
-  static long long* prof = nullptr;
-  if (!prof && getenv("QB_F5_PROF")) { cudaMalloc(&prof, 64); cudaMemset(prof, 0, 64); }
   fa5_kernel<D, SPLIT><<<dim3((unsigned)ceil_div(L, F5_BQ), (unsigned)H, (unsigned)B), F5_THREADS, C::SMEM, st>>>(tmQ, tmK, tmV, (int)L, H,
-                                                                                                                (int)BH, causal, out_hi, out_lo, prof);
+                                                                                                                (int)BH, causal, out_hi, out_lo);
   g_launches++;
   QB_CHECK_CUDA(cudaGetLastError());
-  if (prof) {       // QB_F5_PROF=1: per-tile cycle split of the softmax thread of CTA (0,0,0), row 0 (synchronises)
-    long long h[8];
-    cudaStreamSynchronize(st);
-    cudaMemcpy(h, prof, 64, cudaMemcpyDeviceToHost);
-    const double n = (double)(h[5] > 0 ? h[5] : 1);
-    fprintf(stderr, "[fa5 prof D=%d split=%d L=%d] cycles / key tile (cta0 row0, %lld tiles): wait S %.0f | load S + max %.0f | rescale O (rare) %.0f | exp2 + pack + "
-                    "wait P slot %.0f | P stores + fence + arrive %.0f\n", D, (int)SPLIT, (int)L, h[5], h[0] / n, h[1] / n, h[2] / n, h[3] / n, h[4] / n);
-  }
   return 0;
 }
 }  // namespace qb

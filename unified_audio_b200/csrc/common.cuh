@@ -1,5 +1,5 @@
-// Shared device helpers for libquark_b200 (sm_100a only).
-// Raw PTX wrappers for mbarrier / TMA / tcgen05 / TMEM - no CUTLASS dependency.
+// Shared device helpers for libquark_b200 (sm_90a).
+// Raw PTX wrappers for mbarrier / TMA - no CUTLASS dependency (wgmma wrappers: wgmma.cuh).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -77,7 +77,7 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
-// ---------------------------------------------------------------- PTX: mbarrier / TMA / tcgen05
+// ---------------------------------------------------------------- PTX: mbarrier / TMA
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ bool elect_one() {
@@ -110,7 +110,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded spin: a mis-programmed pipeline traps instead of hanging the GPU box.
+// Bounded spin: a mis-programmed pipeline traps instead of hanging the GPU.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
@@ -120,8 +120,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 
 // Same wait for warps that have slack (epilogue warps waiting for their accumulator tile, producers waiting for a free stage):
 // try_wait with a suspend-time hint parks the thread in hardware until the phase completes (or the hint expires) instead of
-// spinning on the barrier - the spinning epilogue warps were 16 M issued instructions per GEMM launch (profiles/r02_gemm_issue_
-// analysis.md) on a power-capped part.
+// spinning on the barrier, so that waiting warps do not take issue slots from the ones doing the work.
 __device__ __forceinline__ void mbar_wait_parked(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   for (;;) {
@@ -152,140 +151,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, ui
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(x), "r"(y), "r"(z)
       : "memory");
-}
-
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (fp16/bf16 inputs, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- CTA-pair (cta_group::2) variants --------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same smem offset in CTA `rank` of this cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load executed by both CTAs of a pair; completion bytes are signalled on `bar_cluster_addr` (the leader's barrier)
-__device__ __forceinline__ void tma2_load_2d(void* smem_dst, const void* tmap, uint32_t bar_cluster_addr, int x, int y) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(bar_cluster_addr), "r"(x), "r"(y)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_3d(void* smem_dst, const void* tmap, uint32_t bar_cluster_addr, int x, int y, int z) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(bar_cluster_addr), "r"(x), "r"(y), "r"(z)
-      : "memory");
-}
-// multicast variants: the box lands at the same smem offset in every CTA of `mask`; each destination's completion bytes are
-// signalled on the barrier at the same offset in that destination's PAIR LEADER (peer bit 24 of the shared::cluster address
-// cleared - the CUTLASS SM100_TMA_2SM_LOAD_MULTICAST convention)
-__device__ __forceinline__ void tma2_load_2d_mc(void* smem_dst, const void* tmap, uint64_t* bar, int x, int y, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(x), "r"(y), "h"(mask)
-      : "memory");
-}
-// same address convention for a non-multicast load of a pair inside a larger cluster
-__device__ __forceinline__ void tma2_load_3d_peer(void* smem_dst, const void* tmap, uint64_t* bar, int x, int y, int z) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(x), "r"(y), "r"(z)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs, 256 x N] (+)= A[128 rows from each CTA] * B[N/2 rows from each CTA]
-__device__ __forceinline__ void umma2_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once) on the barrier at this smem offset in every CTA of `cta_mask` when the pair's MMAs complete
-__device__ __forceinline__ void umma2_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(cta_mask) : "memory");
-}
-
-// UMMA shared-memory descriptor: K-major operand, 128-byte swizzle, rows densely packed at 128 B
-// (one swizzle row = 64 fp16), 8-row groups 1024 B apart.  Field layout per the PTX ISA "matrix
-// descriptor" for tcgen05: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48),
-// layout_type [61,64) with SWIZZLE_128B = 2.
-__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;              // LBO (unused for swizzled K-major; canonical value 1)
-  d |= (uint64_t)(1024 >> 4) << 32;    // SBO = 8 rows * 128 B
-  d |= (uint64_t)1 << 46;              // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;              // SWIZZLE_128B
-  return d;
-}
-// Instruction descriptor for kind::f16: fp16 A/B (format 0), fp32 accumulate, both K-major.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-  return (1u << 4)                        // c_format = F32
-         | (0u << 7) | (0u << 10)         // a/b format = F16
-         | (0u << 15) | (0u << 16)        // K-major A and B
-         | ((uint32_t)(N >> 3) << 17)     // n_dim
-         | ((uint32_t)(M >> 4) << 24);    // m_dim
 }
 
 }  // namespace qb

@@ -511,7 +511,7 @@ using namespace qb;
 extern "C" int qb_split_f16(const float* x, qb_half* hi, qb_half* lo, int64_t n, void* stream) {
   QB_REQUIRE(x && hi && n >= 0, "split: bad args");
   if (n == 0) return 0;
-  int blocks = (int)(ceil_div(n, 256) < 148 * 16 ? ceil_div(n, 256) : 148 * 16);
+  int blocks = (int)(ceil_div(n, 256) < 132 * 16 ? ceil_div(n, 256) : 132 * 16);
   split_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, (__half*)hi, (__half*)lo, n);
   QB_LAUNCH_END();
 }
@@ -797,7 +797,7 @@ extern "C" int qb_stft_gather(const float* wav, int64_t B, int64_t T, int32_t ho
              "stft_gather: needs n_fft == P*Q, P <= 64, Q <= 64, T a multiple of hop");
   const int64_t F = T / hop;
   const long long total = B * F * Q * 64;
-  stft_gather_kernel<<<(unsigned)(ceil_div(total, 256) < 148 * 32 ? ceil_div(total, 256) : 148 * 32), 256, 0, (cudaStream_t)stream>>>(
+  stft_gather_kernel<<<(unsigned)(ceil_div(total, 256) < 132 * 32 ? ceil_div(total, 256) : 132 * 32), 256, 0, (cudaStream_t)stream>>>(
       wav, T, hop, n_fft, P, Q, (int)F, window, (__half*)hi, (__half*)lo, total);
   QB_LAUNCH_END();
 }
@@ -806,7 +806,7 @@ extern "C" int qb_stft_twiddle(const float* Y, int64_t ldY, int64_t frames_total
                                qb_half* hi, qb_half* lo, void* stream) {
   QB_REQUIRE(Y && twiddle && hi && ldY >= 2 * P && 2 * Q <= 128, "stft_twiddle: bad args");
   const long long total = frames_total * P * Q;
-  stft_twiddle_kernel<<<(unsigned)(ceil_div(total, 256) < 148 * 32 ? ceil_div(total, 256) : 148 * 32), 256, 0, (cudaStream_t)stream>>>(
+  stft_twiddle_kernel<<<(unsigned)(ceil_div(total, 256) < 132 * 32 ? ceil_div(total, 256) : 132 * 32), 256, 0, (cudaStream_t)stream>>>(
       Y, ldY, P, Q, (const float2*)twiddle, (__half*)hi, (__half*)lo, total);
   QB_LAUNCH_END();
 }

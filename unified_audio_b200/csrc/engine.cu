@@ -175,7 +175,7 @@ __global__ void planes_to_f32_kernel(const __half* __restrict__ hi, const __half
 }
 static inline unsigned grid_for(long long total) {
   long long g = (total + 255) / 256;
-  return (unsigned)(g < 1 ? 1 : (g > 148 * 32 ? 148 * 32 : g));
+  return (unsigned)(g < 1 ? 1 : (g > 132 * 32 ? 132 * 32 : g));
 }
 
 // ------------------------------------------------------------------ weights
@@ -380,7 +380,7 @@ static int load_transformer(Loader& L, const std::string& prefix, int n, int C, 
     add_vec_kernel<<<grid_for(4 * C), 256>>>(bih->data, bhh->data, 4 * C, b);
     l.b_ih = b;
     QB_TRY(L.get(&whh, a + "rnn.weight_hh_l0", 2));
-    QB_REQUIRE(lstm_u > 0, "load: LSTM width %d unsupported by the tcgen05 recurrence (needs H %% 256 == 0)", C);
+    QB_REQUIRE(lstm_u > 0, "load: LSTM width %d unsupported by the wgmma recurrence (needs H %% 256 == 0)", C);
     QB_TRY(L.arena.alloc((void**)&l.whh_perm, (size_t)4 * C * C * 2, false));
     lstm_permute_kernel<<<grid_for(4LL * C * C), 256>>>(whh->data, C, lstm_u, l.whh_perm);
     // q|k|v rows concatenated
@@ -516,7 +516,7 @@ static int run_transformer(qb_codec* c, const std::vector<TfLayerW>& layers, flo
   QB_TRY(c->ws.f32(&xp, "tf_xp", (size_t)M * 4 * C));
   QB_TRY(c->ws.f32(&qkv, "tf_qkv", (size_t)M * 3 * C));
   QB_TRY(c->ws.get(&lstm_ws, "lstm_ws", (size_t)qb_lstm_tc_workspace_bytes(B, C)));
-  // tcgen05 attention (attention_umma.cu) in both precision policies; QB_ATTENTION=legacy keeps the round-1 kernels (mma.sync flash
+  // wgmma attention (attention_umma.cu) in both precision policies; QB_ATTENTION=legacy keeps the round-1 kernels (mma.sync flash
   // attention for the single-pass policy, fp32 SIMT for the split one) for A/B runs
   static const bool legacy = [] { const char* e = getenv("QB_ATTENTION"); return e && !strcmp(e, "legacy"); }();
   const bool tc_att = legacy && !pa;
@@ -735,9 +735,10 @@ extern "C" int qb_init(int device, qb_handle** out) {
   QB_CHECK_CUDA(cudaGetDeviceCount(&n));
   QB_REQUIRE(device >= 0 && device < n, "qb_init: device %d out of range (%d visible)", device, n);
   QB_CHECK_CUDA(cudaSetDevice(device));
-  int major = 0;
+  int major = 0, minor = 0;
   QB_CHECK_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-  QB_REQUIRE(major == 10, "qb_init: libquark_b200 is built for sm_100a only (device %d is sm_%d*)", device, major);
+  QB_CHECK_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
+  QB_REQUIRE(major == 9 && minor == 0, "qb_init: libquark_b200 is built for sm_90a only (device %d is sm_%d%d)", device, major, minor);
   qb_handle* h = new qb_handle();
   h->device = device;
   *out = h;
@@ -1147,7 +1148,7 @@ static int lm_layers_prefill(qb_lm* m, float* x, int64_t B, int64_t L, qb_kv* kv
   QB_TRY(m->ws.planes(&hid, "hid", (size_t)M * I, true));
   QB_TRY(m->ws.f32(&qkv, "qkv", (size_t)M * 3 * H));
   QB_TRY(m->ws.f32(&q32, "q32", (size_t)M * H));
-  // prefill from an empty cache: causal tcgen05 attention over the qkv rows (attention_umma.cu); a continuation reads the cache
+  // prefill from an empty cache: causal wgmma attention over the qkv rows (attention_umma.cu); a continuation reads the cache
   static const bool legacy_att = [] { const char* e = getenv("QB_ATTENTION"); return e && !strcmp(e, "legacy"); }();
   const bool umma = pos0 == 0 && !legacy_att;
   void* att_ws = nullptr;

@@ -1,12 +1,12 @@
-// Dense contraction kernels: tcgen05/TMA/TMEM persistent GEMM (product path) and a SIMT
+// Dense contraction kernels: wgmma/TMA persistent GEMM (product path) and a SIMT
 // cross-check.  Both evaluate the same qb_gemm_desc (include/quark_b200.h).
 //
-// Tile: 128 (rows) x BN (cols) x 64 (K) per pipeline stage, fp16 planes K-major in shared memory
-// with the 128-byte TMA/UMMA swizzle; accumulators live in TMEM (double buffered: 2 x BN columns)
-// so the epilogue of tile i overlaps the MMAs of tile i+1.  Warp roles (576 threads):
-//   warps 0-15 epilogue   (TMEM -> registers -> bias/act/gamma/residual -> global)
-//   warp  16   TMA producer (one lane)
-//   warp  17   TMEM allocator + MMA issuer (one lane)
+// Tile: 128 (rows) x 128 (cols) x 64 (K) per pipeline stage, fp16 planes K-major in shared memory
+// with the 128-byte TMA/wgmma swizzle; accumulators live in registers.  Warp roles (384 threads):
+//   warpgroup 0     TMA producer (one thread)
+//   warpgroups 1-2  wgmma m64n128k16 on rows [0, 64) / [64, 128) of the tile, then the epilogue
+//                   (bias/act/gamma/residual -> global) straight from the accumulator registers;
+//                   the producer already fills the stages of the next tile meanwhile.
 // Convolutions are expressed as `taps` shifted K-panels over a zero-padded channel-last buffer:
 // the A tensor map views the buffer as [batch][rows/stride][stride*C], so tap t of output row m is
 // the box at (x = (t % stride)*C + c, y = m + t / stride) - TMA-staged im2col without an im2col
@@ -19,6 +19,7 @@
 
 #include "common.cuh"
 #include "quark_b200.h"
+#include "wgmma.cuh"
 
 namespace qb {
 
@@ -105,199 +106,92 @@ __device__ __forceinline__ void epi_finish_scalar(const GemmParams& p, int b, in
   }
 }
 
-// Epilogue for 32 consecutive accumulator columns [n_base, n_base+32) of output row (b, m).
-__device__ __forceinline__ void epilogue_row32(const GemmParams& p, int b, int m, int n_base, const uint32_t (&r)[32]) {
-  if (m >= p.m_per_batch || n_base >= p.N) return;
-  float v[32];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-  if (p.bias) {
-    if (n_base + 32 <= p.N && ((reinterpret_cast<uintptr_t>(p.bias) & 15) == 0)) {
-      const float4* bp = reinterpret_cast<const float4*>(p.bias + n_base);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 t = __ldg(bp + j);
-        v[4 * j] += t.x; v[4 * j + 1] += t.y; v[4 * j + 2] += t.z; v[4 * j + 3] += t.w;
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (n_base + j < p.N) v[j] += __ldg(p.bias + n_base + j);
-    }
-  }
-  // ---- specialised tight paths (no per-element predicates) for the two epilogues that carry >90 % of the
-  //      single-pass GEMM work: ConvNeXt pwconv1 (bias + GELU -> fp16 hi plane) and pwconv2 (bias, gamma,
-  //      + residual -> fp32).  Everything else takes the generic path below.
-  if (n_base + 32 <= p.N && p.act2 == QB_ACT_NONE && (p.act == QB_ACT_NONE || p.act == QB_ACT_GELU)) {
-    if (p.ohi.ptr && !p.olo.ptr && !p.o32.ptr && !p.res.ptr && !p.gamma && (p.ohi.ld & 7) == 0) {
-      if (p.act == QB_ACT_GELU) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = gelu_fast(v[j]);
-      }
-      uint4* hp = (uint4*)((__half*)p.ohi.ptr + ((long long)b * p.ohi.rpb + p.ohi.off + m) * p.ohi.ld + n_base);
-      const __half2 hmax = __float2half2_rn(65504.f), hmin = __float2half2_rn(-65504.f);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        __half2 h2[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-          h2[e] = __hmax2(__hmin2(__floats2half2_rn(v[8 * j + 2 * e], v[8 * j + 2 * e + 1]), hmax), hmin);
-        hp[j] = *reinterpret_cast<uint4*>(h2);
-      }
-      return;
-    }
-    if (p.o32.ptr && !p.ohi.ptr && (p.o32.ld & 3) == 0 && (!p.res.ptr || (p.res.ld & 3) == 0) && p.act == QB_ACT_NONE &&
-        (!p.gamma || (reinterpret_cast<uintptr_t>(p.gamma) & 15) == 0)) {
-      if (p.gamma) {
-        const float4* gp = reinterpret_cast<const float4*>(p.gamma + n_base);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 t = __ldg(gp + j);
-          v[4 * j] *= t.x; v[4 * j + 1] *= t.y; v[4 * j + 2] *= t.z; v[4 * j + 3] *= t.w;
-        }
-      }
-      if (p.res.ptr) {
-        const float4* rp = (const float4*)((const float*)p.res.ptr + ((long long)b * p.res.rpb + p.res.off + m) * p.res.ld + n_base);
-        float4 t[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) t[j] = rp[j];          // all 8 loads in flight before the adds
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { v[4 * j] += t[j].x; v[4 * j + 1] += t[j].y; v[4 * j + 2] += t[j].z; v[4 * j + 3] += t[j].w; }
-      }
-      float4* op = (float4*)((float*)p.o32.ptr + ((long long)b * p.o32.rpb + p.o32.off + m) * p.o32.ld + n_base);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) op[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-      return;
-    }
-  }
-  int ncols = 32, n_out = n_base, N_out = p.N;
-  if (p.act == QB_ACT_SWIGLU) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v[j] = silu_f(v[2 * j]) * v[2 * j + 1];
-    ncols = 16;
-    n_out = n_base >> 1;
-    N_out = p.N >> 1;
-  } else if (p.act == QB_ACT_SNAKE) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (n_base + j < p.N) v[j] = snake_f(v[j], __ldg(p.act_p + n_base + j));
-  } else if (p.act != QB_ACT_NONE) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = apply_act(p.act, v[j]);
-  }
-  const bool full = (n_out + ncols <= N_out);
-  const bool vec32 = full && (!p.res.ptr || (p.res.ld & 3) == 0) && (!p.o32.ptr || (p.o32.ld & 3) == 0) &&
-                     (!p.ohi.ptr || (p.ohi.ld & 7) == 0);
-  if (!vec32) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (j < ncols && n_out + j < N_out) epi_finish_scalar(p, b, m, n_out + j, v[j]);
-    return;
-  }
-  if (p.gamma) {
-    if ((reinterpret_cast<uintptr_t>(p.gamma) & 15) == 0) {
-      const float4* gp = reinterpret_cast<const float4*>(p.gamma + n_out);
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        if (4 * j < ncols) {
-          const float4 t = __ldg(gp + j);
-          v[4 * j] *= t.x; v[4 * j + 1] *= t.y; v[4 * j + 2] *= t.z; v[4 * j + 3] *= t.w;
-        }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (j < ncols) v[j] *= __ldg(p.gamma + n_out + j);
-    }
-  }
-  if (p.res.ptr) {
-    const float4* rp = (const float4*)((const float*)p.res.ptr + ((long long)b * p.res.rpb + p.res.off + m) * p.res.ld + n_out);
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      if (4 * j < ncols) {
-        float4 t = rp[j];
-        v[4 * j] += t.x; v[4 * j + 1] += t.y; v[4 * j + 2] += t.z; v[4 * j + 3] += t.w;
-      }
-  }
-  if (p.o32.ptr) {
-    float4* op = (float4*)((float*)p.o32.ptr + ((long long)b * p.o32.rpb + p.o32.off + m) * p.o32.ld + n_out);
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      if (4 * j < ncols) op[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-  }
-  if (p.ohi.ptr) {
-    long long o = ((long long)b * p.ohi.rpb + p.ohi.off + m) * p.ohi.ld + n_out;
-    uint4* hp = (uint4*)((__half*)p.ohi.ptr + o);
-    uint4* lp = p.olo.ptr ? (uint4*)((__half*)p.olo.ptr + o) : nullptr;
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      if (8 * j < ncols) {
-        __half2 h2[4], l2[4];
-        const __half2 hmax = __float2half2_rn(65504.f), hmin = __float2half2_rn(-65504.f);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          float u0 = v[8 * j + 2 * e], u1 = v[8 * j + 2 * e + 1];
-          if (p.act2 == QB_ACT_ELU) { u0 = elu_f(u0); u1 = elu_f(u1); }
-          if (p.act2 == QB_ACT_SNAKE) {
-            const float2 al = __ldg(reinterpret_cast<const float2*>(p.act2_p + n_out + 8 * j + 2 * e));
-            u0 = snake_f(u0, al.x); u1 = snake_f(u1, al.y);
-          }
-          const __half2 hh = __hmax2(__hmin2(__floats2half2_rn(u0, u1), hmax), hmin);   // saturate, no inf
-          h2[e] = hh;
-          if (lp) {
-            const float2 back = __half22float2(hh);
-            l2[e] = __floats2half2_rn(u0 - back.x, u1 - back.y);
-          }
-        }
-        hp[j] = *reinterpret_cast<uint4*>(h2);
-        if (lp) lp[j] = *reinterpret_cast<uint4*>(l2);
-      }
-  }
-}
-
 __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
   return (uint8_t*)(((uintptr_t)p + 1023) & ~(uintptr_t)1023);
 }
 
-constexpr int GEMM_EPI_WARPS = 16, GEMM_THREADS = (GEMM_EPI_WARPS + 2) * 32;
+// Epilogue for the accumulator pair (row m, columns n, n + 1) a thread holds after the warpgroup MMA.
+__device__ __forceinline__ void epilogue_pair(const GemmParams& p, int b, int m, int n, float v0, float v1) {
+  if (m >= p.m_per_batch || n >= p.N) return;
+  const bool has1 = n + 1 < p.N;
+  if (p.bias) {
+    v0 += __ldg(p.bias + n);
+    if (has1) v1 += __ldg(p.bias + n + 1);
+  }
+  if (p.act == QB_ACT_SWIGLU) {                // interleaved gate / up columns -> one output column n / 2 (n is even, N even)
+    epi_finish_scalar(p, b, m, n >> 1, silu_f(v0) * v1);
+    return;
+  }
+  // vectorised paths for the two epilogues that carry most of the single-pass GEMM work: ConvNeXt pwconv1 (bias + GELU -> fp16
+  // hi plane) and pwconv2 (bias, gamma, + residual -> fp32); n is even, so a pair is one aligned half2 / float2 when the row
+  // pitches are even and the bases 8-byte aligned
+  if (has1 && p.act2 == QB_ACT_NONE && (p.act == QB_ACT_NONE || p.act == QB_ACT_GELU)) {
+    if (p.ohi.ptr && !p.olo.ptr && !p.o32.ptr && !p.res.ptr && !p.gamma && (p.ohi.ld & 1) == 0 &&
+        (reinterpret_cast<uintptr_t>(p.ohi.ptr) & 3) == 0) {
+      if (p.act == QB_ACT_GELU) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
+      const __half2 hmax = __float2half2_rn(65504.f), hmin = __float2half2_rn(-65504.f);
+      *reinterpret_cast<__half2*>((__half*)p.ohi.ptr + ((long long)b * p.ohi.rpb + p.ohi.off + m) * p.ohi.ld + n) =
+          __hmax2(__hmin2(__floats2half2_rn(v0, v1), hmax), hmin);
+      return;
+    }
+    if (p.o32.ptr && !p.ohi.ptr && p.act == QB_ACT_NONE && (p.o32.ld & 1) == 0 && (reinterpret_cast<uintptr_t>(p.o32.ptr) & 7) == 0 &&
+        (!p.res.ptr || ((p.res.ld & 1) == 0 && (reinterpret_cast<uintptr_t>(p.res.ptr) & 7) == 0)) &&
+        (!p.gamma || (reinterpret_cast<uintptr_t>(p.gamma) & 7) == 0)) {
+      if (p.gamma) {
+        const float2 g = __ldg(reinterpret_cast<const float2*>(p.gamma + n));
+        v0 *= g.x; v1 *= g.y;
+      }
+      if (p.res.ptr) {
+        const float2 r = *reinterpret_cast<const float2*>((const float*)p.res.ptr + ((long long)b * p.res.rpb + p.res.off + m) * p.res.ld + n);
+        v0 += r.x; v1 += r.y;
+      }
+      *reinterpret_cast<float2*>((float*)p.o32.ptr + ((long long)b * p.o32.rpb + p.o32.off + m) * p.o32.ld + n) = make_float2(v0, v1);
+      return;
+    }
+  }
+  if (p.act == QB_ACT_SNAKE) {
+    v0 = snake_f(v0, __ldg(p.act_p + n));
+    if (has1) v1 = snake_f(v1, __ldg(p.act_p + n + 1));
+  } else if (p.act != QB_ACT_NONE) {
+    v0 = apply_act(p.act, v0);
+    v1 = apply_act(p.act, v1);
+  }
+  epi_finish_scalar(p, b, m, n, v0);
+  if (has1) epi_finish_scalar(p, b, m, n + 1, v1);
+}
 
-template <int BN, int NTERMS, int STAGES>
+constexpr int GEMM_BM = 128, GEMM_BN = 128, GEMM_BK = 64;
+constexpr int GEMM_THREADS = 3 * 128;           // warpgroup 0: TMA producer; warpgroups 1-2: MMA + epilogue, 64 rows each
+
+template <int NTERMS, int STAGES>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
                const GemmParams p) {
-  constexpr int BM = 128, BK = 64;
+  constexpr int BM = GEMM_BM, BN = GEMM_BN, BK = GEMM_BK;
   constexpr int NPL = (NTERMS == 1) ? 1 : 2;
   constexpr uint32_t A_BYTES = BM * BK * 2, W_BYTES = BN * BK * 2;
   constexpr uint32_t STAGE_BYTES = NPL * (A_BYTES + W_BYTES);
-  constexpr uint32_t TMEM_COLS = 2 * BN;
-  static_assert(TMEM_COLS == 256 || TMEM_COLS == 512, "TMEM columns must be a power of two <= 512");
+  constexpr int CONSUMER_WARPS = 8;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   uint64_t* full = (uint64_t*)(smem + STAGES * STAGE_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = (uint32_t*)(tempty + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], GEMM_EPI_WARPS); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], CONSUMER_WARPS); }
     fence_mbar_init();
   }
-  if (warp == GEMM_EPI_WARPS + 1) { tmem_alloc(tmem_slot, TMEM_COLS); tmem_relinquish(); }
-  if (warp == GEMM_EPI_WARPS && lane == 0) {
+  if (threadIdx.x == 32) {
     prefetch_tmap(&tmA_hi); prefetch_tmap(&tmW_hi);
     if (NPL == 2) { prefetch_tmap(&tmA_lo); prefetch_tmap(&tmW_lo); }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == GEMM_EPI_WARPS) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (threadIdx.x == 0) {
       uint32_t stage = 0, phase = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         const int n_tile = tile % p.num_n_tiles, m_tile = tile / p.num_n_tiles;
@@ -317,334 +211,44 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         }
       }
     }
-  } else if (warp == GEMM_EPI_WARPS + 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(BM, BN);
-      uint32_t stage = 0, phase = 0, it = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-        const uint32_t acc = it & 1, acc_phase = (it >> 1) & 1;
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t a_hi = make_sw128_kmajor_desc(sa + k * 32);
-            const uint64_t w_hi = make_sw128_kmajor_desc(sa + NPL * A_BYTES + k * 32);
-            umma_f16(d_tmem, a_hi, w_hi, idesc, (kb | k) != 0 ? 1u : 0u);
-            if (NTERMS == 3) {
-              const uint64_t a_lo = make_sw128_kmajor_desc(sa + A_BYTES + k * 32);
-              const uint64_t w_lo = make_sw128_kmajor_desc(sa + NPL * A_BYTES + W_BYTES + k * 32);
-              umma_f16(d_tmem, a_lo, w_hi, idesc, 1u);
-              umma_f16(d_tmem, a_hi, w_lo, idesc, 1u);
-            }
-          }
-          umma_commit(&empty[stage]);
-          if (kb == p.num_kb - 1) umma_commit(&tfull[acc]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
   } else {
-    constexpr int CPW = BN / (GEMM_EPI_WARPS / 4);   // accumulator columns per epilogue warp
-    const int q = warp & 3, hc = warp >> 2;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
+    const int cw = wg - 1, wq = warp & 3;      // consumer warpgroup: rows [cw * 64, +64) of the tile
+    uint32_t stage = 0, phase = 0;
+    float acc[BN / 2];
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const int n_tile = tile % p.num_n_tiles, m_tile = tile / p.num_n_tiles;
       const int b = m_tile / p.tiles_per_batch, m0 = (m_tile % p.tiles_per_batch) * BM, n0 = n_tile * BN;
-      const uint32_t acc = it & 1, acc_phase = (it >> 1) & 1;
-      if (QB_PARK) mbar_wait_parked(&tfull[acc], acc_phase); else mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN + hc * CPW;
-#pragma unroll 1
-      for (int c = 0; c < CPW; c += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(taddr + c, r);
-        tmem_ld_wait();
-        epilogue_row32(p, b, m0 + q * 32 + lane, n0 + hc * CPW + c, r);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == GEMM_EPI_WARPS + 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-// ------------------------------------------------------------------ CTA-pair kernel (cta_group::2)
-// A cluster of two CTAs (one TPC) owns a 256 x BN output tile: CTA r holds A rows [r*128, r*128+128) and
-// HALF of the weight tile (rows [r*BN/2, (r+1)*BN/2)); the leader issues tcgen05.mma.cta_group::2 (M = 256)
-// which reads both halves of B across the pair, so each SM ingests A 16 KB + W 16 KB per K-block instead of
-// 16 + 32: the L2 -> SM traffic of the single-pass GEMM drops by a third (it was load-paced, profiles/).
-// Barrier protocol: TMA of both CTAs signals the LEADER's full barrier; the leader's commit is multicast to
-// both CTAs' empty / tmem-full barriers; both epilogues arrive on the leader's tmem-empty barrier.
-template <int BN, int NTERMS, int STAGES>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_tc2_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
-                const GemmParams p) {
-  constexpr int BM = 128, BK = 64;
-  constexpr int NPL = (NTERMS == 1) ? 1 : 2;
-  constexpr uint32_t A_BYTES = BM * BK * 2, W_BYTES = (BN / 2) * BK * 2;
-  constexpr uint32_t STAGE_BYTES = NPL * (A_BYTES + W_BYTES);
-  constexpr uint32_t TMEM_COLS = 2 * BN;
-  static_assert(TMEM_COLS == 256 || TMEM_COLS == 512, "TMEM columns must be a power of two <= 512");
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = align1024(smem_raw);
-  uint64_t* full = (uint64_t*)(smem + STAGES * STAGE_BYTES);
-  uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = (uint32_t*)(tempty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], 2 * GEMM_EPI_WARPS); }
-    fence_mbar_init();
-  }
-  if (warp == GEMM_EPI_WARPS + 1) { tmem_alloc2(tmem_slot, TMEM_COLS); tmem_relinquish2(); }
-  if (warp == GEMM_EPI_WARPS && lane == 0) {
-    prefetch_tmap(&tmA_hi); prefetch_tmap(&tmW_hi);
-    if (NPL == 2) { prefetch_tmap(&tmA_lo); prefetch_tmap(&tmW_lo); }
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int num_clusters = gridDim.x >> 1, cluster_id = blockIdx.x >> 1;
-
-  if (warp == GEMM_EPI_WARPS) {
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      for (int tile = cluster_id; tile < p.num_tiles; tile += num_clusters) {
-        const int n_tile = tile % p.num_n_tiles, m_tile = tile / p.num_n_tiles;
-        const int b = m_tile / p.tiles_per_batch, m0 = (m_tile % p.tiles_per_batch) * 2 * BM + rank * BM;
-        const int n0 = n_tile * BN + rank * (BN / 2);
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          const int tap = kb / p.cblocks, cb = kb - tap * p.cblocks;
-          if (QB_PARK) mbar_wait_parked(&empty[stage], phase ^ 1); else mbar_wait(&empty[stage], phase ^ 1);
-          if (leader) mbar_arrive_expect_tx(&full[stage], 2 * STAGE_BYTES);
-          const uint32_t fb = mapa_u32(smem_u32(&full[stage]), 0);
-          uint8_t* s = smem + stage * STAGE_BYTES;
-          const int tt = tap * p.dil;      // input row of output row m: m * stride + tap * dilation
-          const int ax = (tt % p.stride) * p.Cld + cb * BK, ay = m0 + tt / p.stride, wx = tap * p.C + cb * BK;
-          tma2_load_3d(s, &tmA_hi, fb, ax, ay, b);
-          if (NPL == 2) tma2_load_3d(s + A_BYTES, &tmA_lo, fb, ax, ay, b);
-          tma2_load_2d(s + NPL * A_BYTES, &tmW_hi, fb, wx, n0);
-          if (NPL == 2) tma2_load_2d(s + NPL * A_BYTES + W_BYTES, &tmW_lo, fb, wx, n0);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == GEMM_EPI_WARPS + 1) {
-    if (lane == 0 && leader) {
-      constexpr uint32_t idesc = make_idesc_f16(2 * BM, BN);
-      uint32_t stage = 0, phase = 0, it = 0;
-      for (int tile = cluster_id; tile < p.num_tiles; tile += num_clusters, ++it) {
-        const uint32_t acc = it & 1, acc_phase = (it >> 1) & 1;
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+      uint32_t prev_stage = 0;
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + cw * (A_BYTES / 2);
+        const uint32_t sw = smem_u32(smem + stage * STAGE_BYTES) + NPL * A_BYTES;
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t a_hi = make_sw128_kmajor_desc(sa + k * 32);
-            const uint64_t w_hi = make_sw128_kmajor_desc(sa + NPL * A_BYTES + k * 32);
-            umma2_f16(d_tmem, a_hi, w_hi, idesc, (kb | k) != 0 ? 1u : 0u);
-            if (NTERMS == 3) {
-              const uint64_t a_lo = make_sw128_kmajor_desc(sa + A_BYTES + k * 32);
-              const uint64_t w_lo = make_sw128_kmajor_desc(sa + NPL * A_BYTES + W_BYTES + k * 32);
-              umma2_f16(d_tmem, a_lo, w_hi, idesc, 1u);
-              umma2_f16(d_tmem, a_hi, w_lo, idesc, 1u);
-            }
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t a_hi = make_wgmma_desc_sw128(sa + k * 32), w_hi = make_wgmma_desc_sw128(sw + k * 32);
+          Wgmma<BN>::ss(acc, a_hi, w_hi, (kb | k) != 0 ? 1u : 0u);
+          if (NTERMS == 3) {
+            Wgmma<BN>::ss(acc, make_wgmma_desc_sw128(sa + A_BYTES + k * 32), w_hi, 1u);
+            Wgmma<BN>::ss(acc, a_hi, make_wgmma_desc_sw128(sw + W_BYTES + k * 32), 1u);
           }
-          umma2_commit_mc(&empty[stage], 3);
-          if (kb == p.num_kb - 1) umma2_commit_mc(&tfull[acc], 3);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
+        wgmma_commit();
+        wgmma_wait<1>();                          // the MMAs of K-block kb - 1 are done: release their stage
+        if (kb > 0 && lane == 0) mbar_arrive(&empty[prev_stage]);
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-    }
-  } else {
-    constexpr int CPW = BN / (GEMM_EPI_WARPS / 4);
-    const int q = warp & 3, hc = warp >> 2;
-    uint32_t it = 0;
-    for (int tile = cluster_id; tile < p.num_tiles; tile += num_clusters, ++it) {
-      const int n_tile = tile % p.num_n_tiles, m_tile = tile / p.num_n_tiles;
-      const int b = m_tile / p.tiles_per_batch, m0 = (m_tile % p.tiles_per_batch) * 2 * BM + rank * BM, n0 = n_tile * BN;
-      const uint32_t acc = it & 1, acc_phase = (it >> 1) & 1;
-      if (QB_PARK) mbar_wait_parked(&tfull[acc], acc_phase); else mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN + hc * CPW;
-#pragma unroll 1
-      for (int c = 0; c < CPW; c += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(taddr + c, r);
-        tmem_ld_wait();
-        epilogue_row32(p, b, m0 + q * 32 + lane, n0 + hc * CPW + c, r);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty[acc]), 0));
-    }
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == GEMM_EPI_WARPS + 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, TMEM_COLS);
-  }
-}
-
-// ------------------------------------------------------------------ two CTA pairs per cluster, weight tile multicast
-// The pair kernel above is bound by the bytes the L2 can deliver per SM (measured 40 B/clk/SM = the chip-level
-// 6.3 kB/clk cap, profiles/r01_ncu_gemm_pair_final.txt): per K-block every CTA pulls A 16 KB + W 16 KB for 512 MMA cycles.
-// Here a cluster of FOUR CTAs = two pairs owns a 512 x BN super-tile: the pairs take adjacent 256-row M tiles of the SAME
-// N tile, so the CTAs with equal pair rank need the same half of the weight tile - each loads a quarter (64 rows) and
-// multicasts it to its counterpart.  L2 -> SM requests per CTA and K-block: 16 + 8 = 24 KB (48 B/clk at full tensor rate).
-// Protocol: full[]: as the pair kernel (all bytes that land in a pair's two CTAs are signalled on that pair's leader);
-// empty[]: a stage of CTA c is also written by its counterpart, so BOTH leaders' commits arrive on every CTA's empty
-// barrier (count 2); tfull / tempty stay pair-local.  a_batch == 1 only (nn.Linear shapes); rows past M are zero-filled
-// by TMA and masked in the epilogue, so an odd number of pair tiles needs no special case.
-template <int BN, int NTERMS, int STAGES>
-__global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_tc4_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
-                const GemmParams p) {
-  constexpr int BM = 128, BK = 64;
-  constexpr int NPL = (NTERMS == 1) ? 1 : 2;
-  constexpr uint32_t A_BYTES = BM * BK * 2, W_BYTES = (BN / 2) * BK * 2, WQ_BYTES = W_BYTES / 2;
-  constexpr uint32_t STAGE_BYTES = NPL * (A_BYTES + W_BYTES);
-  constexpr uint32_t TMEM_COLS = 2 * BN;
-  static_assert(TMEM_COLS == 256 || TMEM_COLS == 512, "TMEM columns must be a power of two <= 512");
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = align1024(smem_raw);
-  uint64_t* full = (uint64_t*)(smem + STAGES * STAGE_BYTES);
-  uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = (uint32_t*)(tempty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank(), pair = rank >> 1, r = rank & 1;
-  const bool leader = r == 0;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], 2 * GEMM_EPI_WARPS); }
-    fence_mbar_init();
-  }
-  if (warp == GEMM_EPI_WARPS + 1) { tmem_alloc2(tmem_slot, TMEM_COLS); tmem_relinquish2(); }
-  if (warp == GEMM_EPI_WARPS && lane == 0) {
-    prefetch_tmap(&tmA_hi); prefetch_tmap(&tmW_hi);
-    if (NPL == 2) { prefetch_tmap(&tmA_lo); prefetch_tmap(&tmW_lo); }
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int num_clusters = gridDim.x >> 2, cluster_id = blockIdx.x >> 2;
-  const int num_super = p.tiles_per_batch * p.num_n_tiles;       // tiles_per_batch = ceil(M / 512) here
-
-  if (warp == GEMM_EPI_WARPS) {
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      const uint16_t mc_mask = (uint16_t)((1u << r) | (1u << (2 + r)));
-      for (int tile = cluster_id; tile < num_super; tile += num_clusters) {
-        const int n_tile = tile % p.num_n_tiles, m_super = tile / p.num_n_tiles;
-        const int m0 = (m_super * 2 + (int)pair) * 2 * BM + (int)r * BM;
-        const int n0 = n_tile * BN + (int)r * (BN / 2) + (int)pair * (BN / 4);      // this CTA's quarter of the weight tile
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          if (QB_PARK) mbar_wait_parked(&empty[stage], phase ^ 1); else mbar_wait(&empty[stage], phase ^ 1);
-          if (leader) mbar_arrive_expect_tx(&full[stage], 2 * STAGE_BYTES);
-          uint8_t* s = smem + stage * STAGE_BYTES;
-          const int kx = kb * BK;
-          tma2_load_3d_peer(s, &tmA_hi, &full[stage], kx, m0, 0);
-          if (NPL == 2) tma2_load_3d_peer(s + A_BYTES, &tmA_lo, &full[stage], kx, m0, 0);
-          tma2_load_2d_mc(s + NPL * A_BYTES + pair * WQ_BYTES, &tmW_hi, &full[stage], kx, n0, mc_mask);
-          if (NPL == 2) tma2_load_2d_mc(s + NPL * A_BYTES + W_BYTES + pair * WQ_BYTES, &tmW_lo, &full[stage], kx, n0, mc_mask);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == GEMM_EPI_WARPS + 1) {
-    if (lane == 0 && leader) {
-      constexpr uint32_t idesc = make_idesc_f16(2 * BM, BN);
-      const uint16_t pair_mask = (uint16_t)(3u << (2 * pair));
-      uint32_t stage = 0, phase = 0, it = 0;
-      for (int tile = cluster_id; tile < num_super; tile += num_clusters, ++it) {
-        const uint32_t acc = it & 1, acc_phase = (it >> 1) & 1;
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (lane == 0) mbar_arrive(&empty[prev_stage]);
+      const int r = m0 + cw * 64 + wq * 16 + (lane >> 2), c = n0 + 2 * (lane & 3);
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t a_hi = make_sw128_kmajor_desc(sa + k * 32);
-            const uint64_t w_hi = make_sw128_kmajor_desc(sa + NPL * A_BYTES + k * 32);
-            umma2_f16(d_tmem, a_hi, w_hi, idesc, (kb | k) != 0 ? 1u : 0u);
-            if (NTERMS == 3) {
-              const uint64_t a_lo = make_sw128_kmajor_desc(sa + A_BYTES + k * 32);
-              const uint64_t w_lo = make_sw128_kmajor_desc(sa + NPL * A_BYTES + W_BYTES + k * 32);
-              umma2_f16(d_tmem, a_lo, w_hi, idesc, 1u);
-              umma2_f16(d_tmem, a_hi, w_lo, idesc, 1u);
-            }
-          }
-          umma2_commit_mc(&empty[stage], 0xF);          // the stage is free once BOTH pairs have consumed it
-          if (kb == p.num_kb - 1) umma2_commit_mc(&tfull[acc], pair_mask);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
+      for (int j = 0; j < BN / 8; ++j) {
+        epilogue_pair(p, b, r, c + 8 * j, acc[4 * j], acc[4 * j + 1]);
+        epilogue_pair(p, b, r + 8, c + 8 * j, acc[4 * j + 2], acc[4 * j + 3]);
       }
     }
-  } else {
-    constexpr int CPW = BN / (GEMM_EPI_WARPS / 4);
-    const int q = warp & 3, hc = warp >> 2;
-    uint32_t it = 0;
-    const uint32_t tempty_leader = mapa_u32(smem_u32(&tempty[0]), rank & ~1u);
-    for (int tile = cluster_id; tile < num_super; tile += num_clusters, ++it) {
-      const int n_tile = tile % p.num_n_tiles, m_super = tile / p.num_n_tiles;
-      const int m0 = (m_super * 2 + (int)pair) * 2 * BM + (int)r * BM, n0 = n_tile * BN;
-      const uint32_t acc = it & 1, acc_phase = (it >> 1) & 1;
-      if (QB_PARK) mbar_wait_parked(&tfull[acc], acc_phase); else mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN + hc * CPW;
-#pragma unroll 1
-      for (int c = 0; c < CPW; c += 32) {
-        uint32_t rr[32];
-        tmem_ld_32x32b_x32(taddr + c, rr);
-        tmem_ld_wait();
-        epilogue_row32(p, 0, m0 + q * 32 + lane, n0 + hc * CPW + c, rr);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(tempty_leader + acc * 8);
-    }
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == GEMM_EPI_WARPS + 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, TMEM_COLS);
   }
 }
 
@@ -754,8 +358,9 @@ static int fill_params(const qb_gemm_desc* d, GemmParams* p, int BN) {
   return 0;
 }
 
-template <int BN, int NTERMS, int STAGES>
+template <int NTERMS, int STAGES>
 static int launch_tc(const qb_gemm_desc* d, cudaStream_t st, int num_sms) {
+  constexpr int BN = GEMM_BN;
   GemmParams p;
   if (int e = fill_params(d, &p, BN)) return e;
   CUtensorMap mA_hi, mA_lo, mW_hi, mW_lo;
@@ -776,8 +381,9 @@ static int launch_tc(const qb_gemm_desc* d, cudaStream_t st, int num_sms) {
     mA_lo = mA_hi; mW_lo = mW_hi;
   }
   constexpr int NPL = NTERMS == 1 ? 1 : 2;
-  constexpr size_t smem = (size_t)STAGES * NPL * (128 * 64 * 2 + BN * 64 * 2) + 1024 + 256;
-  auto kern = gemm_tc_kernel<BN, NTERMS, STAGES>;
+  constexpr size_t smem = (size_t)STAGES * NPL * (GEMM_BM * 64 * 2 + BN * 64 * 2) + 1024 + 256;
+  static_assert(smem <= 227 * 1024, "GEMM pipeline exceeds the 227 KB of shared memory a block may use");
+  auto kern = gemm_tc_kernel<NTERMS, STAGES>;
   static bool attr_set[QB_MAX_DEVICES] = {};          // the opt-in shared-memory limit is per-device state
   const int dev = current_device();
   if (!attr_set[dev]) {
@@ -786,96 +392,6 @@ static int launch_tc(const qb_gemm_desc* d, cudaStream_t st, int num_sms) {
   }
   int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
   kern<<<grid, GEMM_THREADS, smem, st>>>(mA_hi, mA_lo, mW_hi, mW_lo, p);
-  g_launches++;
-  QB_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-template <int BN, int NTERMS, int STAGES>
-static int launch_tc2(const qb_gemm_desc* d, cudaStream_t st, int num_sms) {
-  GemmParams p;
-  if (int e = fill_params(d, &p, BN)) return e;
-  p.tiles_per_batch = (int)ceil_div(d->m_per_batch, 256);      // pair tiles of 256 rows
-  p.num_tiles = (int)(d->a_batch * p.tiles_per_batch * p.num_n_tiles);
-  CUtensorMap mA_hi, mA_lo, mW_hi, mW_lo;
-  const cuuint64_t C = (cuuint64_t)d->a_ld, s = (cuuint64_t)d->stride;
-  cuuint64_t adims[3] = {s * C, (cuuint64_t)d->a_rows_per_batch / s, (cuuint64_t)d->a_batch};
-  cuuint64_t astr[2] = {s * C * 2, (cuuint64_t)d->a_rows_per_batch * C * 2};
-  cuuint32_t abox[3] = {64, 128, 1};
-  const cuuint64_t Ck = (cuuint64_t)(d->a_cols > 0 ? d->a_cols : d->a_ld);
-  cuuint64_t wdims[2] = {(cuuint64_t)d->taps * Ck, (cuuint64_t)d->n};
-  cuuint64_t wstr[1] = {(cuuint64_t)d->taps * Ck * 2};
-  cuuint32_t wbox[2] = {64, (cuuint32_t)(BN / 2)};
-  if (int e = make_map(&mA_hi, d->a_hi, 3, adims, astr, abox)) return e;
-  if (int e = make_map(&mW_hi, d->w_hi, 2, wdims, wstr, wbox)) return e;
-  if (NTERMS == 3) {
-    if (int e = make_map(&mA_lo, d->a_lo, 3, adims, astr, abox)) return e;
-    if (int e = make_map(&mW_lo, d->w_lo, 2, wdims, wstr, wbox)) return e;
-  } else {
-    mA_lo = mA_hi; mW_lo = mW_hi;
-  }
-  constexpr int NPL = NTERMS == 1 ? 1 : 2;
-  constexpr size_t smem = (size_t)STAGES * NPL * (128 * 64 * 2 + (BN / 2) * 64 * 2) + 1024 + 256;
-  auto kern = gemm_tc2_kernel<BN, NTERMS, STAGES>;
-  static bool attr_set[QB_MAX_DEVICES] = {};
-  const int dev = current_device();
-  if (!attr_set[dev]) {
-    QB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set[dev] = true;
-  }
-  int clusters = p.num_tiles < num_sms / 2 ? p.num_tiles : num_sms / 2;
-  kern<<<2 * clusters, GEMM_THREADS, smem, st>>>(mA_hi, mA_lo, mW_hi, mW_lo, p);
-  g_launches++;
-  QB_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-
-template <int BN, int NTERMS, int STAGES>
-static int launch_tc4(const qb_gemm_desc* d, cudaStream_t st, int num_sms) {
-  GemmParams p;
-  if (int e = fill_params(d, &p, BN)) return e;
-  QB_REQUIRE(d->a_batch == 1 && d->taps == 1 && d->stride == 1, "gemm: the 4-CTA multicast kernel serves plain linear layers only");
-  p.tiles_per_batch = (int)ceil_div(d->m_per_batch, 512);      // super-tiles of 2 x 256 rows
-  p.num_tiles = p.tiles_per_batch * p.num_n_tiles;
-  CUtensorMap mA_hi, mA_lo, mW_hi, mW_lo;
-  const cuuint64_t C = (cuuint64_t)d->a_ld;
-  cuuint64_t adims[3] = {C, (cuuint64_t)d->a_rows_per_batch, 1};
-  cuuint64_t astr[2] = {C * 2, (cuuint64_t)d->a_rows_per_batch * C * 2};
-  cuuint32_t abox[3] = {64, 128, 1};
-  cuuint64_t wdims[2] = {C, (cuuint64_t)d->n};
-  cuuint64_t wstr[1] = {C * 2};
-  cuuint32_t wbox[2] = {64, (cuuint32_t)(BN / 4)};
-  if (int e = make_map(&mA_hi, d->a_hi, 3, adims, astr, abox)) return e;
-  if (int e = make_map(&mW_hi, d->w_hi, 2, wdims, wstr, wbox)) return e;
-  if (NTERMS == 3) {
-    if (int e = make_map(&mA_lo, d->a_lo, 3, adims, astr, abox)) return e;
-    if (int e = make_map(&mW_lo, d->w_lo, 2, wdims, wstr, wbox)) return e;
-  } else {
-    mA_lo = mA_hi; mW_lo = mW_hi;
-  }
-  constexpr int NPL = NTERMS == 1 ? 1 : 2;
-  constexpr size_t smem = (size_t)STAGES * NPL * (128 * 64 * 2 + (BN / 2) * 64 * 2) + 1024 + 256;
-  auto kern = gemm_tc4_kernel<BN, NTERMS, STAGES>;
-  static int max_clusters[QB_MAX_DEVICES] = {};
-  const int dev = current_device();
-  if (!max_clusters[dev]) {
-    QB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(4 * 64); cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = smem;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 4; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    int n = 0;
-    QB_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
-    QB_REQUIRE(n >= 1, "gemm: no 4-CTA cluster fits on this device");
-    if (const char* e = getenv("QB_GEMM4_CLUSTERS")) n = atoi(e) < n ? atoi(e) : n;
-    max_clusters[dev] = n;
-  }
-  (void)num_sms;
-  int clusters = p.num_tiles < max_clusters[dev] ? p.num_tiles : max_clusters[dev];
-  kern<<<4 * clusters, GEMM_THREADS, smem, st>>>(mA_hi, mA_lo, mW_hi, mW_lo, p);
   g_launches++;
   QB_CHECK_CUDA(cudaGetLastError());
   return 0;
@@ -900,58 +416,17 @@ extern "C" int qb_version(void) { return 100; }
 extern "C" int64_t qb_launch_count(void) { return (int64_t)g_launches.load(); }
 extern "C" void qb_launch_count_reset(void) { g_launches = 0; }
 
-// kernel variant for a problem shape (one place: qb_gemm dispatches on it, qb_gemm_kernel_name reports it)
-enum GemmVariant { GV_QUAD_SINGLE, GV_PAIR_SINGLE, GV_PAIR_SPLIT, GV_TC_256_SINGLE, GV_TC_128_SINGLE, GV_TC_256_SPLIT, GV_TC_128_SPLIT };
-// QB_GEMM_QUAD=1: single-pass linear layers with M >= 4096 rows and N a multiple of 256 go to the 4-CTA multicast kernel
-static int quad_mode() {
-  static const int v = getenv("QB_GEMM_QUAD") ? atoi(getenv("QB_GEMM_QUAD")) : 0;
-  return v;
-}
-static GemmVariant pick_variant(int64_t m_per_batch, int64_t n, bool split, bool linear = false) {
-  if (linear && !split && quad_mode() && m_per_batch >= 4096 && n % 256 == 0) return GV_QUAD_SINGLE;
-  int bn = n > 128 ? 256 : 128;
-  if (split) bn = 128;
-  static const char* env_bn = getenv("QB_GEMM_BN_SPLIT");
-  if (split && env_bn) bn = atoi(env_bn);
-  if (n <= 128) bn = 128;
-  // CTA pairs (256-row tiles) when they do not add row padding and the N extent fills a 256-wide tile
-  static const int pair_mode = getenv("QB_GEMM_PAIR") ? atoi(getenv("QB_GEMM_PAIR")) : 1;
-  // (a pair tile that is 3/4 full in N still halves the operand bytes each SM ingests per MMA; up to 3 % of padded rows
-  //  per batch are accepted - the 1-CTA kernel is ingest-bound on every conv shape of the BiCodec generator)
-  const long long m256 = ceil_div(m_per_batch, 256) * 256;
-  const bool pair_ok = pair_mode && n >= 192 &&
-                       (ceil_div(m_per_batch, 256) * 2 == ceil_div(m_per_batch, 128) || m256 * 100 <= m_per_batch * 103);
-  if (pair_ok) return split ? GV_PAIR_SPLIT : GV_PAIR_SINGLE;
-  if (!split) return bn == 256 ? GV_TC_256_SINGLE : GV_TC_128_SINGLE;
-  return bn == 256 ? GV_TC_256_SPLIT : GV_TC_128_SPLIT;
-}
-
+// One tile shape (128 x 128 x 64) for every problem: single pass with 6 pipeline stages (192 KB), hi + lo split with 3.
 extern "C" const char* qb_gemm_kernel_name(int64_t m_per_batch, int64_t n, int32_t split) {
-  switch (pick_variant(m_per_batch, n, split != 0, true)) {
-    case GV_QUAD_SINGLE: return "gemm_tc4_kernel<256,1,6> (2 x cta_group::2, weight tile multicast)";
-    case GV_PAIR_SINGLE: return "gemm_tc2_kernel<256,1,6> (cta_group::2)";
-    case GV_PAIR_SPLIT: return "gemm_tc2_kernel<256,3,3> (cta_group::2)";
-    case GV_TC_256_SINGLE: return "gemm_tc_kernel<256,1,4>";
-    case GV_TC_128_SINGLE: return "gemm_tc_kernel<128,1,6>";
-    case GV_TC_256_SPLIT: return "gemm_tc_kernel<256,3,2>";
-    default: return "gemm_tc_kernel<128,3,3>";
-  }
+  (void)m_per_batch; (void)n;
+  return split ? "gemm_tc_kernel<3,3>" : "gemm_tc_kernel<1,6>";
 }
 
 extern "C" int qb_gemm(const qb_gemm_desc* d, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   QB_REQUIRE(d != nullptr, "gemm: null desc");
   const int sms = num_sms_cached();
-  const bool linear = d->a_batch == 1 && d->taps == 1 && d->stride == 1;
-  switch (pick_variant(d->m_per_batch, d->n, d->a_lo != nullptr, linear)) {
-    case GV_QUAD_SINGLE: return launch_tc4<256, 1, 6>(d, st, sms);
-    case GV_PAIR_SINGLE: return launch_tc2<256, 1, 6>(d, st, sms);
-    case GV_PAIR_SPLIT: return launch_tc2<256, 3, 3>(d, st, sms);
-    case GV_TC_256_SINGLE: return launch_tc<256, 1, 4>(d, st, sms);
-    case GV_TC_128_SINGLE: return launch_tc<128, 1, 6>(d, st, sms);
-    case GV_TC_256_SPLIT: return launch_tc<256, 3, 2>(d, st, sms);
-    default: return launch_tc<128, 3, 3>(d, st, sms);
-  }
+  return d->a_lo != nullptr ? launch_tc<3, 3>(d, st, sms) : launch_tc<1, 6>(d, st, sms);
 }
 
 extern "C" int qb_gemm_simt(const qb_gemm_desc* d, void* stream) {

@@ -2,7 +2,7 @@
 // decoder layers: RMSNorm(1e-6) -> q/k/v (no bias) -> RoPE -> causal attention -> o_proj -> +res ->
 // RMSNorm -> SwiGLU MLP -> +res).
 //
-// Prefill / teacher-forced forward (L > 1) runs on the tcgen05 GEMM (gemm.cu) plus the two kernels here:
+// Prefill / teacher-forced forward (L > 1) runs on the wgmma GEMM (gemm.cu) plus the two kernels here:
 //   lm_qkv_prep   RoPE at absolute positions, 1/sqrt(d) folded into q, K/V appended to the static fp32 cache
 //   lm_flash_attn causal flash attention (mma.sync m16n8k16, 3-term fp16 split of Q/K/P/V) over the cache
 // KV-cache decode (L == 1, B <= 32) is HBM-bound (weights + cache streamed once per step): "skinny" fp32
@@ -800,7 +800,7 @@ __global__ void lm_pack_weight_kernel(const float* __restrict__ w, long long tot
 }
 
 // 256-thread variants are capped at 128 registers so that TWO CTAs fit an SM: the gate/up projection (inter/8 = 256 CTAs) and the
-// head (256 / 512 CTAs) then run in one / two waves on 148 SMs instead of two / four (QB_LM_SKINNY_OCC, measured in profiles/).
+// head (256 / 512 CTAs) then run in one / two waves on 132 SMs instead of two / four (QB_LM_SKINNY_OCC).
 template <int MODE, int SPW, int NW>
 __global__ void __launch_bounds__(NW * 32, NW == 8 ? 2 : 1)
 lm_skinny_kernel(const SkParams p) {
@@ -1222,8 +1222,7 @@ extern "C" int qb_lm_decode_layer_tc(float* x, int64_t B, int32_t hidden, int32_
   p.x = x; p.K = hidden; p.W = (const uint4*)wqkv; p.out = q_buf;
   if (int e = launch_skinny<SK_QKV>(p, 3 * heads * 4, st)) return e;
   // keys in flight per half-warp trip (K and V rows of LM_ATT_U keys per lane), qb_lm_set_att_unroll: 8 for a single decode chain
-  // (latency-bound: 103.3 -> 98.2 ms per SR generate, 111.5 -> 101.9 ms TSE), 4 when several chains share the GPU (throughput-
-  // bound: 474 vs 492 ms for 256 sequences on 4 lanes) - profiles/r02_lm_lanes_ab.md
+  // (latency-bound), 4 when several chains share the GPU (throughput-bound)
   auto att = g_lm_att_unroll == 4 ? lm_decode_attn2_kernel<4> : lm_decode_attn2_kernel<8>;
   QB_CHECK_CUDA(launch_pdl(att, dim3((unsigned)heads, (unsigned)B), dim3(256), 0, st, (const float*)q_buf,
                            (const float*)k_cache, (const float*)v_cache, (int)heads, (int)Lmax, (const int*)pos, attn_buf,

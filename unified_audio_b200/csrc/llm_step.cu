@@ -1,7 +1,7 @@
 // UniSE AR-LM cached decode as ONE persistent cooperative kernel (QuarkAudio-UniSE/model/llm/llm_sft.py:137-193, greedy).
 //
 // The per-kernel decode step (llm.cu: 5 kernels per layer + 2 for the head = 62 dependent launches per token) is bound by
-// launch-to-launch dependency latency: ~5.8 us per kernel for 2.6 us of HBM traffic (profiles/r02_launches_lm.md).  Here the
+// launch-to-launch dependency latency rather than by its HBM traffic.  Here the
 // whole generation loop runs inside one kernel of one CTA per SM: the 62 stages of a step are separated by a device-side grid
 // barrier (one atomic arrive + one polled word) instead of a kernel boundary, every worker issues the weight loads of its
 // next tile BEFORE it waits at the barrier (weights do not depend on activations), and all step state (position, output slot)

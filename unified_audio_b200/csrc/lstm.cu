@@ -2,7 +2,7 @@
 // (reference: nn.LSTM(H,H,1,batch_first) inside every attention block,
 //  HCodec-2.0/vq/encoder_modules/transformer.py:115,133).
 //
-// The input projection x W_ih^T + b_ih + b_hh is done beforehand by the tcgen05 GEMM (xp).  Here:
+// The input projection x W_ih^T + b_ih + b_hh is done beforehand by the wgmma GEMM (xp).  Here:
 //  * hidden units are sharded over CTAs (U = 4*MT units -> 16*MT gate rows i|f|g|o per CTA);
 //    the CTA's fp16 W_hh slice stays resident in shared memory for all T steps;
 //  * per step every CTA computes gates[16*MT x B] = W_slice . h_{t-1}^T with mma.sync m16n8k16

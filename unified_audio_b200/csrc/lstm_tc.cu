@@ -1,19 +1,15 @@
-// LSTM recurrence on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), persistent cooperative kernel.
+// LSTM recurrence on the Hopper tensor cores (wgmma + TMA + mbarrier), persistent cooperative kernel.
 // Reference: nn.LSTM(H,H,1,batch_first), HCodec-2.0/vq/encoder_modules/transformer.py:115,133.
 //
-// Measured (profiles/): the mma.sync version (lstm.cu) spends 15.4k of its 26k cycles per step in legacy
-// HMMA issue - mma.sync runs at a fraction of the tcgen05 rate on sm_100.  Here each CTA keeps its W_hh
-// slice [4U gate rows x H] resident in shared memory as the UMMA *B* operand (K-major, 128B swizzle, loaded
-// once by TMA) and streams h_{t-1} (fp16, published by all CTAs) through a TMA ring as the *A* operand;
-// gates accumulate in TMEM.
+// Each CTA keeps its W_hh slice [4U gate rows x H] resident in shared memory as the wgmma *B* operand (K-major, 128B swizzle,
+// loaded once by TMA) and streams h_{t-1} (fp16, published by all CTAs) through a bulk-copy ring as the *A* operand; the gates
+// accumulate in registers of the consumer warpgroups.
 //
-// The batch is split into GROUPS of 32 rows that are independent recurrences: group g lives in TMEM lane
-// quadrant g (A-tile rows 32g..32g+31, own accumulator columns, own flags, own epilogue warps g and g+4).
-// The groups are software-pipelined: while group g waits for the grid-wide publication of its h_t (epilogue +
-// fence + flag round trip), the TMA/MMA pipeline is busy with the other groups' steps.  An A tile always spans
-// 128 rows; a group's 4 KB K-block sits at tile row 32g by pointing the UMMA descriptor 4g KB below the slot
-// (same 128B-swizzle phase since 32 rows = 4 x 1024 B); the other rows read whatever finite fp16 data
-// neighbours the slot and only produce garbage in D rows nobody reads.
+// The batch is split into GROUPS of 32 rows that are independent recurrences: group g is served by consumer warpgroup g (own
+// accumulators, own flags).  The groups are software-pipelined: while group g waits for the grid-wide publication of its h_t
+// (epilogue + fence + flag round trip), the TMA ring and the other warpgroups' MMAs carry the other groups' steps.  wgmma reads 64
+// A rows: a group's 32 rows are rows 0..31 of the tile, rows 32..63 read whatever finite fp16 data follows the K-block in the ring
+// (zeroed pad past its end) and only produce accumulators nobody reads (warps 2-3 of the warpgroup).
 // W rows are pre-permuted by the host to unit-major order: row (4*j + g) of CTA c = gate g of unit c*U + j.
 #include <atomic>
 #include <cstdio>
@@ -21,16 +17,17 @@
 
 #include "common.cuh"
 #include "quark_b200.h"
+#include "wgmma.cuh"
 
 namespace qb {
 extern std::atomic<long long> g_launches;
 
-constexpr int LT_EPI_WARPS = 8, LT_THREADS = (LT_EPI_WARPS + 2) * 32;
-constexpr int LT_KG = 4;                          // K-blocks fetched by one TMA instruction (5-D box)
+constexpr int LT_GROUPS = 4, LT_THREADS = LT_GROUPS * 128 + 32;   // 4 consumer warpgroups + one producer warp
+constexpr int LT_KG = 4;                          // K-blocks fetched by one bulk copy
 constexpr int LT_STAGES = 4;                      // ring: 4 x (LT_KG x 4 KB) = 64 KB
 constexpr uint32_t LT_KBLK = 32 * 128;            // one K-block of one group: 32 rows x 128 B
 constexpr uint32_t LT_SLOT = LT_KBLK * LT_KG;
-constexpr uint32_t LT_PAD = 12 * 1024;            // A tiles read up to 12 KB past a group-0 K-block
+constexpr uint32_t LT_PAD = 4 * 1024;             // a 64-row A tile reads up to 4 KB past the last K-block of the ring
 
 // flag polling: relaxed loads (the four of a lane are independent and in flight together - acquire loads would serialise
 // into four L2 round trips per poll), one acquire fence once every flag has been seen
@@ -44,14 +41,9 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tmem_ld_32x32b_x8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr) : "memory");
-}
 
 // Gate non-linearities of the epilogue: ex2.approx + rcp.approx (2^-21 relative on exp, 1 ulp on the reciprocal; absolute
-// error < 3e-7 on sigmoid / tanh) - the epilogue sits on the step's critical chain (3.1 k of ~21 k cycles with expf / tanhf).
+// error < 3e-7 on sigmoid / tanh) - the epilogue sits on the step's critical chain.
 __device__ __forceinline__ float lt_rcp(float x) {
   float r;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
@@ -60,90 +52,55 @@ __device__ __forceinline__ float lt_rcp(float x) {
 __device__ __forceinline__ float lt_sigmoid(float x) { return lt_rcp(1.0f + __expf(-x)); }
 __device__ __forceinline__ float lt_tanh(float x) { return fmaf(-2.0f, lt_rcp(1.0f + __expf(2.0f * x)), 1.0f); }
 
-// ---- A operand from TMEM (round 2).  One step's MMA phase is bound by shared-memory bytes per MMA (profiles/r01_lstm_step_anatomy.md:
-// cycles per MMA ~ (A read + B read + ring fill) / 64 B/clk); an M = 128 A tile reads 128 rows of which 32 are a group's.  With
-// `tcgen05.cp.32x128b.warpx4` the group's 32 rows x 8 halves are copied smem -> TMEM once (512 B, broadcast to the four lane
-// quadrants) and `tcgen05.mma` takes A from TMEM: 1 KB instead of 4 KB of A traffic per MMA.  h is published in the no-swizzle
-// core-matrix layout the copy reads: K-block = [kc = k/8][rb = row/8][row%8][k%8] (8 x 8 halves per core matrix, 128 B).
-// Probe of the instruction semantics: profiles/experiments/ts_mma_probe.cu (2e-6 vs the host on all four quadrants).
-// RESULT (B200, B = 64): bit-identical outputs, but 21.1 us / step against 11.8 us for the shared-memory A operand: the 192
-// `tcgen05.cp` per group-step cost ~100 cycles EACH (first h slot -> last MMA issued: 18.9 k cycles instead of 8.1 k) - the copy's
-// instruction throughput, not its bytes, binds.  Kept behind QB_LSTM_TS=1 as a measured negative result.
-__device__ __forceinline__ uint64_t lt_desc_core(uint32_t addr) {      // 4 core matrices 128 B apart, no swizzle
-  uint64_t d = 0;
-  d |= (uint64_t)((addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(128 >> 4) << 16;
-  d |= (uint64_t)(128 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
-}
-__device__ __forceinline__ void lt_cp_32x128b_warpx4(uint32_t taddr, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(taddr), "l"(sdesc) : "memory");
-}
-__device__ __forceinline__ void lt_umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(acc)
-      : "memory");
-}
-constexpr uint32_t LT_TS_ACOL = 256;     // TMEM columns 256..511: two A buffers of LT_KG K-blocks (32 columns each)
-
-template <int U, bool TS>
+template <int U>
 __global__ void __launch_bounds__(LT_THREADS, 1)
 lstm_tc_kernel(const __grid_constant__ CUtensorMap tmW,
                const float* __restrict__ xp, int B, int T, int H, __half* __restrict__ out_hi,
-               __half* __restrict__ out_lo, __half* hbuf, unsigned* flags, int Bp, int n_groups, int poll_ns, long long* prof) {
-  constexpr int N = 4 * U;                      // gate rows of this CTA = UMMA N
-  constexpr int HALF = U / 2;                   // units per epilogue thread
-  static_assert(N % 16 == 0 && N <= 64 && HALF * 4 % 8 == 0, "unsupported slice width");
+               __half* __restrict__ out_lo, __half* hbuf, unsigned* flags, int n_groups, int poll_ns) {
+  constexpr int N = 4 * U;                      // gate rows of this CTA = wgmma N
+  constexpr int UPT = N / 8;                    // units per epilogue thread
+  static_assert(N % 16 == 0 && N <= 48, "unsupported slice width");
   constexpr uint32_t WBLK = N * 128;            // bytes of one [N x 64] K-block of W
-  constexpr uint32_t TCOLS = TS ? 512 : (4 * N <= 64 ? 64 : (4 * N <= 128 ? 128 : 256));
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  const int KB = H / 64;
+  const int KB = H / 64, SLOTS = KB / LT_KG;    // ring slots per group and step
   uint8_t* Wsm = smem;
   uint8_t* ring = smem + (size_t)KB * WBLK;     // KB*WBLK is a multiple of 1024 (N % 8 == 0)
   uint64_t* full = (uint64_t*)(ring + LT_STAGES * LT_SLOT + LT_PAD);
   uint64_t* empty = full + LT_STAGES;
   uint64_t* wbar = empty + LT_STAGES;
-  uint64_t* tfull = wbar + 1;                   // [4] one per group
-  uint32_t* tmem_slot = (uint32_t*)(tfull + 4);
-  __shared__ long long ts_flag[4], ts_first[4], ts_last[4];     // profiling timestamps (group-indexed)
+  // slot_tag[s]: index of the ring slot stage s currently holds (written by the producer once it owns the stage).  The groups share
+  // the ring, so a warpgroup may wait for a slot whose stage is still several phases behind; a parity wait is only meaningful one
+  // phase ahead, hence the tag is checked first.
+  int* slot_tag = (int*)(wbar + 1);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int u0 = blockIdx.x * U, G = gridDim.x;
 
   if (tid == 0) {
-    for (int s = 0; s < LT_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+    for (int s = 0; s < LT_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4); }
     mbar_init(wbar, 1);
-    for (int g = 0; g < 4; ++g) mbar_init(&tfull[g], 1);
+    for (int s = 0; s < LT_STAGES; ++s) slot_tag[s] = -1;
     fence_mbar_init();
   }
   // ring + pad zeroed once: tile rows outside a group's K-block must be finite
   for (int i = tid; i < (int)((LT_STAGES * LT_SLOT + LT_PAD) / 16); i += LT_THREADS)
     reinterpret_cast<uint4*>(ring)[i] = make_uint4(0, 0, 0, 0);
   fence_proxy_async();
-  if (warp == LT_EPI_WARPS + 1) { tmem_alloc(tmem_slot, TCOLS); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == LT_EPI_WARPS) {
-    // ===================== TMA producer =====================
+  if (warp == LT_GROUPS * 4) {
+    // ===================== producer: flags -> bulk copies of h_{t-1} =====================
     if (lane == 0) {
       prefetch_tmap(&tmW);
       mbar_arrive_expect_tx(wbar, (uint32_t)KB * WBLK);
       for (int kb = 0; kb < KB; ++kb) tma_load_2d(Wsm + (size_t)kb * WBLK, &tmW, wbar, kb * 64, blockIdx.x * N);
     }
     uint32_t stage = 0, phase = 0;
-    long long pw = 0;
+    int slot = 0;
     for (int t = 1; t < T; ++t) {
       for (int g = 0; g < n_groups; ++g) {
         // wait until every CTA has published h_{t-1} of group g
-        const long long c0 = clock64();
         const unsigned* fl = flags + (size_t)g * G;
         unsigned spins = 0;
         for (;;) {
@@ -155,14 +112,14 @@ lstm_tc_kernel(const __grid_constant__ CUtensorMap tmW,
         }
         asm volatile("fence.acq_rel.gpu;" ::: "memory");        // acquire side of the flags every lane has just observed
         __syncwarp();
-        pw += clock64() - c0;
         if (lane == 0) {
-          ts_flag[g] = clock64();
-          asm volatile("fence.proxy.async;" ::: "memory");    // generic-proxy writes of h -> async-proxy (TMA) reads
+          asm volatile("fence.proxy.async;" ::: "memory");    // generic-proxy writes of h -> async-proxy (bulk copy) reads
           const int buf = (t + 1) & 1;                          // h_{t-1} lives in buffer (t-1)&1
-          for (int kb = 0; kb < KB; kb += LT_KG) {
+          for (int kb = 0; kb < KB; kb += LT_KG, ++slot) {
             mbar_wait(&empty[stage], phase ^ 1);
             mbar_arrive_expect_tx(&full[stage], LT_SLOT);
+            __threadfence_block();
+            *(volatile int*)(slot_tag + stage) = slot;
             bulk_load_1d(ring + stage * LT_SLOT, hbuf + (((size_t)buf * n_groups + g) * KB + kb) * (LT_KBLK / 2), LT_SLOT,
                          &full[stage]);
             if (++stage == LT_STAGES) { stage = 0; phase ^= 1; }
@@ -171,146 +128,88 @@ lstm_tc_kernel(const __grid_constant__ CUtensorMap tmW,
         __syncwarp();
       }
     }
-    if (prof && lane == 0 && blockIdx.x == 0) prof[0] = pw;
-  } else if (warp == LT_EPI_WARPS + 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(128, N);
-      mbar_wait(wbar, 0);
-      uint32_t stage = 0, phase = 0, abuf = 0;
-      for (int t = 1; t < T; ++t) {
-        for (int g = 0; g < n_groups; ++g) {
-          const uint32_t d_tmem = tmem_base + g * N;
-          for (int kb0 = 0; kb0 < KB; kb0 += LT_KG) {
-            mbar_wait(&full[stage], phase);
-            tc_fence_after();
-            if (kb0 == 0) ts_first[g] = clock64();
-            if (TS) {
-              // smem -> TMEM: LT_KG K-blocks x 8 chunks of 8 halves, then the MMAs with A in TMEM (in order on this thread's pipe)
-              const uint32_t a_tmem = tmem_base + LT_TS_ACOL + abuf * (LT_KG * 32);
-              const uint32_t slot = smem_u32(ring + stage * LT_SLOT);
-#pragma unroll
-              for (int j = 0; j < LT_KG; ++j)
-#pragma unroll
-                for (int kc = 0; kc < 8; ++kc) lt_cp_32x128b_warpx4(a_tmem + j * 32 + kc * 4, lt_desc_core(slot + j * LT_KBLK + kc * 512));
-#pragma unroll
-              for (int j = 0; j < LT_KG; ++j) {
-                const int kb = kb0 + j;
-                const uint32_t sw = smem_u32(Wsm + (size_t)kb * WBLK);
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                  lt_umma_ts(d_tmem, a_tmem + j * 32 + k * 8, make_sw128_kmajor_desc(sw + k * 32), idesc, (kb | k) != 0 ? 1u : 0u);
-              }
-              abuf ^= 1;
-            } else
-#pragma unroll
-            for (int j = 0; j < LT_KG; ++j) {
-              const int kb = kb0 + j;
-              // tile base 4g KB below the K-block: the group's 32 rows are tile rows 32g..32g+31
-              const uint32_t sa = smem_u32(ring + stage * LT_SLOT + j * LT_KBLK) - (uint32_t)g * LT_KBLK;
-              const uint32_t sw = smem_u32(Wsm + (size_t)kb * WBLK);
-#pragma unroll
-              for (int k = 0; k < 4; ++k)
-                umma_f16(d_tmem, make_sw128_kmajor_desc(sa + k * 32), make_sw128_kmajor_desc(sw + k * 32), idesc,
-                         (kb | k) != 0 ? 1u : 0u);
-            }
-            umma_commit(&empty[stage]);
-            if (++stage == LT_STAGES) { stage = 0; phase ^= 1; }
-          }
-          umma_commit(&tfull[g]);
-          ts_last[g] = clock64();
-        }
-      }
-    }
   } else {
-    // ===================== epilogue: cell update (warps g and g+4 serve group g) =====================
-    const int g = warp & 3, half = warp >> 2;
+    // ===================== consumer warpgroup g: gates = h_{t-1} W^T, then the cell update of its 32 rows =====================
+    const int g = warp >> 2, wq = warp & 3;
     if (g < n_groups) {
-      float c[HALF];
+      // accumulator (row 16 wq + lane / 4 (+8), columns 8j + 2 (lane % 4) + {0, 1}): an even lane holds gates i, f and an odd lane
+      // gates g, o of unit 2j + (lane / 2) % 2 for both rows; one exchange gives an even lane row +0 and an odd lane row +8
+      const int rr = wq * 16 + (lane >> 2) + (lane & 1) * 8;     // row of the group this thread updates (wq < 2)
+      const int n = g * 32 + rr;
+      const bool act = wq < 2 && n < B;
+      float c[UPT];
 #pragma unroll
-      for (int i = 0; i < HALF; ++i) c[i] = 0.f;
-      const int n = g * 32 + lane;
-      const bool act = n < B;
-      const int u = u0 + half * HALF;
-      long long ew = 0, ec = 0, ep = 0, pa = 0, pb = 0, pc = 0, pd = 0;
+      for (int i = 0; i < UPT; ++i) c[i] = 0.f;
+      mbar_wait(wbar, 0);
       for (int t = 0; t < T; ++t) {
-        const long long e0 = clock64();
         // tile-native layout [buf][group][K-block][32 rows][128 B], 16-byte chunks XOR-swizzled by (row & 7)
         __half* hcur = hbuf + ((size_t)(t & 1) * n_groups + g) * KB * (LT_KBLK / 2);
-        float xg[4][HALF];
+        float xg[4][UPT];
 #pragma unroll
         for (int gg = 0; gg < 4; ++gg)
 #pragma unroll
-          for (int i = 0; i < HALF; ++i)
-            xg[gg][i] = act ? xp[((long long)n * T + t) * 4 * H + (long long)gg * H + u + i] : 0.f;
-        float acc[HALF * 4];
+          for (int j = 0; j < UPT; ++j)
+            xg[gg][j] = act ? xp[((long long)n * T + t) * 4 * H + (long long)gg * H + u0 + 2 * j + ((lane >> 1) & 1)] : 0.f;
+        float acc[N / 2];
 #pragma unroll
-        for (int i = 0; i < HALF * 4; ++i) acc[i] = 0.f;
-        long long e1 = e0;
+        for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
         if (t > 0) {
-          mbar_wait(&tfull[g], (t - 1) & 1);
-          tc_fence_after();
-          e1 = clock64();
-          if (prof) {   // own publish -> all flags seen -> first h stage landed -> last MMA issued -> accumulators ready
-            const volatile long long* vf = ts_flag; const volatile long long* v1 = ts_first; const volatile long long* v2 = ts_last;
-            pa += vf[g] - e0; pb += v1[g] - vf[g]; pc += v2[g] - v1[g]; pd += e1 - v2[g];
-          }
-          const uint32_t taddr = tmem_base + ((uint32_t)(g * 32) << 16) + g * N + half * HALF * 4;
+          // ring slot index of this group's first slot of step t (the producer fills slots in (t, group, K) order)
+          const long long s0 = ((long long)(t - 1) * n_groups + g) * SLOTS;
+          for (int sidx = 0; sidx < SLOTS; ++sidx) {
+            const long long q = s0 + sidx;
+            const int stage = (int)(q % LT_STAGES);
+            unsigned spins = 0;
+            while (*(volatile int*)(slot_tag + stage) != (int)q)
+              if (++spins > (1u << 26)) asm volatile("trap;");
+            __threadfence_block();
+            mbar_wait(&full[stage], (uint32_t)((q / LT_STAGES) & 1));
+            wgmma_fence();
 #pragma unroll
-          for (int cc = 0; cc < HALF * 4; cc += 8) {
-            uint32_t r[8];
-            tmem_ld_32x32b_x8(taddr + cc, r);
-            tmem_ld_wait();
+            for (int j = 0; j < LT_KG; ++j) {
+              const int kb = sidx * LT_KG + j;
+              const uint32_t sa = smem_u32(ring + stage * LT_SLOT + j * LT_KBLK), sw = smem_u32(Wsm + (size_t)kb * WBLK);
 #pragma unroll
-            for (int e = 0; e < 8; ++e) acc[cc + e] = __uint_as_float(r[e]);
-          }
-        }
-        if (act) {
-          __half hv[HALF], lv[HALF];
-#pragma unroll
-          for (int i = 0; i < HALF; ++i) {
-            const float gi = acc[4 * i] + xg[0][i], gf = acc[4 * i + 1] + xg[1][i];
-            const float gc = acc[4 * i + 2] + xg[2][i], go = acc[4 * i + 3] + xg[3][i];
-            const float ig = lt_sigmoid(gi), fg = lt_sigmoid(gf), cg = lt_tanh(gc), og = lt_sigmoid(go);
-            const float cn = fg * c[i] + ig * cg;
-            c[i] = cn;
-            split_f16(og * lt_tanh(cn), hv[i], lv[i]);
-          }
-          const long long o = ((long long)n * T + t) * H + u;
-#pragma unroll
-          for (int i = 0; i < HALF; i += 2) {   // HALF halves are contiguous and 4-byte aligned (u0, HALF even)
-            const __half2 h2 = __halves2half2(hv[i], hv[i + 1]);
-            {
-              const int uu = u + i, kbk = uu >> 6, col = uu & 63;
-              const int off = TS ? kbk * (int)(LT_KBLK / 2) + ((((col >> 3) * 4 + (lane >> 3)) * 8 + (lane & 7)) << 3 | (col & 7))
-                                 : kbk * (int)(LT_KBLK / 2) + lane * 64 + ((((col >> 3) ^ (lane & 7)) << 3) | (col & 7));
-              *reinterpret_cast<__half2*>(hcur + off) = h2;
+              for (int k = 0; k < 4; ++k)
+                Wgmma<N>::ss(acc, make_wgmma_desc_sw128(sa + k * 32), make_wgmma_desc_sw128(sw + k * 32), 1u);
             }
-            *reinterpret_cast<__half2*>(out_hi + o + i) = h2;
-            if (out_lo) *reinterpret_cast<__half2*>(out_lo + o + i) = __halves2half2(lv[i], lv[i + 1]);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc);
+            if (lane == 0) mbar_arrive(&empty[stage]);
           }
         }
-        // publish h_t of this group: both warps of the group done (TMEM reads + h stores) -> flag
-        tc_fence_before();
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + g) : "memory");
-        const long long e2 = clock64();
-        if (half == 0 && lane == 0) {   // release is cumulative over the group's h stores ordered before it by the bar.sync
-          asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(flags + (size_t)g * G + blockIdx.x), "r"((unsigned)(t + 1))
-                       : "memory");
+        if (wq < 2) {
+          const bool odd = lane & 1;
+#pragma unroll
+          for (int j = 0; j < UPT; ++j) {
+            const float s0 = odd ? acc[4 * j] : acc[4 * j + 2], s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
+            const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+            const float a_i = odd ? r0 : acc[4 * j], a_f = odd ? r1 : acc[4 * j + 1];
+            const float a_g = odd ? acc[4 * j + 2] : r0, a_o = odd ? acc[4 * j + 3] : r1;
+            if (act) {
+              const float ig = lt_sigmoid(a_i + xg[0][j]), fg = lt_sigmoid(a_f + xg[1][j]);
+              const float cg = lt_tanh(a_g + xg[2][j]), og = lt_sigmoid(a_o + xg[3][j]);
+              const float cn = fg * c[j] + ig * cg;
+              c[j] = cn;
+              __half hv, lv;
+              split_f16(og * lt_tanh(cn), hv, lv);
+              const int uu = u0 + 2 * j + ((lane >> 1) & 1), kbk = uu >> 6, col = uu & 63;
+              hcur[kbk * (int)(LT_KBLK / 2) + rr * 64 + ((((col >> 3) ^ (rr & 7)) << 3) | (col & 7))] = hv;
+              const long long o = ((long long)n * T + t) * H + uu;
+              out_hi[o] = hv;
+              if (out_lo) out_lo[o] = lv;
+            }
+          }
+          // publish h_t of this group: both warps of the group done (h stores) -> flag
+          asm volatile("bar.sync %0, 64;" ::"r"(1 + g) : "memory");
+          if (wq == 0 && lane == 0) {   // release is cumulative over the group's h stores ordered before it by the bar.sync
+            asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(flags + (size_t)g * G + blockIdx.x), "r"((unsigned)(t + 1))
+                         : "memory");
+          }
         }
-        ew += e1 - e0; ec += e2 - e1; ep += clock64() - e2;
-      }
-      if (prof && warp == 0 && lane == 0 && blockIdx.x == 0) {
-        prof[4] = ew; prof[5] = ec; prof[6] = ep; prof[1] = pa; prof[2] = pb; prof[3] = pc; prof[7] = pd;
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == LT_EPI_WARPS + 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TCOLS);
   }
 }
 
@@ -352,30 +251,14 @@ static int lstm_tc_chunk(const float* xp, const qb_half* whh_perm, int U, int B,
   const size_t hbytes = (size_t)2 * Bp * H * 2;
   QB_CHECK_CUDA(cudaMemsetAsync(workspace, 0, hbytes + 4096, st));
   unsigned* flags = (unsigned*)((uint8_t*)workspace + hbytes);
-  static long long* prof = nullptr;
-  if (!prof && getenv("QB_LSTM_PROF")) { cudaMalloc(&prof, 64); cudaMemset(prof, 0, 64); }
-  int Bi = B, Ti = (int)T, Hi = (int)H, Bpi = Bp, ng = n_groups;
+  int Bi = B, Ti = (int)T, Hi = (int)H, ng = n_groups;
   static int poll_ns = -1;
-  if (poll_ns < 0) { const char* e = getenv("QB_LSTM_POLL_NS"); poll_ns = e ? atoi(e) : 0; }   // measured 0/16/32/64/128 ns: 11.31 / 11.41 / 11.44 / 11.49 / 11.60 us per step
-  void* args[] = {&tmW, &xp, &Bi, &Ti, &Hi, &oh, &ol, &hbuf, &flags, &Bpi, &ng, &poll_ns, &prof};
-  static int ts_mode = -1;
-  if (ts_mode < 0) { const char* e = getenv("QB_LSTM_TS"); ts_mode = e ? atoi(e) : 0; }     // 0: A operand from shared memory (product); 1: from TMEM (experiment, see above)
-  const void* fn = ts_mode ? (U == 4 ? (const void*)lstm_tc_kernel<4, true> : U == 8 ? (const void*)lstm_tc_kernel<8, true>
-                                                                                     : (const void*)lstm_tc_kernel<12, true>)
-                           : (U == 4 ? (const void*)lstm_tc_kernel<4, false> : U == 8 ? (const void*)lstm_tc_kernel<8, false>
-                                                                                      : (const void*)lstm_tc_kernel<12, false>);
+  if (poll_ns < 0) { const char* e = getenv("QB_LSTM_POLL_NS"); poll_ns = e ? atoi(e) : 0; }   // optional back-off of the flag polls
+  void* args[] = {&tmW, &xp, &Bi, &Ti, &Hi, &oh, &ol, &hbuf, &flags, &ng, &poll_ns};
+  const void* fn = U == 4 ? (const void*)lstm_tc_kernel<4> : U == 8 ? (const void*)lstm_tc_kernel<8> : (const void*)lstm_tc_kernel<12>;
   QB_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   QB_CHECK_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(LT_THREADS), args, smem, st));
   g_launches++;
-  if (prof) {
-    long long h[8];
-    cudaStreamSynchronize(st);
-    cudaMemcpy(h, prof, 64, cudaMemcpyDeviceToHost);
-    const double d = (double)Ti;
-    fprintf(stderr, "[lstm_tc prof] cycles/step (cta0): producer flag-wait %.0f | epilogue(group0) wait-acc %.0f compute %.0f publish %.0f\n"
-                    "               wait-acc split: step start -> all flags seen %.0f | -> first h stage landed %.0f | -> last MMA issued %.0f | -> accumulators ready %.0f\n",
-            h[0] / d, h[4] / d, h[5] / d, h[6] / d, h[1] / d, h[2] / d, h[3] / d, h[7] / d);
-  }
   return 0;
 }
 
@@ -386,7 +269,7 @@ extern "C" int32_t qb_lstm_tc_units(int64_t H) {
   // units per CTA: H/U CTAs must be co-resident (<= SM count) and 4U a multiple of 16
   int dev = 0, sms = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-    sms = 148;
+    sms = 132;
   for (int U : {4, 8, 12}) if (H % U == 0 && H / U <= sms) return U;
   return 0;
 }

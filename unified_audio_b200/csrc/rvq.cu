@@ -2,7 +2,7 @@
 // template HCodec-2.0/vq/core_vq.py:223-238, 394-412; upstream vector-quantize-pytorch 1.22.15).
 //
 // Encode, per layer q (strictly sequential - the residual chain):
-//   1. scores[m,j] = |e_j|^2 - 2 r_m.e_j  on the tensor cores: the tcgen05 GEMM with 3-term fp16
+//   1. scores[m,j] = |e_j|^2 - 2 r_m.e_j  on the tensor cores: the wgmma GEMM with 3-term fp16
 //      split operands (~2^-21 relative), bias = -|e|^2/2 and gamma = -2 folded into its epilogue;
 //   2. rvq_select (this file): warp per token - arg-min over the K scores; every candidate whose
 //      score lies within `tol` of the minimum is re-ranked by its EXACT squared distance in fp64

@@ -3,7 +3,7 @@
 //   HCodecTokenizer.extract_ssl_features   QuarkAudio-HCodec/HCodec-2.0/audio_tokenizer.py:47-61
 //   Model.extract_semantic_features        QuarkAudio-UniSE/model/model.py:38-51
 //   transformers HubertFeatureEncoder layer 0 (Conv1d(1, 512, k=10, s=5, bias=False) -> GroupNorm(512 groups) -> GELU)
-// Everything else of the encoders runs on the tcgen05 GEMM / attention / LayerNorm ops of this library
+// Everything else of the encoders runs on the wgmma GEMM / attention / LayerNorm ops of this library
 // (unified_audio_b200/ssl.py).
 #include <atomic>
 #include <cstdio>
@@ -113,7 +113,7 @@ __global__ void pad_wav_kernel(const float* __restrict__ x, long long T_in, long
 }
 static inline unsigned ssl_grid(long long total) {
   long long g = (total + 255) / 256;
-  return (unsigned)(g < 1 ? 1 : (g > 148 * 16 ? 148 * 16 : g));
+  return (unsigned)(g < 1 ? 1 : (g > 132 * 16 ? 132 * 16 : g));
 }
 }  // namespace qb
 using namespace qb;

@@ -9,7 +9,7 @@ state_dict keys are the reference's (HF Llama layer names under `layers.*`, `nor
 `output_head`, `adapter`, `task_embedding`, `enroll_sos_embedding`, `mix_sos_embedding`); the conformer
 condition encoder (`cond_*`, built but never executed: llm_sft.py:62-65,112-115) is accepted at load and ignored.
 
-Prefill / teacher-forced forward: tcgen05 GEMMs (3-term split) + causal split-precision flash attention over a static fp32 KV cache.
+Prefill / teacher-forced forward: wgmma GEMMs (3-term split) + causal split-precision flash attention over a static fp32 KV cache.
 Decode: fused skinny kernels (3-term fp16-split mma.sync over pre-packed weights, programmatic dependent launch; the fp32
 SIMT versions are the cross-check, QB_LM_DECODE=simt), one CUDA graph per step replayed 33 + T times; greedy (do_sample=False, the shipped
 setting U/model/model.py:173).  No PyTorch / CPU fallback for the transformer stack.
@@ -111,8 +111,7 @@ class LLM_SFT(nn.Module):
         # generate() walks a batch in chunks of <= `chunk` sequences; `lanes` > 1 runs that many chunks CONCURRENTLY, each on its own
         # CUDA stream with its own KV cache / workspace / captured graphs (the decode step is a chain of ~62 short dependent kernels:
         # one chain leaves most of the GPU idle, independent chains fill it).  Tokens do not depend on either setting.
-        # Measured on B200 (profiles/r02_lm_lanes_ab.md), 256 sequences: 851.7 ms serial, 584.9 / 513.5 / 511.0 ms with 2 / 4 / 8 lanes;
-        # cutting a batch of <= 32 into smaller chunks is slower (a chain costs the same for 8, 16 or 32 rows), hence chunk = 32.
+        # A chain costs about the same for 8, 16 or 32 rows, so a batch of <= 32 is not cut into smaller chunks: chunk = 32.
         self.lanes = max(1, int(os.environ.get("QB_LM_LANES", "4")))
         # K / V rows a lane of the decode attention keeps in flight: 8 for one chain (latency-bound), 4 on concurrent lanes
         # (throughput-bound); QB_LM_ATT_U pins it.  Fixed per decode state (it is baked into the captured graphs).
@@ -204,7 +203,7 @@ class LLM_SFT(nn.Module):
     # ------------------------------------------------------------------ transformer stack
     def _prefill(self, x: torch.Tensor, B: int, L: int, cache: StaticKVCache):
         """x [B*L, hidden] fp32, updated in place by the 12 layers; K/V written at cache.length..  cache None = a teacher-forced
-        forward that nobody will decode from: no KV cache is allocated or written (tcgen05 attention only)."""
+        forward that nobody will decode from: no KV cache is allocated or written (wgmma attention only)."""
         W = self._prepare()
         H, heads, inter, M = self.hidden, self.heads, 4 * self.hidden, B * L
         pos0 = cache.length if cache is not None else 0
@@ -223,11 +222,11 @@ class LLM_SFT(nn.Module):
         xm = rowmap(x, H, M, 0)
         lin = lambda a, w, n, K, **kw: ops.gemm(a, w, n, a_batch=1, a_rows_per_batch=M, a_ld=K, m_per_batch=M, **kw)
         # a prefill from an empty cache (every call of llm_forward / forward / generate) attends within its own L positions: the causal
-        # tcgen05 attention (csrc/attention_umma.cu) reads the qkv GEMM's output directly; lm_qkv_prep still fills the fp32 KV cache for
+        # wgmma attention (csrc/attention_umma.cu) reads the qkv GEMM's output directly; lm_qkv_prep still fills the fp32 KV cache for
         # the decode steps.  A continuation (pos0 > 0) keeps the cache-reading mma.sync kernel.
         umma = pos0 == 0 and os.environ.get("QB_ATTENTION", "umma") != "legacy"
         if cache is None and not umma:
-            raise RuntimeError("cache-less prefill needs the tcgen05 attention path")
+            raise RuntimeError("cache-less prefill needs the wgmma attention path")
         att_ws = self._buf("att5_ws", (ops.attention_umma_workspace_bytes(B, L, heads, 64, True),), torch.uint8) if umma else None
         for i, Lw in enumerate(W["layers"]):
             ops.rmsnorm(x, Lw["in_w"], M, H, t1)

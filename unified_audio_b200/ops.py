@@ -224,7 +224,7 @@ def attention_umma_workspace_bytes(B, L, heads, head_dim, split):
 
 
 def attention_umma(qkv, B, L, heads, head_dim, rope_cos, rope_sin, out: Planes, workspace, split=None, causal=False):
-    """tcgen05 attention (head_dim 64 / 128); split defaults to whether `out` carries a lo plane"""
+    """wgmma attention (head_dim 64 / 128); split defaults to whether `out` carries a lo plane"""
     split = (out.lo is not None) if split is None else split
     _lib.check(_lib.load().qb_attention_umma(_p(qkv), B, L, heads, head_dim, _p(rope_cos), _p(rope_sin), _p(out.hi), _p(out.lo),
                                              int(bool(split)), int(bool(causal)), _p(workspace), _stream()))

@@ -15,7 +15,7 @@
 Kernels: torchaudio's sinc resampler is a stride-3 41-tap FIR = a 2-tap Toeplitz GEMM over 192-sample rows; conv layer 0
 (one input channel) + per-channel GroupNorm + GELU are csrc/ssl.cu; conv layers 1-6 are TMA-im2col GEMMs with a GELU epilogue;
 the weight-normed grouped positional conv (k = 128, 16 groups) is 16 GEMMs over a group-padded buffer (`a_cols`); the 12 post-LN
-layers run on the tcgen05 GEMMs (3-term split) + the tcgen05 attention (HuBERT; WavLM's gated relative-position bias keeps the fp32 kernel).  No PyTorch / CPU fallback.
+layers run on the wgmma GEMMs (3-term split) + the wgmma attention (HuBERT; WavLM's gated relative-position bias keeps the fp32 kernel).  No PyTorch / CPU fallback.
 """
 from __future__ import annotations
 
@@ -343,7 +343,7 @@ class SSLFrontEnd(nn.Module):
             if wavlm:        # gated relative position bias from the layer INPUT (WavLMAttention.forward)
                 ops.wavlm_gate(xs, B, Tf, heads, hd, L["gru_w"], L["gru_b"], L["gru_c"], gate)
                 ops.attention_relbias(qkv, B, Tf, heads, hd, rel_table, gate, att)
-            elif umma:       # tcgen05 attention, split precision (csrc/attention_umma.cu)
+            elif umma:       # wgmma attention, split precision (csrc/attention_umma.cu)
                 ops.attention_umma(qkv, B, Tf, heads, hd, cos, sin, att, att_ws)
             else:
                 ops.attention_hd(qkv, B, Tf, heads, hd, cos, sin, att)
