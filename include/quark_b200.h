@@ -117,6 +117,10 @@ int qb_bct_to_planes(const float* x, int64_t B, int64_t C, int64_t T, qb_half* h
 int qb_layernorm(const float* x, const float* w, const float* b, float eps, int64_t B, int64_t rows, int64_t C,
                  float* out_f32, qb_half* hi, qb_half* lo, int64_t ld, int64_t rows_per_batch, int64_t row_off,
                  void* stream);
+/* qb_layernorm followed by an activation (QB_ACT_NONE or QB_ACT_GELU, exact erf): wav2vec2's conv layers with
+ * feat_extract_norm="layer" (conv -> LayerNorm over channels -> GELU). */
+int qb_layernorm_act(const float* x, const float* w, const float* b, float eps, int64_t B, int64_t rows, int64_t C, int32_t act,
+                     float* out_f32, qb_half* hi, qb_half* lo, int64_t ld, int64_t rows_per_batch, int64_t row_off, void* stream);
 /* RMSNorm (encoder_modules/transformer.py:77-96; HF LlamaRMSNorm) -> fp32 and/or planes (any may be NULL). */
 int qb_rmsnorm(const float* x, const float* w, float eps, int64_t rows, int64_t C, float* out_f32, qb_half* hi,
                qb_half* lo, void* stream);
@@ -343,6 +347,13 @@ int64_t qb_ssl_conv0_workspace_bytes(int64_t B, int64_t T0, int32_t C);
 int qb_ssl_conv0_gn_gelu(const float* x, int64_t B, int64_t T_in, const float* w, int32_t C, int32_t k, int32_t stride,
                          const float* gn_w, const float* gn_b, float eps, float* y_scratch, void* workspace, qb_half* hi,
                          qb_half* lo, int64_t ld, int64_t rows_per_batch, int64_t row_off, void* stream);
+/* wav2vec2-large-xlsr-53 (transformers Wav2Vec2Model, conv_bias=True) feature-encoder layer 0: x [B, T_in] fp32 ->
+ * Conv1d(1, C, k, stride) + bias -> y [B, T0, C] fp32, T0 = (T_in - k) / stride + 1 (LayerNorm + GELU: qb_layernorm_act). */
+int qb_ssl_conv0_bias(const float* x, int64_t B, int64_t T_in, const float* w, const float* bias, int32_t C, int32_t k,
+                      int32_t stride, float* y, void* stream);
+/* Wav2Vec2FeatureExtractor(do_normalize=True): per utterance out = (x - mean) / sqrt(var + eps), population variance,
+ * statistics in fp64 (BiCodecTokenizer.extract_wav2vec2_features, QuarkAudio-UniSE/model/bicodec/audio_tokenizer.py:74-90). */
+int qb_wav_normalize(const float* x, int64_t B, int64_t T, float eps, float* out, void* stream);
 /* WavLM-base-plus attention (transformers modeling_wavlm.WavLMAttention as UniSE drives it, U/model/model.py:30,38-51):
  * gate[b, h, t] = ga (gb const_h - 1) + 2, (ga, gb) = sigmoid of the two 4-sums of Linear(head_dim -> 8)(x[b, t, head h]);
  * qb_attention_relbias: softmax(q k^T / sqrt(d) + gate[b, h, i] * rel_table[h, (j - i) + T - 1]) v, no rotary embedding;

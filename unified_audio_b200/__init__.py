@@ -23,5 +23,5 @@ from .rvq import ResidualVQ  # noqa: E402,F401
 from .llm import LLM_SFT  # noqa: E402,F401
 from .bicodec import BiCodec  # noqa: E402,F401
 from . import adaptive  # noqa: E402,F401
-from .ssl import HCodecTokenizer, HUBERT_BASE, SSLFrontEnd, WAVLM_BASE_PLUS, pad_wav, wrap_segments  # noqa: E402,F401
+from .ssl import HCodecTokenizer, HUBERT_BASE, SSLFrontEnd, WAV2VEC2_XLSR53, WAVLM_BASE_PLUS, pad_wav, wrap_segments  # noqa: E402,F401
 from . import unise  # noqa: E402,F401

@@ -62,6 +62,7 @@ SIGNATURES = {
     "qb_rows_to_planes": (C.c_int, [_vp, _i64, _i64, _i64, _i32, _i32, _vp, _vp, _i64, _i64, _i64, _vp]),
     "qb_bct_to_planes": (C.c_int, [_vp, _i64, _i64, _i64, _vp, _vp, _i64, _i64, _i64, _vp]),
     "qb_layernorm": (C.c_int, [_vp, _vp, _vp, _f32, _i64, _i64, _i64, _vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "qb_layernorm_act": (C.c_int, [_vp, _vp, _vp, _f32, _i64, _i64, _i64, _i32, _vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "qb_rmsnorm": (C.c_int, [_vp, _vp, _f32, _i64, _i64, _vp, _vp, _vp, _vp]),
     "qb_dwconv7_ln": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp]),
     "qb_dwconv7_adaln": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp]),
@@ -106,6 +107,8 @@ SIGNATURES = {
     "qb_lm_head_argmax_tc": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "qb_ssl_conv0_workspace_bytes": (C.c_int64, [_i64, _i64, _i32]),
     "qb_ssl_conv0_gn_gelu": (C.c_int, [_vp, _i64, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "qb_ssl_conv0_bias": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "qb_wav_normalize": (C.c_int, [_vp, _i64, _i64, _f32, _vp, _vp]),
     "qb_wavlm_gate": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "qb_attention_relbias": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "qb_axpy": (C.c_int, [_vp, _f32, _i64, _i32, _vp, _vp]),

@@ -60,6 +60,8 @@ __global__ void bct_to_planes_kernel(const float* __restrict__ x, int C, int T, 
 }
 
 // ------------------------------------------------------------------ LayerNorm / RMSNorm (warp per row)
+// ACT = QB_ACT_GELU applies the exact GELU after the affine (wav2vec2's conv layers: conv -> LayerNorm over channels -> GELU)
+template <int ACT>
 __global__ void layernorm_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bz,
                                  float eps, long long rows_total, int rows, int C, float* __restrict__ out,
                                  __half* __restrict__ hi, __half* __restrict__ lo, long long ld, long long rpb,
@@ -80,6 +82,7 @@ __global__ void layernorm_kernel(const float* __restrict__ x, const float* __res
   bz += b * wb_bstride;
   for (int c = lane; c < C; c += 32) {
     float v = (xr[c] - mean) * rstd * w[c] + bz[c];
+    if (ACT == QB_ACT_GELU) v = gelu_erf(v);
     if (out) out[row * C + c] = v;
     if (hi) store_planes(hi, lo, o + c, v);
   }
@@ -542,8 +545,24 @@ extern "C" int qb_layernorm(const float* x, const float* w, const float* b, floa
   QB_REQUIRE(x && w && b && (out_f32 || hi), "layernorm: bad args");
   QB_REQUIRE(!hi || (C <= ld && row_off + rows <= rows_per_batch), "layernorm: plane buffer too small");
   const long long total = B * rows;
-  layernorm_kernel<<<(unsigned)ceil_div(total, 8), 256, 0, (cudaStream_t)stream>>>(
+  layernorm_kernel<QB_ACT_NONE><<<(unsigned)ceil_div(total, 8), 256, 0, (cudaStream_t)stream>>>(
       x, w, b, eps, total, (int)rows, (int)C, out_f32, (__half*)hi, (__half*)lo, ld, rows_per_batch, row_off, 0);
+  QB_LAUNCH_END();
+}
+
+extern "C" int qb_layernorm_act(const float* x, const float* w, const float* b, float eps, int64_t B, int64_t rows, int64_t C,
+                                int32_t act, float* out_f32, qb_half* hi, qb_half* lo, int64_t ld, int64_t rows_per_batch,
+                                int64_t row_off, void* stream) {
+  QB_REQUIRE(x && w && b && (out_f32 || hi), "layernorm_act: bad args");
+  QB_REQUIRE(act == QB_ACT_NONE || act == QB_ACT_GELU, "layernorm_act: activation %d unsupported (none / gelu)", act);
+  QB_REQUIRE(!hi || (C <= ld && row_off + rows <= rows_per_batch), "layernorm_act: plane buffer too small");
+  const long long total = B * rows;
+  if (act == QB_ACT_GELU)
+    layernorm_kernel<QB_ACT_GELU><<<(unsigned)ceil_div(total, 8), 256, 0, (cudaStream_t)stream>>>(
+        x, w, b, eps, total, (int)rows, (int)C, out_f32, (__half*)hi, (__half*)lo, ld, rows_per_batch, row_off, 0);
+  else
+    layernorm_kernel<QB_ACT_NONE><<<(unsigned)ceil_div(total, 8), 256, 0, (cudaStream_t)stream>>>(
+        x, w, b, eps, total, (int)rows, (int)C, out_f32, (__half*)hi, (__half*)lo, ld, rows_per_batch, row_off, 0);
   QB_LAUNCH_END();
 }
 
@@ -553,7 +572,7 @@ extern "C" int qb_adalayernorm(const float* x, const float* scale, const float* 
   QB_REQUIRE(x && scale && shift && (out_f32 || hi), "adalayernorm: bad args");
   QB_REQUIRE(!hi || (C <= ld && row_off + rows <= rows_per_batch), "adalayernorm: plane buffer too small");
   const long long total = B * rows;
-  layernorm_kernel<<<(unsigned)ceil_div(total, 8), 256, 0, (cudaStream_t)stream>>>(
+  layernorm_kernel<QB_ACT_NONE><<<(unsigned)ceil_div(total, 8), 256, 0, (cudaStream_t)stream>>>(
       x, scale, shift, eps, total, (int)rows, (int)C, out_f32, (__half*)hi, (__half*)lo, ld, rows_per_batch, row_off,
       cond_stride);
   QB_LAUNCH_END();

@@ -3,6 +3,8 @@
 //   HCodecTokenizer.extract_ssl_features   QuarkAudio-HCodec/HCodec-2.0/audio_tokenizer.py:47-61
 //   Model.extract_semantic_features        QuarkAudio-UniSE/model/model.py:38-51
 //   transformers HubertFeatureEncoder layer 0 (Conv1d(1, 512, k=10, s=5, bias=False) -> GroupNorm(512 groups) -> GELU)
+//   Wav2Vec2FeatureExtractor(do_normalize=True) and Wav2Vec2 (feat_extract_norm="layer") layer 0: Conv1d(1, 512, k=10, s=5) + bias;
+//   its LayerNorm over channels + GELU is qb_layernorm_act (elementwise.cu)
 // Everything else of the encoders runs on the wgmma GEMM / attention / LayerNorm ops of this library
 // (unified_audio_b200/ssl.py).
 #include <atomic>
@@ -15,12 +17,12 @@ namespace qb {
 extern std::atomic<long long> g_launches;
 
 // ---- conv layer 0: one input channel.  Block = SSL_TT output frames x all C channels; thread c keeps w[c][0..k) in registers;
-// writes y [B, T0, C] fp32 (channel-last, coalesced over c) and fp64 per-(block, channel) partial sums for the per-channel
-// GroupNorm over time (deterministic: partials are reduced in a fixed order by ssl_gn_stats_kernel).
+// writes y [B, T0, C] fp32 (channel-last, coalesced over c), plus bias[c] when given, and (part != NULL) fp64 per-(block, channel)
+// partial sums for the per-channel GroupNorm over time (deterministic: partials are reduced in a fixed order by ssl_gn_stats_kernel).
 constexpr int SSL_TT = 64, SSL_KMAX = 16;
 __global__ void __launch_bounds__(512)
-ssl_conv0_kernel(const float* __restrict__ x, long long x_stride, int T_in, const float* __restrict__ w, int C, int k, int s, int T0,
-                 float* __restrict__ y, double* __restrict__ part) {
+ssl_conv0_kernel(const float* __restrict__ x, long long x_stride, int T_in, const float* __restrict__ w, const float* __restrict__ bias,
+                 int C, int k, int s, int T0, float* __restrict__ y, double* __restrict__ part) {
   extern __shared__ float xs[];                         // (SSL_TT - 1) * s + k input samples
   const int b = blockIdx.y, t0 = blockIdx.x * SSL_TT;
   const int nt = min(SSL_TT, T0 - t0), need = (nt - 1) * s + k;
@@ -33,9 +35,10 @@ ssl_conv0_kernel(const float* __restrict__ x, long long x_stride, int T_in, cons
     float wr[SSL_KMAX];
 #pragma unroll
     for (int j = 0; j < SSL_KMAX; ++j) wr[j] = j < k ? w[c * k + j] : 0.f;
+    const float b0 = bias ? bias[c] : 0.f;
     double sum = 0.0, sq = 0.0;
     for (int t = 0; t < nt; ++t) {
-      float acc = 0.f;
+      float acc = b0;
 #pragma unroll
       for (int j = 0; j < SSL_KMAX; ++j)
         if (j < k) acc = fmaf(wr[j], xs[t * s + j], acc);
@@ -43,8 +46,10 @@ ssl_conv0_kernel(const float* __restrict__ x, long long x_stride, int T_in, cons
       sum += acc;
       sq += (double)acc * acc;
     }
-    double* p = part + (((long long)b * gridDim.x + blockIdx.x) * C + c) * 2;
-    p[0] = sum; p[1] = sq;
+    if (part) {
+      double* p = part + (((long long)b * gridDim.x + blockIdx.x) * C + c) * 2;
+      p[0] = sum; p[1] = sq;
+    }
   }
 }
 __global__ void ssl_gn_stats_kernel(const double* __restrict__ part, int nblk, int C, int T0, float eps, float* __restrict__ stats) {
@@ -76,6 +81,34 @@ __global__ void ssl_gn_gelu_kernel(const float* __restrict__ y, const float* __r
     hi[o] = h;
     if (lo) lo[o] = l;
   }
+}
+
+// ---- Wav2Vec2FeatureExtractor.zero_mean_unit_var_norm: one block per utterance, two-pass fp64 statistics (population variance)
+// reduced in a fixed order, out = (x - mean) / sqrt(var + eps) rounded once to fp32.
+constexpr int WN_THREADS = 1024;
+__device__ double block_sum_f64(double v, double* red) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if (lane == 0) red[wid] = v;
+  __syncthreads();
+  double t = 0.0;
+  for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i];
+  __syncthreads();
+  return t;
+}
+__global__ void __launch_bounds__(WN_THREADS)
+wav_normalize_kernel(const float* __restrict__ x, long long T, double eps, float* __restrict__ out) {
+  __shared__ double red[WN_THREADS / 32];
+  const float* xb = x + (long long)blockIdx.x * T;
+  float* ob = out + (long long)blockIdx.x * T;
+  double s = 0.0;
+  for (long long i = threadIdx.x; i < T; i += blockDim.x) s += xb[i];
+  const double mean = block_sum_f64(s, red) / (double)T;
+  double q = 0.0;
+  for (long long i = threadIdx.x; i < T; i += blockDim.x) { const double d = xb[i] - mean; q += d * d; }
+  const double inv = 1.0 / sqrt(block_sum_f64(q, red) / (double)T + eps);
+  for (long long i = threadIdx.x; i < T; i += blockDim.x) ob[i] = (float)((xb[i] - mean) * inv);
 }
 
 // out (+)= scale * x  (running mean of the encoder's hidden states, audio_tokenizer.py:55)
@@ -135,12 +168,34 @@ extern "C" int qb_ssl_conv0_gn_gelu(const float* x, int64_t B, int64_t T_in, con
   float* stats = (float*)((uint8_t*)workspace + (size_t)B * nblk * C * 2 * 8);
   dim3 grid((unsigned)nblk, (unsigned)B);
   const size_t smem = ((size_t)(SSL_TT - 1) * stride + k) * 4;
-  ssl_conv0_kernel<<<grid, 512, smem, st>>>(x, T_in, (int)T_in, w, C, k, stride, (int)T0, y_scratch, part);
+  ssl_conv0_kernel<<<grid, 512, smem, st>>>(x, T_in, (int)T_in, w, nullptr, C, k, stride, (int)T0, y_scratch, part);
   ssl_gn_stats_kernel<<<dim3((unsigned)ceil_div(C, 128), (unsigned)B), 128, 0, st>>>(part, nblk, C, (int)T0, eps, stats);
   const long long total = B * T0 * C;
   ssl_gn_gelu_kernel<<<ssl_grid(total), 256, 0, st>>>(y_scratch, stats, gn_w, gn_b, T0, C, (__half*)hi, (__half*)lo, ld, rows_per_batch,
                                                      row_off, total);
   g_launches += 3;
+  QB_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int qb_ssl_conv0_bias(const float* x, int64_t B, int64_t T_in, const float* w, const float* bias, int32_t C, int32_t k,
+                                 int32_t stride, float* y, void* stream) {
+  QB_REQUIRE(x && w && bias && y && B >= 1 && C >= 1, "ssl_conv0_bias: bad args");
+  QB_REQUIRE(k >= 1 && k <= SSL_KMAX && stride >= 1 && T_in >= k, "ssl_conv0_bias: kernel size %d unsupported (<= %d)", k, SSL_KMAX);
+  const int64_t T0 = (T_in - k) / stride + 1;
+  dim3 grid((unsigned)ceil_div(T0, SSL_TT), (unsigned)B);
+  const size_t smem = ((size_t)(SSL_TT - 1) * stride + k) * 4;
+  ssl_conv0_kernel<<<grid, 512, smem, (cudaStream_t)stream>>>(x, T_in, (int)T_in, w, bias, C, k, stride, (int)T0, y, nullptr);
+  g_launches++;
+  QB_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int qb_wav_normalize(const float* x, int64_t B, int64_t T, float eps, float* out, void* stream) {
+  QB_REQUIRE(x && out && B >= 0 && T >= 1, "wav_normalize: bad args");
+  if (B == 0) return 0;
+  wav_normalize_kernel<<<(unsigned)B, WN_THREADS, 0, (cudaStream_t)stream>>>(x, T, (double)eps, out);
+  g_launches++;
   QB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

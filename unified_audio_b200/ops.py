@@ -111,6 +111,17 @@ def layernorm(x, w, b, B, rows, Cc, eps=1e-6, out_f32=None, out: Optional[Planes
                                         rows_per_batch, row_off, _stream()))
 
 
+def layernorm_act(x, w, b, B, rows, Cc, act, eps=1e-5, out_f32=None, out: Optional[Planes] = None, ld=0, rows_per_batch=0,
+                  row_off=0):
+    """layernorm followed by `act` (ACT_NONE / ACT_GELU)"""
+    hi = out.hi if out is not None else None
+    lo = out.lo if out is not None else None
+    if out is not None and ld == 0:
+        ld, rows_per_batch, row_off = Cc, rows, 0
+    _lib.check(_lib.load().qb_layernorm_act(_p(x), _p(w), _p(b), eps, B, rows, Cc, act, _p(out_f32), _p(hi), _p(lo), ld,
+                                            rows_per_batch, row_off, _stream()))
+
+
 def rmsnorm(x, w, rows, Cc, out: Optional[Planes] = None, eps=1e-6, out_f32=None):
     hi = out.hi if out is not None else None
     lo = out.lo if out is not None else None
@@ -333,6 +344,18 @@ def ssl_conv0_gn_gelu(x, w, gn_w, gn_b, eps, k, stride, out: Planes, ld, rows_pe
 
 def ssl_conv0_workspace_bytes(B, T0, Cc):
     return int(_lib.load().qb_ssl_conv0_workspace_bytes(B, T0, Cc))
+
+
+def ssl_conv0_bias(x, w, bias, k, stride, y):
+    """x [B, T_in] -> y [B, T0, C] = Conv1d(1, C, k, stride)(x) + bias, channel-last"""
+    B, T_in = x.shape
+    _lib.check(_lib.load().qb_ssl_conv0_bias(_p(x), B, T_in, _p(w), _p(bias), w.shape[0], k, stride, _p(y), _stream()))
+
+
+def wav_normalize(x, eps, out):
+    """per row: (x - mean) / sqrt(var + eps) (Wav2Vec2FeatureExtractor, do_normalize=True)"""
+    B, T = x.shape
+    _lib.check(_lib.load().qb_wav_normalize(_p(x), B, T, float(eps), _p(out), _stream()))
 
 
 def wavlm_gate(x, B, T, heads, head_dim, w, bias, cst, gate):

@@ -5,17 +5,25 @@
         mean of the 13 hidden states -> sign(x) |x|^0.3                                       [B, T50, 768]
     HCodecTokenizer.pad_wav / tokenize      audio_tokenizer.py:63-75
     Model.extract_semantic_features         QuarkAudio-UniSE/model/model.py:38-51  (WavLM-base-plus, no compression)
+    BiCodecTokenizer.extract_wav2vec2_features   QuarkAudio-UniSE/model/bicodec/audio_tokenizer.py:74-90
+        Wav2Vec2FeatureExtractor(do_normalize=True) -> wav2vec2-large-xlsr-53 (no padding) ->
+        (hidden_states[11] + hidden_states[14] + hidden_states[16]) / 3                       [B, T', 1024]
     wrap padding + 5 s segmenting           QuarkAudio-UniSE/model/model.py:175-181
 
 `SSLFrontEnd(config)` holds the parameters under the key names of `transformers.HubertModel` / `WavLMModel`
 (`feature_extractor.conv_layers.{i}.conv.weight`, `feature_projection.*`, `encoder.pos_conv_embed.conv.parametrizations.weight.*`,
 `encoder.layers.{i}.attention.{q,k,v,out}_proj.*`, `feed_forward.*`, `layer_norm`, `final_layer_norm`; WavLM adds
-`attention.gru_rel_pos_*` and `encoder.layers.0.attention.rel_attn_embed.weight`), so a checkpoint's state-dict loads as is.
+`attention.gru_rel_pos_*` and `encoder.layers.0.attention.rel_attn_embed.weight`; `transformers.Wav2Vec2Model` adds
+`feature_extractor.conv_layers.{i}.conv.bias` and `.layer_norm.*` for every conv), so a checkpoint's state-dict loads as is.
 
 Kernels: torchaudio's sinc resampler is a stride-3 41-tap FIR = a 2-tap Toeplitz GEMM over 192-sample rows; conv layer 0
 (one input channel) + per-channel GroupNorm + GELU are csrc/ssl.cu; conv layers 1-6 are TMA-im2col GEMMs with a GELU epilogue;
 the weight-normed grouped positional conv (k = 128, 16 groups) is 16 GEMMs over a group-padded buffer (`a_cols`); the 12 post-LN
-layers run on the wgmma GEMMs (3-term split) + the wgmma attention (HuBERT; WavLM's gated relative-position bias keeps the fp32 kernel).  No PyTorch / CPU fallback.
+layers run on the wgmma GEMMs (3-term split) + the wgmma attention (HuBERT; WavLM's gated relative-position bias keeps the fp32 kernel).
+wav2vec2 (feat_extract_norm="layer", do_stable_layer_norm=True): the processor normalisation (fp64 statistics) and conv layer 0 +
+bias are csrc/ssl.cu, every conv is followed by LayerNorm over channels + GELU (qb_layernorm_act) written as planes of the next
+conv's buffer, and the pre-LN layers run up to the last hidden state the output needs (layers 17-24 and `encoder.layer_norm` of
+XLSR-53 are loaded but never computed).  No PyTorch / CPU fallback.
 """
 from __future__ import annotations
 
@@ -33,16 +41,23 @@ from .ops import ACT_GELU, Planes, rowmap
 HUBERT_BASE = dict(conv_dim=[512] * 7, conv_kernel=[10, 3, 3, 3, 3, 2, 2], conv_stride=[5, 2, 2, 2, 2, 2, 2], hidden=768,
                    layers=12, heads=12, ffn=3072, pos_k=128, pos_groups=16, eps=1e-5, kind="hubert")
 WAVLM_BASE_PLUS = dict(HUBERT_BASE, num_buckets=320, max_distance=800, kind="wavlm")
+# facebook/wav2vec2-large-xlsr-53 as BiCodec's tokenizer uses it: hidden_state_ids are the averaged hidden states (0 = the
+# positional-conv output, k = the residual stream after layer k), do_normalize the feature extractor's per-utterance normalisation
+WAV2VEC2_XLSR53 = dict(HUBERT_BASE, hidden=1024, layers=24, heads=16, ffn=4096, kind="wav2vec2", hidden_state_ids=(11, 14, 16),
+                       do_normalize=True)
 
 
 def ssl_spec(c: dict) -> Dict[str, tuple]:
     out: Dict[str, tuple] = {}
     cin = 1
+    w2v = c.get("kind") == "wav2vec2"
     for i, (co, k) in enumerate(zip(c["conv_dim"], c["conv_kernel"])):
         out[f"feature_extractor.conv_layers.{i}.conv.weight"] = (co, cin, k)
-        if i == 0:
-            out["feature_extractor.conv_layers.0.layer_norm.weight"] = (co,)
-            out["feature_extractor.conv_layers.0.layer_norm.bias"] = (co,)
+        if w2v:                                 # conv_bias=True, feat_extract_norm="layer"
+            out[f"feature_extractor.conv_layers.{i}.conv.bias"] = (co,)
+        if i == 0 or w2v:
+            out[f"feature_extractor.conv_layers.{i}.layer_norm.weight"] = (co,)
+            out[f"feature_extractor.conv_layers.{i}.layer_norm.bias"] = (co,)
         cin = co
     H = c["hidden"]
     out["feature_projection.layer_norm.weight"] = (cin,)
@@ -94,10 +109,14 @@ def resample_kernel(orig: int, new: int, lowpass_filter_width: int = 6, rolloff:
 
 class SSLFrontEnd(nn.Module):
     def __init__(self, config: Optional[dict] = None, in_rate: int = 16000, compress: bool = False):
-        """config: HUBERT_BASE / WAVLM_BASE_PLUS (or a reduced dict of the same keys).  in_rate 48000 adds the tokenizer's
-        Resample(48k -> 16k); compress adds sign(x)|x|^0.3 (H-Codec tokenizer) - UniSE uses neither."""
+        """config: HUBERT_BASE / WAVLM_BASE_PLUS / WAV2VEC2_XLSR53 (or a reduced dict of the same keys).  in_rate 48000 adds the
+        tokenizer's Resample(48k -> 16k); compress adds sign(x)|x|^0.3 (H-Codec tokenizer) - UniSE and BiCodec use neither."""
         super().__init__()
         self.cfg = dict(config or HUBERT_BASE)
+        if self.cfg.get("kind") == "wav2vec2":
+            ids = self.cfg["hidden_state_ids"]
+            if not ids or min(ids) < 0 or max(ids) >= self.cfg["layers"]:
+                raise ValueError(f"hidden_state_ids {ids} must lie in [0, layers) (the last state carries encoder.layer_norm)")
         self.in_rate, self.compress = in_rate, compress
         tree = _Tree.build(ssl_spec(self.cfg))
         for name, child in tree.named_children():
@@ -165,9 +184,15 @@ class SSLFrontEnd(nn.Module):
             for j in range(64):
                 wt[j, o * j: o * j + kern.shape[1]] = kern[0].double()
             W["resample"] = dict(w=Planes.from_f32(wt.float().to(dev), True), width=width, o=o, R=R, k=kern.shape[1])
+        w2v = c.get("kind") == "wav2vec2"
+        nconv = len(c["conv_dim"])
         W["conv0_w"] = f32("feature_extractor.conv_layers.0.conv.weight").reshape(c["conv_dim"][0], -1).contiguous()
         W["gn_w"], W["gn_b"] = f32("feature_extractor.conv_layers.0.layer_norm.weight"), f32("feature_extractor.conv_layers.0.layer_norm.bias")
-        W["convs"] = [conv_w(sd[f"feature_extractor.conv_layers.{i}.conv.weight"]) for i in range(1, len(c["conv_dim"]))]
+        W["convs"] = [conv_w(sd[f"feature_extractor.conv_layers.{i}.conv.weight"]) for i in range(1, nconv)]
+        if w2v:
+            W["conv_b"] = [f32(f"feature_extractor.conv_layers.{i}.conv.bias") for i in range(nconv)]
+            W["conv_ln"] = [(f32(f"feature_extractor.conv_layers.{i}.layer_norm.weight"), f32(f"feature_extractor.conv_layers.{i}.layer_norm.bias"))
+                            for i in range(nconv)]
         W["fp_ln_w"], W["fp_ln_b"] = f32("feature_projection.layer_norm.weight"), f32("feature_projection.layer_norm.bias")
         W["fp_w"], W["fp_b"] = Planes.from_f32(sd["feature_projection.projection.weight"], True), f32("feature_projection.projection.bias")
         # weight-normed grouped positional conv: w = g * v / ||v|| (norm over (out, in) per tap); per group [Cg, k * 64] planes
@@ -183,7 +208,7 @@ class SSLFrontEnd(nn.Module):
         W["pos_b"] = f32("encoder.pos_conv_embed.conv.bias")
         W["enc_ln_w"], W["enc_ln_b"] = f32("encoder.layer_norm.weight"), f32("encoder.layer_norm.bias")
         layers = []
-        for i in range(c["layers"]):
+        for i in range(max(c["hidden_state_ids"]) if w2v else c["layers"]):     # wav2vec2: layers past the last state used are dead
             p = f"encoder.layers.{i}."
             wqkv = torch.cat([sd[p + f"attention.{n}_proj.weight"] for n in "qkv"], 0)
             L = dict(wqkv=Planes.from_f32(wqkv, True), bqkv=torch.cat([sd[p + f"attention.{n}_proj.bias"] for n in "qkv"], 0).contiguous(),
@@ -230,6 +255,43 @@ class SSLFrontEnd(nn.Module):
             self._ws[key] = r
         return r
 
+    def _embed(self, feats: torch.Tensor, B: int, Tf: int, taps: Optional[dict] = None) -> torch.Tensor:
+        """conv features [B * Tf, Cf] -> feature projection (LayerNorm -> Linear) -> x + GELU(positional conv(x)) [B * Tf, H]"""
+        W = self._w
+        c = self.cfg
+        Cf, H = c["conv_dim"][-1], c["hidden"]
+        M = B * Tf
+        if taps is not None:
+            taps["features"] = feats.reshape(B, Tf, Cf).clone()
+        # ---- feature projection: LayerNorm -> Linear
+        cfp = _pad_to(Cf, 64)
+        pn = self._planes("fp_in", (M, cfp))
+        ops.layernorm(feats, W["fp_ln_w"], W["fp_ln_b"], B, Tf, Cf, eps=c["eps"], out=pn, ld=cfp, rows_per_batch=Tf, row_off=0)
+        wfp = W.get("fp_w_pad")
+        if wfp is None:
+            w = torch.zeros(H, cfp, device=self._dev())
+            w[:, :Cf] = self.feature_projection.projection.weight.detach().float()
+            wfp = W["fp_w_pad"] = Planes.from_f32(w, True)
+        xh = self._buf("x", (M, H))
+        # projected features also go, group-padded, into the positional conv's zero-padded buffer
+        ops.gemm(pn, wfp, H, a_batch=1, a_rows_per_batch=M, a_ld=cfp, m_per_batch=M, bias=W["fp_b"], out_f32=rowmap(xh, H, M, 0))
+        # ---- positional conv embedding: x + GELU(conv_k128_g16(x))  (HubertPositionalConvEmbedding + SamePad)
+        G, K = c["pos_groups"], c["pos_k"]
+        cg = H // G
+        pad_l = K // 2
+        rows_p = Tf + K                                       # pad_l zeros in front, K - pad_l (>= needed K - 1 - pad_l) behind
+        pbuf = self._planes("pos_in", (B, rows_p, G * 64))
+        xg = self._buf("pos_xg", (M, G * 64))
+        xg.view(M, G, 64)[:, :, :cg].copy_(xh.view(M, G, cg))   # group-padded copy (device glue: strided copy, no arithmetic)
+        ops.rows_to_planes(xg, B, Tf, G * 64, pbuf, G * 64, rows_p, pad_l)
+        x1 = self._buf("x1", (M, H))
+        for g in range(G):
+            res = ops.RowMap(xh.data_ptr() + 4 * g * cg, H, Tf, 0)
+            out = ops.RowMap(x1.data_ptr() + 4 * g * cg, H, Tf, 0)
+            ops.gemm(pbuf, W["pos_w"][g], cg, a_batch=B, a_rows_per_batch=rows_p, a_ld=G * 64, m_per_batch=Tf, taps=K,
+                     a_cols=64, a_col_off=64 * g, bias=W["pos_b"][g * cg:(g + 1) * cg], act=ACT_GELU, residual=res, out_f32=out)
+        return x1
+
     # ------------------------------------------------------------------ stages
     def resample(self, wav: torch.Tensor) -> torch.Tensor:
         """torchaudio.transforms.Resample(in_rate, 16000) (audio_tokenizer.py:41,50): wav [B,T] -> [B, ceil(T / 3)]"""
@@ -252,9 +314,12 @@ class SSLFrontEnd(nn.Module):
 
     def hidden_state_mean(self, wav16: torch.Tensor, taps: Optional[dict] = None) -> torch.Tensor:
         """pad 160/160 -> feature encoder -> projection -> positional conv -> encoder; returns the mean of the
-        1 + layers hidden states [B, T', H] fp32 (audio_tokenizer.py:51-55 / model.py:43-46)."""
+        1 + layers hidden states [B, T', H] fp32 (audio_tokenizer.py:51-55 / model.py:43-46).  wav2vec2: no padding, the mean of
+        the `hidden_state_ids` states (bicodec/audio_tokenizer.py:85-88)."""
         W = self._prepare()
         c = self.cfg
+        if c.get("kind") == "wav2vec2":
+            return self._wav2vec2_mean(wav16, taps)
         B, T = wav16.shape
         x = ops.pad_wav(wav16, 160, T + 320)
         Tin = T + 320
@@ -286,37 +351,9 @@ class SSLFrontEnd(nn.Module):
                          act=ACT_GELU, out_planes=nxt, out_planes_map=(_pad_to(co, 64), rpb_n, 0))
                 cur, rpb, cin_pad = nxt, rpb_n, _pad_to(co, 64)
             Tc = Tn
-        Tf, Cf, H = Tc, c["conv_dim"][-1], c["hidden"]
+        Tf, H = Tc, c["hidden"]
         M = B * Tf
-        if taps is not None:
-            taps["features"] = feats.reshape(B, Tf, Cf).clone()
-        # ---- feature projection: LayerNorm -> Linear
-        cfp = _pad_to(Cf, 64)
-        pn = self._planes("fp_in", (M, cfp))
-        ops.layernorm(feats, W["fp_ln_w"], W["fp_ln_b"], B, Tf, Cf, eps=c["eps"], out=pn, ld=cfp, rows_per_batch=Tf, row_off=0)
-        wfp = W.get("fp_w_pad")
-        if wfp is None:
-            w = torch.zeros(H, cfp, device=self._dev())
-            w[:, :Cf] = self.feature_projection.projection.weight.detach().float()
-            wfp = W["fp_w_pad"] = Planes.from_f32(w, True)
-        xh = self._buf("x", (M, H))
-        # projected features also go, group-padded, into the positional conv's zero-padded buffer
-        ops.gemm(pn, wfp, H, a_batch=1, a_rows_per_batch=M, a_ld=cfp, m_per_batch=M, bias=W["fp_b"], out_f32=rowmap(xh, H, M, 0))
-        # ---- positional conv embedding: x + GELU(conv_k128_g16(x))  (HubertPositionalConvEmbedding + SamePad)
-        G, K = c["pos_groups"], c["pos_k"]
-        cg = H // G
-        pad_l = K // 2
-        rows_p = Tf + K                                       # pad_l zeros in front, K - pad_l (>= needed K - 1 - pad_l) behind
-        pbuf = self._planes("pos_in", (B, rows_p, G * 64))
-        xg = self._buf("pos_xg", (M, G * 64))
-        xg.view(M, G, 64)[:, :, :cg].copy_(xh.view(M, G, cg))   # group-padded copy (device glue: strided copy, no arithmetic)
-        ops.rows_to_planes(xg, B, Tf, G * 64, pbuf, G * 64, rows_p, pad_l)
-        x1 = self._buf("x1", (M, H))
-        for g in range(G):
-            res = ops.RowMap(xh.data_ptr() + 4 * g * cg, H, Tf, 0)
-            out = ops.RowMap(x1.data_ptr() + 4 * g * cg, H, Tf, 0)
-            ops.gemm(pbuf, W["pos_w"][g], cg, a_batch=B, a_rows_per_batch=rows_p, a_ld=G * 64, m_per_batch=Tf, taps=K,
-                     a_cols=64, a_col_off=64 * g, bias=W["pos_b"][g * cg:(g + 1) * cg], act=ACT_GELU, residual=res, out_f32=out)
+        x1 = self._embed(feats, B, Tf, taps)
         xs = self._buf("xs", (M, H))
         xp = self._planes("xp", (M, H))
         ops.layernorm(x1, W["enc_ln_w"], W["enc_ln_b"], B, Tf, H, eps=c["eps"], out_f32=xs, out=xp)
@@ -360,12 +397,97 @@ class SSLFrontEnd(nn.Module):
                 taps[f"hs{li + 1}"] = xs.reshape(B, Tf, H).clone()
         return acc.reshape(B, Tf, H)
 
+    def min_samples(self) -> int:
+        """receptive field of the conv stack: the shortest input that yields one frame (400 samples for XLSR-53)"""
+        n, hop = self.cfg["conv_kernel"][0], 1
+        for k, s in zip(self.cfg["conv_kernel"][1:], self.cfg["conv_stride"]):
+            hop *= s
+            n += (k - 1) * hop
+        return n
+
+    def _wav2vec2_mean(self, wav16: torch.Tensor, taps: Optional[dict] = None) -> torch.Tensor:
+        """Wav2Vec2Model (conv_bias, feat_extract_norm="layer", do_stable_layer_norm): feature encoder -> projection -> positional
+        conv -> pre-LN layers; returns the mean of hidden_states[k] for k in `hidden_state_ids` [B, T', H] fp32."""
+        W = self._w
+        c = self.cfg
+        B, Tin = wav16.shape
+        if Tin < self.min_samples():
+            raise ValueError(f"wav2vec2 needs at least {self.min_samples()} samples per utterance (the conv stack's receptive "
+                             f"field), got {Tin}")
+        # ---- feature encoder: conv + bias -> LayerNorm over channels -> GELU, 7 times (Wav2Vec2LayerNormConvLayer, eps 1e-5)
+        C0, k0, s0 = c["conv_dim"][0], c["conv_kernel"][0], c["conv_stride"][0]
+        Tc = (Tin - k0) // s0 + 1
+        y = self._buf("fe_y0", (B, Tc, C0))
+        ops.ssl_conv0_bias(wav16, W["conv0_w"], W["conv_b"][0], k0, s0, y)
+        nconv = len(c["conv_dim"])
+        for i in range(nconv - 1):
+            co, cn, k, s = c["conv_dim"][i], c["conv_dim"][i + 1], c["conv_kernel"][i + 1], c["conv_stride"][i + 1]
+            rpb, cpad = _pad_to(Tc, s), _pad_to(co, 64)
+            cur = self._planes(f"fe{i}", (B, rpb, cpad))
+            ops.layernorm_act(y, *W["conv_ln"][i], B, Tc, co, ACT_GELU, eps=1e-5, out=cur, ld=cpad, rows_per_batch=rpb, row_off=0)
+            Tn = (Tc - k) // s + 1
+            y = self._buf(f"fe_y{i + 1}", (B, Tn, cn))
+            ops.gemm(cur, W["convs"][i], cn, a_batch=B, a_rows_per_batch=rpb, a_ld=cpad, m_per_batch=Tn, taps=k, stride=s,
+                     bias=W["conv_b"][i + 1], out_f32=rowmap(y, cn, Tn, 0))
+            Tc = Tn
+        Tf, Cf, H = Tc, c["conv_dim"][-1], c["hidden"]
+        M = B * Tf
+        feats = self._buf("fe_out", (M, Cf))
+        ops.layernorm_act(y, *W["conv_ln"][-1], B, Tf, Cf, ACT_GELU, eps=1e-5, out_f32=feats)
+        x = self._embed(feats, B, Tf, taps)                      # hidden_states[0]: no LayerNorm before the pre-LN layers
+        x2 = self._buf("x2", (M, H))
+        ids = c["hidden_state_ids"]
+        acc = self._buf("hs_sum", (M, H))
+        first = True
+        if 0 in ids:
+            ops.axpy(x, 1.0 / len(ids), acc, accumulate=False)
+            first = False
+        if taps is not None:
+            taps["hs0"] = x.reshape(B, Tf, H).clone()
+        heads, hd = c["heads"], H // c["heads"]
+        qkv = self._buf("qkv", (M, 3 * H))
+        xp = self._planes("xp", (M, H))
+        att = self._planes("att", (M, H))
+        hid = self._planes("hid", (M, c["ffn"]))
+        cos, sin = self._identity_rope(Tf, hd)
+        umma = hd in (64, 128) and os.environ.get("QB_ATTENTION", "umma") != "legacy"
+        att_ws = self._buf("att5_ws", (ops.attention_umma_workspace_bytes(B, Tf, heads, hd, True),), torch.uint8) if umma else None
+        for li, L in enumerate(W["layers"]):                      # Wav2Vec2EncoderLayerStableLayerNorm; x <-> x2 ping-pong
+            ops.layernorm(x, L["ln_w"], L["ln_b"], B, Tf, H, eps=c["eps"], out=xp)
+            ops.gemm(xp, L["wqkv"], 3 * H, a_batch=1, a_rows_per_batch=M, a_ld=H, m_per_batch=M, bias=L["bqkv"],
+                     out_f32=rowmap(qkv, 3 * H, M, 0))
+            if umma:
+                ops.attention_umma(qkv, B, Tf, heads, hd, cos, sin, att, att_ws)
+            else:
+                ops.attention_hd(qkv, B, Tf, heads, hd, cos, sin, att)
+            ops.gemm(att, L["wo"], H, a_batch=1, a_rows_per_batch=M, a_ld=H, m_per_batch=M, bias=L["bo"],
+                     residual=rowmap(x, H, M, 0), out_f32=rowmap(x2, H, M, 0))
+            ops.layernorm(x2, L["fln_w"], L["fln_b"], B, Tf, H, eps=c["eps"], out=xp)
+            ops.gemm(xp, L["w1"], c["ffn"], a_batch=1, a_rows_per_batch=M, a_ld=H, m_per_batch=M, bias=L["b1"], act=ACT_GELU,
+                     out_planes=hid, out_planes_map=(c["ffn"], M, 0))
+            ops.gemm(hid, L["w2"], H, a_batch=1, a_rows_per_batch=M, a_ld=c["ffn"], m_per_batch=M, bias=L["b2"],
+                     residual=rowmap(x2, H, M, 0), out_f32=rowmap(x, H, M, 0))
+            if li + 1 in ids:
+                ops.axpy(x, 1.0 / len(ids), acc, accumulate=not first)
+                first = False
+            if taps is not None:
+                taps[f"hs{li + 1}"] = x.reshape(B, Tf, H).clone()
+        return acc.reshape(B, Tf, H)
+
+    def normalize(self, wav: torch.Tensor) -> torch.Tensor:
+        """Wav2Vec2FeatureExtractor(do_normalize=True): each utterance to zero mean, unit (population) variance, eps 1e-7"""
+        out = torch.empty_like(wav)
+        ops.wav_normalize(wav, 1e-7, out)
+        return out
+
     @torch.no_grad()
     def forward(self, wavs: torch.Tensor, channel_first: bool = False, taps: Optional[dict] = None) -> torch.Tensor:
         """extract_ssl_features / extract_semantic_features: wavs [B, T] at `in_rate` -> [B, T', H] (or [B, H, T'])."""
         if wavs.device.type != "cuda":
             raise RuntimeError("unified_audio_b200.SSLFrontEnd runs on CUDA only (no CPU fallback)")
         w16 = self.resample(wavs.float().contiguous())
+        if self.cfg.get("do_normalize"):
+            w16 = self.normalize(w16.contiguous())
         mean = self.hidden_state_mean(w16.contiguous(), taps)
         if taps is not None:
             taps["mean"] = mean.clone()
