@@ -256,37 +256,19 @@ int qb_lm_qkv_prep(const float* qkv, int64_t B, int64_t L, int32_t heads, int32_
  * split into fp16 hi/lo planes on the fly and multiplied as 3-term split MMAs (fp32-grade scores). */
 int qb_lm_flash_attn(const float* q32, const float* k_cache, const float* v_cache, int64_t B, int64_t L,
                      int32_t heads, int32_t pos0, int32_t Lmax, qb_half* out_hi, qb_half* out_lo, void* stream);
-/* One decoder layer for ONE new token per sequence (B <= 32), fp32 weights streamed once:
- * x [B,hidden] updated in place; K/V appended at *pos (device int, not modified here).
- * wqkv = [q;k;v] rows [3*hidden, hidden]; scratch q_buf/attn_buf [B,hidden], mlp_buf [B,inter].
- * The RMSNorm weights must be FOLDED into the following projection by the caller (wqkv' = wqkv diag(in_norm),
- * wgate' / wup' likewise with post_norm): the kernels apply only the per-row 1/rms.  in_norm / post_norm are
- * passed as non-NULL flags that the normalisation is wanted. */
-int qb_lm_decode_layer(float* x, int64_t B, int32_t hidden, int32_t heads, int32_t inter, const float* in_norm,
-                       const float* wqkv, const float* wo, const float* post_norm, const float* wgate,
-                       const float* wup, const float* wdown, float* k_cache, float* v_cache, int32_t Lmax,
-                       const int32_t* pos, const float* rope_cos, const float* rope_sin, float* q_buf,
-                       float* attn_buf, float* mlp_buf, void* stream);
-/* Final RMSNorm + output head restricted to columns [range[0], range[1]) (device ints; llm_sft.py:148-153)
- * + greedy arg-max (llm.py:286-287, do_sample=False) -> out_ids[b*out_stride + slot[0]]; x_next[b] =
- * embedding[token]; then slot[0]++ and *pos++ (slot is int32[2], second word is scratch).
- * w_head must have final_norm folded in (w_head' = w_head diag(final_norm)).
- * part_val/part_idx: scratch [max_cols/16 * 32]. */
-int qb_lm_head_argmax(const float* x, int64_t B, int32_t hidden, const float* final_norm, const float* w_head,
-                      const int32_t* range, int32_t max_cols, const float* embedding, float* x_next,
-                      int64_t* out_ids, int32_t out_stride, int32_t* pos, int32_t* slot, float* part_val,
-                      int32_t* part_idx, void* stream);
-
-/* ---- tensor-core decode step (the product path; the fp32 kernels above stay as the cross-check) ----
+/* ---- KV-cache decode step ----
  * Weights are pre-packed ONCE with qb_lm_pack_weight: row-major [n][k] fp32 -> [n][k/4] 16-byte groups
  * {hi[4], lo[4]} of fp16 (hi = rn16(w), lo = rn16(w - hi)): 4 bytes / parameter like fp32, and one 16-byte load is
- * directly the B fragment of two MMA k-slots.  Same folding contract as qb_lm_decode_layer (RMSNorm weights folded
- * into wqkv / wgate / wup / w_head BEFORE packing).  Each kernel issues its weight loads before
- * `griddepcontrol.wait` and is launched as a programmatic dependent of its predecessor (works inside stream capture;
- * QB_LM_PDL=0 disables), products are 3-term fp16-split mma.sync tiles with fp32 accumulation.
+ * directly the B fragment of two MMA k-slots.  Each kernel issues its weight loads before `griddepcontrol.wait` and is
+ * launched as a programmatic dependent of its predecessor (works inside stream capture); products are 3-term
+ * fp16-split mma.sync tiles with fp32 accumulation.
  * Replaces: HF Llama decoder layer on one cached token - QuarkAudio-UniSE/model/llm/llm.py:195-228 driven by
  * llm_sft.py:155-191. */
 int qb_lm_pack_weight(const float* w, int64_t n, int64_t k, qb_half* out /* [n][2k] */, void* stream);
+/* One decoder layer for ONE new token per sequence (B <= 32): x [B,hidden] updated in place; K/V appended at *pos
+ * (device int, not modified here).  wqkv = packed [q;k;v] rows [3*hidden, hidden]; scratch q_buf/attn_buf [B,hidden],
+ * mlp_buf [B,inter].  The RMSNorm weights must be FOLDED into the following projection by the caller BEFORE packing
+ * (wqkv' = wqkv diag(in_norm), wgate' / wup' likewise with post_norm): the kernels apply only the per-row 1/rms. */
 int qb_lm_decode_layer_tc(float* x, int64_t B, int32_t hidden, int32_t heads, int32_t inter, const qb_half* wqkv,
                           const qb_half* wo, const qb_half* wgate, const qb_half* wup, const qb_half* wdown,
                           float* k_cache, float* v_cache, int32_t Lmax, const int32_t* pos, const float* rope_cos,
@@ -296,26 +278,15 @@ int qb_lm_decode_layer_tc(float* x, int64_t B, int32_t hidden, int32_t heads, in
  * read at launch (and therefore fixed inside a captured graph).  Tokens do not depend on it only up to the fp32 summation order of
  * the online softmax: set it once per decode state. */
 int qb_lm_set_att_unroll(int32_t keys_per_lane);
-/* as qb_lm_head_argmax with a packed head; max_cols and the range width must be multiples of 16;
- * part_val/part_idx: scratch [max_cols/16 * 32]. */
+/* Final RMSNorm + packed output head restricted to columns [range[0], range[1]) (device ints; llm_sft.py:148-153)
+ * + greedy arg-max (llm.py:286-287, do_sample=False) -> out_ids[b*out_stride + slot[0]]; x_next[b] =
+ * embedding[token]; then slot[0]++ and *pos++ (slot is int32[2], second word is scratch).  B <= 32.
+ * w_head must have final_norm folded in BEFORE packing (w_head' = w_head diag(final_norm)); max_cols and the range
+ * width must be multiples of 16; part_val/part_idx: scratch [max_cols/16 * 32]. */
 int qb_lm_head_argmax_tc(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
                          int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride,
                          int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx, void* stream);
 
-/* n_steps cached greedy decode steps in ONE persistent cooperative kernel (csrc/llm_step.cu): the 62 stages of a step (5 per
- * layer + head + arg-max) are separated by a device-side grid barrier instead of a kernel boundary, weights of the next tile are
- * requested before the barrier, position / output slot live in registers.  Tile arithmetic identical to
- * qb_lm_decode_layer_tc / qb_lm_head_argmax_tc (tokens bit-identical).  wqkv..wdown, k_cache, v_cache: HOST arrays of `layers`
- * device pointers (packed weights as qb_lm_pack_weight writes them, RMSNorm weights folded); x [B, hidden] = embedding of the
- * first input token on entry / of the last produced token on exit; *pos, *slot (device ints) advance by n_steps; `barrier`: one
- * device uint32 (zeroed by the call).  B <= 32; shipped LM dimensions only (hidden 512, FFN 2048).
- * Replaces the decoding loops of llm_sft.py:137-164 / 166-193 (do_sample=False). */
-int qb_lm_decode_steps(float* x, int64_t B, int32_t hidden, int32_t heads, int32_t inter, int32_t layers, const qb_half* const* wqkv,
-                       const qb_half* const* wo, const qb_half* const* wgate, const qb_half* const* wup, const qb_half* const* wdown,
-                       float* const* k_cache, float* const* v_cache, int32_t Lmax, const qb_half* w_head, const int32_t* range,
-                       int32_t max_cols, const float* embedding, const float* rope_cos, const float* rope_sin, float* q_buf,
-                       float* attn_buf, float* mlp_buf, float* part_val, int32_t* part_idx, int64_t* out_ids, int32_t out_stride,
-                       int32_t* pos, int32_t* slot, int32_t n_steps, uint32_t* barrier, void* stream);
 /* Teacher-forced loss + accuracy (CustomLlamaModel.loss_function, QuarkAudio-UniSE/model/llm/llm.py:87-104): label-smoothed KL
  * (reduction batchmean) of log_softmax(logits [M, ld >= V]) against the smoothed one-hot targets [M] int64, and the arg-max
  * accuracy -> out = {loss, accuracy}; workspace: 2*M floats.  One pass over the logits, deterministic reduction. */

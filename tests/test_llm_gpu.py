@@ -100,28 +100,24 @@ def test_lm_full_config_vs_oracle(lib):
 
 
 @pytest.mark.parametrize("B", [1, 5, 32])
-def test_lm_decode_kernels_agree(lib, B):
-    """The product decode step (packed fp16-split weights, mma.sync, programmatic dependent launch) against the
-    fp32 SIMT kernels and the oracle: cached single-token hidden states after a 40-token prefill."""
+def test_lm_decode_step_vs_oracle(lib, B):
+    """The decode step (packed fp16-split weights, mma.sync, programmatic dependent launch) against the oracle: cached
+    single-token hidden states after a 40-token prefill."""
     from oracle import llama
     cfg = llama.LM_FULL
     m, sd = build(cfg, 3, 2.0)
     g = torch.Generator().manual_seed(100 + B)
     x = torch.randn(B, 46, 512, generator=g)
     ref, _ = llama.llm_forward(sd, cfg, x)
-    outs = {}
-    for kern in ("tc", "simt"):
-        m.decode_kernel = kern
-        out = m.llm_forward(x[:, :40].cuda(), use_cache=True)
-        cache = out.past_key_values
-        hs = []
-        for i in range(40, 46):
-            hs.append(m.llm_forward(x[:, i:i + 1].cuda(), past_key_values=cache, use_cache=True).last_hidden_state)
-        torch.cuda.synchronize()
-        outs[kern] = torch.cat(hs, 1)
-    e_tc, e_simt, e_x = rel(outs["tc"], ref[:, 40:]), rel(outs["simt"], ref[:, 40:]), rel(outs["tc"], outs["simt"])
-    print(f"B={B}: decode rel vs oracle tc {e_tc:.2e} simt {e_simt:.2e}; tc vs simt {e_x:.2e}")
-    assert e_tc < TOL and e_simt < TOL and e_x < 1e-4
+    out = m.llm_forward(x[:, :40].cuda(), use_cache=True)
+    cache = out.past_key_values
+    hs = []
+    for i in range(40, 46):
+        hs.append(m.llm_forward(x[:, i:i + 1].cuda(), past_key_values=cache, use_cache=True).last_hidden_state)
+    torch.cuda.synchronize()
+    e_tc = rel(torch.cat(hs, 1), ref[:, 40:])
+    print(f"B={B}: decode rel vs oracle {e_tc:.2e}")
+    assert e_tc < TOL
 
 
 def test_lm_sampled_generate_vs_oracle(lib):
@@ -207,29 +203,6 @@ def test_lm_rope_table_grows_and_nan_safe(lib):
     gg, ss = m.generate("se", None, None, mix.cuda(), mix.cuda(), do_sample=False)
     torch.cuda.synchronize()                                                     # no illegal address; ids inside the range
     assert int(gg.min()) >= 0 and int(gg.max()) < 64 and int(ss.min()) >= 0 and int(ss.max()) < 128
-
-
-@pytest.mark.parametrize("B,task", [(5, "se"), (32, "se"), (16, "tse")])
-def test_lm_persistent_decode_matches_per_kernel_path(lib, B, task):
-    """csrc/llm_step.cu: the whole greedy decoding loop in one cooperative kernel (device-side grid barriers between the 62 stages
-    of a step) produces bit-identical tokens to the per-kernel path (same tile arithmetic), for both phases (global / semantic)."""
-    from oracle import llama
-    cfg = llama.LM_FULL
-    m, sd = build(cfg, 7, 2.0)
-    g = torch.Generator().manual_seed(40 + B)
-    T = 20
-    mix = torch.randn(B, T, 768, generator=g).cuda()
-    enr = torch.randn(B, 17, 768, generator=g).cuda() if task == "tse" else None
-    outs = {}
-    for kern in ("tc", "persistent", "persistent"):
-        m.decode_kernel = kern
-        gg, ss = m.generate(task, enr, enr, mix, mix, do_sample=False)
-        torch.cuda.synchronize()
-        outs.setdefault(kern, []).append((gg.cpu(), ss.cpu()))
-    (g0, s0), = outs["tc"]
-    for g1, s1 in outs["persistent"]:
-        assert torch.equal(g0, g1) and torch.equal(s0, s1), "persistent decode differs from the per-kernel path"
-    assert g0.shape == (B, 32) and s0.shape == (B, T)
 
 
 @pytest.mark.parametrize("task", ["se", "tse"])

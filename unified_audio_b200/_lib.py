@@ -97,9 +97,6 @@ SIGNATURES = {
     "qb_rvq_decode": (C.c_int, [_vp, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _vp]),
     "qb_lm_qkv_prep": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
     "qb_lm_flash_attn": (C.c_int, [_vp, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _vp, _vp, _vp]),
-    "qb_lm_decode_layer": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp,
-                                      _vp, _vp, _vp, _vp, _vp, _vp]),
-    "qb_lm_head_argmax": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "qb_lm_pack_weight": (C.c_int, [_vp, _i64, _i64, _vp, _vp]),
     "qb_lm_decode_layer_tc": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp,
                                         _vp, _vp, _vp, _vp]),
@@ -144,8 +141,6 @@ SIGNATURES = {
     "qb_lm_prefill": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp]),
     "qb_lm_decode_greedy": (C.c_int, [_vp, _vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
     "qb_lm_forward_logits": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
-    "qb_lm_decode_steps": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp,
-                                     _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp]),
     "qb_lm_loss": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _f32, _vp, _vp, _vp]),
     "qb_lm_head_sample_tc": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _i32,
                                        _f32, _vp, _vp, _vp]),

@@ -49,7 +49,7 @@ __device__ __forceinline__ float gelu_fast(float x) {
 }
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + __expf(-x)); }
 __device__ __forceinline__ float sigmoid_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
-// cached-decode attention: keys whose K / V rows one lane keeps in flight per trip (llm.cu lm_decode_attn2_kernel, llm_step.cu attn_item)
+// cached-decode attention: keys whose K / V rows one lane keeps in flight per trip (llm.cu lm_decode_attn2_kernel)
 #ifndef LM_ATT_U_DEFAULT
 #define LM_ATT_U_DEFAULT 8
 #endif

@@ -5,11 +5,13 @@
 // Prefill / teacher-forced forward (L > 1) runs on the wgmma GEMM (gemm.cu) plus the two kernels here:
 //   lm_qkv_prep   RoPE at absolute positions, 1/sqrt(d) folded into q, K/V appended to the static fp32 cache
 //   lm_flash_attn causal flash attention (mma.sync m16n8k16, 3-term fp16 split of Q/K/P/V) over the cache
-// KV-cache decode (L == 1, B <= 32) is HBM-bound (weights + cache streamed once per step): "skinny" fp32
-// kernels, one warp per output-column pair, batch rows in registers, x staged in shared memory:
-//   lm_gemv<MODE>  fused RMSNorm -> projection -> {RoPE + cache append | residual | SwiGLU | arg-max partials}
-//   lm_decode_attn one CTA per (batch, head), scores in shared memory
-//   lm_argmax_embed range-restricted greedy token + next input embedding + position bump
+// KV-cache decode (L == 1, B <= 32) is HBM-bound (weights + cache streamed once per step), each stage launched as a
+// programmatic dependent of the previous one:
+//   lm_skinny<MODE>   fused RMSNorm -> projection -> {RoPE + cache append | residual | SwiGLU | arg-max partials},
+//                     3-term fp16-split mma.sync over pre-packed weights
+//   lm_decode_attn2   one CTA per (head, batch row), online softmax over the fp32 cache
+//   lm_argmax_embed   range-restricted greedy token + next input embedding + position bump
+//   lm_sample_embed   top-k / top-p / temperature draw instead of the arg-max (sampled decoding)
 // All decode state (position, token range, output slot) lives in device memory so that one decode step is a
 // fixed launch sequence that can be captured in a CUDA graph and replayed.
 #include <atomic>
@@ -251,247 +253,6 @@ lm_flash_attn_kernel(const float* __restrict__ q32, const float* __restrict__ kc
 }
 
 // ------------------------------------------------------------------------------------------ decode step
-enum { LM_QKV = 0, LM_RESID = 1, LM_GATEUP = 2, LM_HEAD = 3 };
-constexpr int LM_KT = 512;      // K chunk staged in shared memory (fp32, 32 rows -> 64 KB)
-constexpr int LM_WARPS = 8;
-
-struct LmGemvParams {
-  const float* x;        // [B,K]
-  int B, K, n_items;
-  const float* W;        // [N,K] fp32
-  const float* W2;       // up-proj rows (GATEUP)
-  const float* norm_w;   // fused pre-RMSNorm weight or NULL
-  float eps;
-  float* out;            // RESID: x [B,N] updated in place; GATEUP: [B,n_items]; QKV: q32 [B,H*64]
-  int N;                 // RESID: output width
-  // QKV
-  int H, Lmax;
-  const int* pos;
-  const float* rcos;
-  const float* rsin;
-  float* kc;
-  float* vc;
-  // HEAD
-  const int* range;      // {lo, hi}
-  float* part_val;       // [gridDim.x, 32]
-  int* part_idx;
-};
-
-// RMSNorm is applied algebraically: the norm weight g is folded into the projection weights on the host
-// (W' = W diag(g)), so  (x * rstd * g) . W^T  ==  rstd * (x . W'^T)  and the per-row rstd only scales the
-// finished dot products - the raw x is staged with cp.async while the weight rows stream in, and the
-// sum of squares is taken from the staged tile after the FMAs (nothing serialises in front of the loads).
-template <int MODE, bool MULTI>
-__global__ void __launch_bounds__(LM_WARPS * 32, MULTI ? 1 : 2)
-lm_gemv_kernel(const LmGemvParams p) {
-  constexpr bool PAIR = MODE != LM_RESID;        // RESID: one output column per warp (more CTAs in flight)
-  constexpr int NI = LM_KT / 128;                 // float4 weight loads per lane per chunk and column
-  extern __shared__ __align__(16) float xs[];   // [32][LM_KT]
-  __shared__ float ssq[32];
-  __shared__ float bval[LM_WARPS][32];
-  __shared__ int bidx[LM_WARPS][32];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int B = p.B, K = p.K;
-  int lo = 0, n_items = p.n_items;
-  if (MODE == LM_HEAD) { lo = p.range[0]; n_items = (p.range[1] - lo) >> 1; }
-  const int item = blockIdx.x * LM_WARPS + warp;
-  const bool active = item < n_items;
-  int n0 = 0, n1 = 0, sec = 0, hh = 0, dd = 0;
-  const float* w0p = p.W;
-  const float* w1p = p.W;
-  if (active) {
-    if (MODE == LM_QKV) {
-      dd = item & 31; hh = (item >> 5) % p.H; sec = item / (32 * p.H);
-      n0 = sec * p.H * 64 + hh * 64 + dd; n1 = n0 + 32;
-      w0p = p.W + (size_t)n0 * K; w1p = p.W + (size_t)n1 * K;
-    } else if (MODE == LM_GATEUP) {
-      n0 = item; n1 = item;
-      w0p = p.W + (size_t)item * K; w1p = p.W2 + (size_t)item * K;
-    } else if (MODE == LM_RESID) {
-      n0 = item; n1 = item;
-      w0p = p.W + (size_t)n0 * K;
-    } else {
-      n0 = lo + 2 * item; n1 = n0 + 1;
-      w0p = p.W + (size_t)n0 * K; w1p = p.W + (size_t)n1 * K;
-    }
-  }
-  auto stage_x = [&](int k0) {   // asynchronous global -> shared copy of x[:, k0 : k0 + LM_KT]
-    for (int e = tid; e < 32 * (LM_KT / 4); e += LM_WARPS * 32) {
-      const int b = e / (LM_KT / 4), c4 = e - b * (LM_KT / 4);
-      float* dst = xs + (size_t)b * LM_KT + c4 * 4;
-      if (b < B && k0 + c4 * 4 < K) {
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(p.x + (size_t)b * K + k0 + c4 * 4)
-                     : "memory");
-      } else {
-        *reinterpret_cast<float4*>(dst) = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-  };
-  float4 wa[NI], wc[NI];
-  auto fetch = [&](int k0, float4 (&a)[NI], float4 (&c)[NI]) {
-#pragma unroll
-    for (int i = 0; i < NI; ++i) {
-      const int kk = k0 + i * 128 + lane * 4;
-      const bool ok = active && kk < K;
-      a[i] = ok ? __ldg(reinterpret_cast<const float4*>(w0p + kk)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      if (PAIR) c[i] = ok ? __ldg(reinterpret_cast<const float4*>(w1p + kk)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-  };
-  stage_x(0);
-  fetch(0, wa, wc);
-  if (tid < 32) ssq[tid] = 0.f;
-  float acc0[32], acc1[32];
-#pragma unroll
-  for (int b = 0; b < 32; ++b) { acc0[b] = 0.f; acc1[b] = 0.f; }
-  for (int k0 = 0; k0 < K; k0 += LM_KT) {
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    __syncthreads();
-    float4 na[NI], nc[NI];
-    if (MULTI && k0 + LM_KT < K) fetch(k0 + LM_KT, na, nc);      // next chunk's weights in flight
-#pragma unroll
-    for (int i = 0; i < NI; ++i) {
-      const int kk = i * 128 + lane * 4;
-      const float4 a = wa[i], c = wc[i];
-#pragma unroll
-      for (int b = 0; b < 32; ++b) {
-        const float4 xv = *reinterpret_cast<const float4*>(xs + (size_t)b * LM_KT + kk);
-        acc0[b] = fmaf(xv.x, a.x, fmaf(xv.y, a.y, fmaf(xv.z, a.z, fmaf(xv.w, a.w, acc0[b]))));
-        if (PAIR) acc1[b] = fmaf(xv.x, c.x, fmaf(xv.y, c.y, fmaf(xv.z, c.z, fmaf(xv.w, c.w, acc1[b]))));
-      }
-    }
-    if (p.norm_w) {   // sum of squares of the staged rows (rows warp, warp+8, ...)
-      for (int b = warp; b < B; b += LM_WARPS) {
-        float q = 0.f;
-#pragma unroll
-        for (int i = 0; i < LM_KT / 128; ++i) {
-          const float4 v = *reinterpret_cast<const float4*>(xs + (size_t)b * LM_KT + i * 128 + lane * 4);
-          q = fmaf(v.x, v.x, fmaf(v.y, v.y, fmaf(v.z, v.z, fmaf(v.w, v.w, q))));
-        }
-        q = warp_sum(q);
-        if (lane == 0) ssq[b] += q;
-      }
-    }
-    if (MULTI && k0 + LM_KT < K) {
-      __syncthreads();                 // everyone is done with this chunk of xs
-      stage_x(k0 + LM_KT);
-#pragma unroll
-      for (int i = 0; i < NI; ++i) { wa[i] = na[i]; if (PAIR) wc[i] = nc[i]; }
-    }
-  }
-  // lane b keeps the totals of batch row b
-  float r0 = 0.f, r1 = 0.f;
-#pragma unroll
-  for (int b = 0; b < 32; ++b) {
-    const float t0 = warp_sum(acc0[b]);
-    const float t1 = PAIR ? warp_sum(acc1[b]) : 0.f;
-    if (lane == b) { r0 = t0; r1 = t1; }
-  }
-  const int b = lane;
-  if (p.norm_w) {
-    __syncthreads();
-    const float rs = rsqrtf(ssq[b] / K + p.eps);
-    r0 *= rs;
-    r1 *= rs;
-  }
-  if (MODE == LM_HEAD) {
-    float bv = -INFINITY;
-    int bi = 0x7fffffff;
-    if (active && b < B) {
-      bv = r0; bi = n0;
-      if (r1 > bv) { bv = r1; bi = n1; }     // ties -> lower index (n0 < n1)
-    }
-    bval[warp][lane] = bv;
-    bidx[warp][lane] = bi;
-    __syncthreads();
-    if (warp == 0) {
-      for (int w = 1; w < LM_WARPS; ++w) {
-        const float v = bval[w][lane];
-        const int ix = bidx[w][lane];
-        if (v > bv || (v == bv && ix < bi)) { bv = v; bi = ix; }
-      }
-      p.part_val[(size_t)blockIdx.x * 32 + lane] = bv;
-      p.part_idx[(size_t)blockIdx.x * 32 + lane] = bi;
-    }
-    return;
-  }
-  if (!active || b >= B) return;
-  if (MODE == LM_RESID) {
-    p.out[(size_t)b * p.N + n0] += r0;
-  } else if (MODE == LM_GATEUP) {
-    p.out[(size_t)b * p.n_items + item] = silu_f(r0) * r1;
-  } else {  // LM_QKV
-    const int pos = *p.pos;
-    if (sec < 2) {
-      const float c1 = p.rcos[pos * 64 + dd], s1 = p.rsin[pos * 64 + dd];
-      const float c2 = p.rcos[pos * 64 + dd + 32], s2 = p.rsin[pos * 64 + dd + 32];
-      const float y0 = r0 * c1 - r1 * s1, y1 = r1 * c2 + r0 * s2;
-      if (sec == 0) {
-        p.out[(size_t)b * p.H * 64 + hh * 64 + dd] = y0 * 0.125f;
-        p.out[(size_t)b * p.H * 64 + hh * 64 + dd + 32] = y1 * 0.125f;
-      } else {
-        const size_t o = (((size_t)b * p.H + hh) * p.Lmax + pos) * 64 + dd;
-        p.kc[o] = y0;
-        p.kc[o + 32] = y1;
-      }
-    } else {
-      const size_t o = (((size_t)b * p.H + hh) * p.Lmax + pos) * 64 + dd;
-      p.vc[o] = r0;
-      p.vc[o + 32] = r1;
-    }
-  }
-}
-
-// one CTA per (head, batch row): q [B,H*64] fp32 (scaled), fp32 cache, keys 0..pos inclusive
-__global__ void __launch_bounds__(128)
-lm_decode_attn_kernel(const float* __restrict__ q, const float* __restrict__ kc, const float* __restrict__ vc, int H,
-                      int Lmax, const int* __restrict__ posp, float* __restrict__ out) {
-  extern __shared__ float sc[];   // [Lmax] scores
-  __shared__ __align__(16) float qs[64];
-  __shared__ float red[4];
-  __shared__ float part[2][64];
-  const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int n = *posp + 1;
-  if (tid < 64) qs[tid] = q[(size_t)b * H * 64 + h * 64 + tid];
-  __syncthreads();
-  const float* kb = kc + ((size_t)b * H + h) * Lmax * 64;
-  const float* vb = vc + ((size_t)b * H + h) * Lmax * 64;
-  float mx = -INFINITY;
-  for (int j = tid; j < n; j += 128) {
-    const float4* kr = reinterpret_cast<const float4*>(kb + (size_t)j * 64);
-    float acc = 0.f;
-#pragma unroll
-    for (int c = 0; c < 16; ++c) {
-      const float4 v = kr[c];
-      const float4 qq = *reinterpret_cast<const float4*>(qs + 4 * c);
-      acc = fmaf(qq.x, v.x, fmaf(qq.y, v.y, fmaf(qq.z, v.z, fmaf(qq.w, v.w, acc))));
-    }
-    sc[j] = acc;
-    mx = fmaxf(mx, acc);
-  }
-  mx = warp_max(mx);
-  if (lane == 0) red[warp] = mx;
-  __syncthreads();
-  mx = fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
-  __syncthreads();
-  float sum = 0.f;
-  for (int j = tid; j < n; j += 128) {
-    const float e = expf(sc[j] - mx);
-    sc[j] = e;
-    sum += e;
-  }
-  sum = warp_sum(sum);
-  if (lane == 0) red[warp] = sum;
-  __syncthreads();
-  sum = red[0] + red[1] + red[2] + red[3];
-  const int d = tid & 63, half = tid >> 6;
-  float acc = 0.f;
-  for (int j = half; j < n; j += 2) acc = fmaf(sc[j], vb[(size_t)j * 64 + d], acc);
-  part[half][d] = acc;
-  __syncthreads();
-  if (tid < 64) out[(size_t)b * H * 64 + h * 64 + tid] = (part[0][tid] + part[1][tid]) / sum;
-}
-
 // greedy token from the head partials, next input embedding, position / slot bump
 __global__ void lm_argmax_embed_kernel(const float* __restrict__ part_val, const int* __restrict__ part_idx, int n_part,
                                        int B, const float* __restrict__ emb, int Hd, float* __restrict__ x_next,
@@ -747,11 +508,11 @@ lm_sample_embed_kernel(const float* __restrict__ logits, int ld, const int* __re
   }
 }
 
-// ------------------------------------------------------------------------------------------ decode step, tensor-core path
-// The fp32 SIMT kernels above spend their time in shared-memory reads (every warp re-reads the whole x tile for
-// one or two output columns) and in 32-way shuffle reductions.  The product path below keeps the same fusion
-// (RMSNorm folded into W, RoPE + cache append / residual / SwiGLU / arg-max partials in the epilogue) but runs
-// the [32 x K] . [K x 8] products as 3-term fp16-split mma.sync tiles:
+// ------------------------------------------------------------------------------------------ decode step, projections and attention
+// fp32 SIMT dot products spend their time in shared-memory reads (every warp re-reads the whole x tile for one or
+// two output columns) and in 32-way shuffle reductions.  These kernels fuse the same way (RMSNorm folded into W,
+// RoPE + cache append / residual / SwiGLU / arg-max partials in the epilogue) but run the [32 x K] . [K x 8]
+// products as 3-term fp16-split mma.sync tiles:
 //   * weights are pre-packed once (qb_lm_pack_weight) as uint4 {hi[4], lo[4]} per 4 consecutive k of a row:
 //     the same 4 bytes / parameter as fp32, zero conversion work on the streaming side, one 16-byte load per lane
 //     that is directly the B fragment of two MMA k-slots (k-slot order inside an MMA is free as long as A agrees);
@@ -778,8 +539,7 @@ struct SkParams {
   const int* range;
   float* part_val;
   int* part_idx;
-  int pdl_early;         // 1: release the dependent grid before the dependency wait (deep pile-up), 0: after the K loop
-  float* logits;         // HEAD: optional full logits of the range [B][logits_ld] (sampled decoding); NULL = arg-max partials only
+  float* logits;        // HEAD: optional full logits of the range [B][logits_ld] (sampled decoding); NULL = arg-max partials only
   int logits_ld;
 };
 
@@ -800,7 +560,7 @@ __global__ void lm_pack_weight_kernel(const float* __restrict__ w, long long tot
 }
 
 // 256-thread variants are capped at 128 registers so that TWO CTAs fit an SM: the gate/up projection (inter/8 = 256 CTAs) and the
-// head (256 / 512 CTAs) then run in one / two waves on 132 SMs instead of two / four (QB_LM_SKINNY_OCC).
+// head (256 / 512 CTAs) then run in one / two waves on 132 SMs instead of two / four.
 template <int MODE, int SPW, int NW>
 __global__ void __launch_bounds__(NW * 32, NW == 8 ? 2 : 1)
 lm_skinny_kernel(const SkParams p) {
@@ -841,7 +601,6 @@ lm_skinny_kernel(const SkParams p) {
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) wv[nt][s] = ok ? __ldg(wrow[nt] + step * 4 + t) : make_uint4(0u, 0u, 0u, 0u);
   }
-  if (p.pdl_early) pdl_launch_dependents();
   pdl_wait();
   float acc[2][NT][4];
 #pragma unroll
@@ -890,8 +649,9 @@ lm_skinny_kernel(const SkParams p) {
         }
     }
   }
-  // the dependent grid may start (and prefetch its weights) while this one reduces, stores and drains
-  if (!p.pdl_early) pdl_launch_dependents();
+  // the dependent grid may start (and prefetch its weights) while this one reduces, stores and drains.  Not before the dependency
+  // wait: the dependent's L1 would be invalidated at its launch and then refilled with stale x by an older co-resident kernel.
+  pdl_launch_dependents();
   // ---- cross-warp reduction (fixed order)
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt)
@@ -981,10 +741,9 @@ lm_skinny_kernel(const SkParams p) {
 template <int LM_ATT_U>
 __global__ void __launch_bounds__(256)
 lm_decode_attn2_kernel(const float* __restrict__ q, const float* __restrict__ kc, const float* __restrict__ vc, int H,
-                       int Lmax, const int* __restrict__ posp, float* __restrict__ out, int pdl_early) {
+                       int Lmax, const int* __restrict__ posp, float* __restrict__ out) {
   __shared__ __align__(16) float sacc[16][64];
   __shared__ float sm[16], sl[16];
-  if (pdl_early) pdl_launch_dependents();
   pdl_wait();
   const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int c = lane & 15, hw = warp * 2 + (lane >> 4);
@@ -1031,7 +790,7 @@ lm_decode_attn2_kernel(const float* __restrict__ q, const float* __restrict__ kc
       m = mn;
     }
   }
-  if (!pdl_early) pdl_launch_dependents();
+  pdl_launch_dependents();      // after the main loop, as in lm_skinny_kernel
   *reinterpret_cast<float4*>(&sacc[hw][4 * c]) = acc;
   if (c == 0) { sm[hw] = m; sl[hw] = l; }
   __syncthreads();
@@ -1078,96 +837,7 @@ extern "C" int qb_lm_flash_attn(const float* q32, const float* k_cache, const fl
   return 0;
 }
 
-template <int MODE, bool MULTI>
-static int launch_gemv_t(const LmGemvParams& p, int n_items_max, cudaStream_t st) {
-    const size_t smem = (size_t)32 * LM_KT * sizeof(float);
-  QB_CHECK_CUDA(cudaFuncSetAttribute(lm_gemv_kernel<MODE, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   // per-device state: set on every launch (cheap)
-  lm_gemv_kernel<MODE, MULTI><<<(unsigned)ceil_div(n_items_max, LM_WARPS), LM_WARPS * 32, smem, st>>>(p);
-  g_launches++;
-  QB_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-template <int MODE>
-static int launch_gemv(const LmGemvParams& p, int n_items_max, cudaStream_t st) {
-  return p.K > LM_KT ? launch_gemv_t<MODE, true>(p, n_items_max, st) : launch_gemv_t<MODE, false>(p, n_items_max, st);
-}
-
-extern "C" int qb_lm_decode_layer(float* x, int64_t B, int32_t hidden, int32_t heads, int32_t inter, const float* in_norm,
-                                  const float* wqkv, const float* wo, const float* post_norm, const float* wgate,
-                                  const float* wup, const float* wdown, float* k_cache, float* v_cache, int32_t Lmax,
-                                  const int32_t* pos, const float* rope_cos, const float* rope_sin, float* q_buf,
-                                  float* attn_buf, float* mlp_buf, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  QB_REQUIRE(B >= 1 && B <= 32, "lm_decode_layer: batch must be 1..32 (got %lld)", (long long)B);
-  QB_REQUIRE(hidden == heads * 64 && hidden % 128 == 0 && inter % 128 == 0, "lm_decode_layer: unsupported dims");
-  LmGemvParams p = {};
-  p.B = (int)B; p.eps = 1e-6f; p.H = heads; p.Lmax = Lmax; p.pos = pos; p.rcos = rope_cos; p.rsin = rope_sin;
-  p.kc = k_cache; p.vc = v_cache;
-  // RMSNorm + QKV + RoPE + cache append
-  p.x = x; p.K = hidden; p.W = wqkv; p.norm_w = in_norm; p.out = q_buf; p.n_items = 3 * heads * 32;
-  if (int e = launch_gemv<LM_QKV>(p, p.n_items, st)) return e;
-    const size_t asmem = (size_t)Lmax * sizeof(float);
-  QB_CHECK_CUDA(cudaFuncSetAttribute(lm_decode_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));   // per-device state: set on every launch (cheap)
-  QB_REQUIRE(asmem <= 64 * 1024, "lm_decode_layer: Lmax too large for the score buffer");
-  lm_decode_attn_kernel<<<dim3((unsigned)heads, (unsigned)B), 128, asmem, st>>>(q_buf, k_cache, v_cache, heads, Lmax, pos,
-                                                                              attn_buf);
-  g_launches++;
-  // o_proj + residual
-  p.x = attn_buf; p.K = hidden; p.W = wo; p.norm_w = nullptr; p.out = x; p.N = hidden; p.n_items = hidden;
-  if (int e = launch_gemv<LM_RESID>(p, p.n_items, st)) return e;
-  // RMSNorm + gate/up + SwiGLU
-  p.x = x; p.K = hidden; p.W = wgate; p.W2 = wup; p.norm_w = post_norm; p.out = mlp_buf; p.n_items = inter;
-  if (int e = launch_gemv<LM_GATEUP>(p, p.n_items, st)) return e;
-  // down + residual
-  p.x = mlp_buf; p.K = inter; p.W = wdown; p.W2 = nullptr; p.norm_w = nullptr; p.out = x; p.N = hidden; p.n_items = hidden;
-  if (int e = launch_gemv<LM_RESID>(p, p.n_items, st)) return e;
-  QB_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-extern "C" int qb_lm_head_argmax(const float* x, int64_t B, int32_t hidden, const float* final_norm, const float* w_head,
-                                 const int32_t* range, int32_t max_cols, const float* embedding, float* x_next,
-                                 int64_t* out_ids, int32_t out_stride, int32_t* pos, int32_t* slot, float* part_val,
-                                 int32_t* part_idx, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  QB_REQUIRE(B >= 1 && B <= 32 && max_cols % 2 == 0, "lm_head_argmax: bad args");
-  LmGemvParams p = {};
-  p.B = (int)B; p.eps = 1e-6f; p.x = x; p.K = hidden; p.W = w_head; p.norm_w = final_norm; p.range = range;
-  p.part_val = part_val; p.part_idx = part_idx; p.n_items = max_cols / 2;
-  if (int e = launch_gemv<LM_HEAD>(p, max_cols / 2, st)) return e;
-  const int n_part = (int)ceil_div(max_cols / 2, LM_WARPS);
-  lm_argmax_embed_kernel<<<(unsigned)B, 128, 0, st>>>(part_val, part_idx, n_part, (int)B, embedding, hidden, x_next,
-                                                     out_ids, out_stride, pos, slot, range, 0x7ffffffe);
-  g_launches++;
-  QB_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-// ------------------------------------------------------------------------------------------ tensor-core decode (product path)
-// "Early" programmatic launch (griddepcontrol.launch_dependents BEFORE the kernel's own dependency wait) lets a whole cascade of
-// dependents become resident while older kernels still run.  Measured: 102.5 vs 103.9 ms per generate - and NOT token-stable once
-// several decode chains share the GPU: a dependent's L1 is invalidated when it is launched, a co-resident older kernel that still
-// reads x (every gate/up CTA reads all of x) re-fills the SM's L1 with the old lines, and the dependent then reads them after its
-// wait.  With the trigger after the main loop (the product setting) a dependent is launched only when every older kernel's loads
-// of mutable data are over.  The switch therefore needs QB_LM_UNSAFE=1 next to QB_LM_PDL_EARLY=1 (experiments only).
-static int lm_pdl_early() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("QB_LM_PDL_EARLY");
-    const char* u = getenv("QB_LM_UNSAFE");
-    v = (e && e[0] == '1' && u && u[0] == '1') ? 1 : 0;
-  }
-  return v;
-}
-static bool lm_pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("QB_LM_PDL");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-
+// ------------------------------------------------------------------------------------------ decode step, host side
 template <typename... KArgs, typename... Args>
 static cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
   cudaLaunchConfig_t cfg = {};
@@ -1176,7 +846,7 @@ static cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
-  cfg.numAttrs = lm_pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   g_launches++;
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
@@ -1217,7 +887,7 @@ extern "C" int qb_lm_decode_layer_tc(float* x, int64_t B, int32_t hidden, int32_
   QB_REQUIRE(hidden == heads * 64 && hidden % 16 == 0 && inter % 16 == 0, "lm_decode_layer_tc: unsupported dims");
   SkParams p = {};
   p.B = (int)B; p.eps = 1e-6f; p.H = heads; p.Lmax = Lmax; p.pos = pos; p.rcos = rope_cos; p.rsin = rope_sin;
-  p.kc = k_cache; p.vc = v_cache; p.pdl_early = lm_pdl_early();
+  p.kc = k_cache; p.vc = v_cache;
   // RMSNorm + QKV + RoPE + cache append
   p.x = x; p.K = hidden; p.W = (const uint4*)wqkv; p.out = q_buf;
   if (int e = launch_skinny<SK_QKV>(p, 3 * heads * 4, st)) return e;
@@ -1225,8 +895,7 @@ extern "C" int qb_lm_decode_layer_tc(float* x, int64_t B, int32_t hidden, int32_
   // (latency-bound), 4 when several chains share the GPU (throughput-bound)
   auto att = g_lm_att_unroll == 4 ? lm_decode_attn2_kernel<4> : lm_decode_attn2_kernel<8>;
   QB_CHECK_CUDA(launch_pdl(att, dim3((unsigned)heads, (unsigned)B), dim3(256), 0, st, (const float*)q_buf,
-                           (const float*)k_cache, (const float*)v_cache, (int)heads, (int)Lmax, (const int*)pos, attn_buf,
-                           lm_pdl_early()));
+                           (const float*)k_cache, (const float*)v_cache, (int)heads, (int)Lmax, (const int*)pos, attn_buf));
   // o_proj + residual
   p.x = attn_buf; p.K = hidden; p.W = (const uint4*)wo; p.out = x; p.N = hidden;
   if (int e = launch_skinny<SK_RESID>(p, hidden / 8, st)) return e;
@@ -1247,7 +916,7 @@ extern "C" int qb_lm_head_argmax_tc(const float* x, int64_t B, int32_t hidden, c
   QB_REQUIRE(B >= 1 && B <= 32 && max_cols % 16 == 0, "lm_head_argmax_tc: bad args (max_cols must be a multiple of 16)");
   SkParams p = {};
   p.B = (int)B; p.eps = 1e-6f; p.x = x; p.K = hidden; p.W = (const uint4*)w_head; p.range = range;
-  p.part_val = part_val; p.part_idx = part_idx; p.pdl_early = lm_pdl_early();
+  p.part_val = part_val; p.part_idx = part_idx;
   if (int e = launch_skinny<SK_HEAD>(p, max_cols / 16, st)) return e;
   QB_CHECK_CUDA(launch_pdl(lm_argmax_embed_kernel, dim3((unsigned)B), dim3(128), 0, st, (const float*)part_val,
                            (const int*)part_idx, (int)(max_cols / 16), (int)B, embedding, (int)hidden, x_next, out_ids,
@@ -1269,7 +938,7 @@ extern "C" int qb_lm_head_sample_tc(const float* x, int64_t B, int32_t hidden, c
   QB_REQUIRE(top_k >= 1 && top_k <= LS_MAX, "lm_head_sample_tc: top_k must be in 1..%d (got %d)", LS_MAX, top_k);
   SkParams p = {};
   p.B = (int)B; p.eps = 1e-6f; p.x = x; p.K = hidden; p.W = (const uint4*)w_head; p.range = range;
-  p.part_val = part_val; p.part_idx = part_idx; p.pdl_early = lm_pdl_early(); p.logits = logits; p.logits_ld = max_cols;
+  p.part_val = part_val; p.part_idx = part_idx; p.logits = logits; p.logits_ld = max_cols;
   if (int e = launch_skinny<SK_HEAD>(p, max_cols / 16, st)) return e;
   const size_t smem = ((size_t)((max_cols + 3) & ~3) + 2 * LS_MAX) * 4;
     QB_CHECK_CUDA(cudaFuncSetAttribute(lm_sample_embed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));   // per-device state: set on every launch (cheap)

@@ -10,9 +10,9 @@ state_dict keys are the reference's (HF Llama layer names under `layers.*`, `nor
 condition encoder (`cond_*`, built but never executed: llm_sft.py:62-65,112-115) is accepted at load and ignored.
 
 Prefill / teacher-forced forward: wgmma GEMMs (3-term split) + causal split-precision flash attention over a static fp32 KV cache.
-Decode: fused skinny kernels (3-term fp16-split mma.sync over pre-packed weights, programmatic dependent launch; the fp32
-SIMT versions are the cross-check, QB_LM_DECODE=simt), one CUDA graph per step replayed 33 + T times; greedy (do_sample=False, the shipped
-setting U/model/model.py:173).  No PyTorch / CPU fallback for the transformer stack.
+Decode: fused skinny kernels (3-term fp16-split mma.sync over pre-packed weights with the RMSNorm weights folded in,
+programmatic dependent launch), captured in CUDA graphs and replayed for the 33 + T steps; greedy (do_sample=False, the shipped
+setting U/model/model.py:173) or sampled on the device.  No PyTorch / CPU fallback for the transformer stack.
 """
 from __future__ import annotations
 
@@ -102,10 +102,6 @@ class LLM_SFT(nn.Module):
         for name, child in tree.named_children():
             self.add_module(name, child)
         self._w, self._ws = None, {}
-        # "persistent": the whole decoding loop in one cooperative kernel (csrc/llm_step.cu; greedy, shipped dimensions);
-        # "tc": one kernel per stage, packed fp16-split weights + mma.sync + programmatic dependent launch, 8 steps per CUDA graph
-        # (also the sampled-decoding path);  "simt": fp32 cross-check
-        self.decode_kernel = os.environ.get("QB_LM_DECODE", "tc")
         self.graph_steps = int(os.environ.get("QB_LM_GRAPH_STEPS", "8"))     # decode steps per replayed CUDA graph
         self._gen_state = {}
         # generate() walks a batch in chunks of <= `chunk` sequences; `lanes` > 1 runs that many chunks CONCURRENTLY, each on its own
@@ -147,25 +143,23 @@ class LLM_SFT(nn.Module):
             p = f"layers.{i}."
             wqkv = torch.cat([sd[p + f"self_attn.{n}_proj.weight"] for n in "qkv"], 0).contiguous()
             wg, wu = sd[p + "mlp.gate_proj.weight"].contiguous(), sd[p + "mlp.up_proj.weight"].contiguous()
+            in_w, post_w = sd[p + "input_layernorm.weight"].contiguous(), sd[p + "post_attention_layernorm.weight"].contiguous()
             layers.append(dict(
-                in_w=sd[p + "input_layernorm.weight"].contiguous(), post_w=sd[p + "post_attention_layernorm.weight"].contiguous(),
+                in_w=in_w, post_w=post_w,
                 wqkv=Planes.from_f32(wqkv, True), wo=Planes.from_f32(sd[p + "self_attn.o_proj.weight"], True),
                 wgu=Planes.from_f32(torch.stack([wg, wu], 1).reshape(-1, self.hidden), True),
                 wd=Planes.from_f32(sd[p + "mlp.down_proj.weight"], True),
-                # decode path: fp32 weights with the preceding RMSNorm weight folded in (W' = W diag(g))
-                wqkv32=(wqkv * sd[p + "input_layernorm.weight"][None, :]).contiguous(),
-                wo32=sd[p + "self_attn.o_proj.weight"].contiguous(),
-                wg32=(wg * sd[p + "post_attention_layernorm.weight"][None, :]).contiguous(),
-                wu32=(wu * sd[p + "post_attention_layernorm.weight"][None, :]).contiguous(),
-                wd32=sd[p + "mlp.down_proj.weight"].contiguous()))
-            L = layers[-1]       # product decode path: the same folded weights packed as fp16 {hi[4], lo[4]} groups
-            L.update(wqkv_p=ops.lm_pack_weight(L["wqkv32"]), wo_p=ops.lm_pack_weight(L["wo32"]), wg_p=ops.lm_pack_weight(L["wg32"]),
-                     wu_p=ops.lm_pack_weight(L["wu32"]), wd_p=ops.lm_pack_weight(L["wd32"]))
+                # decode path: the preceding RMSNorm weight folded in (W' = W diag(g)), packed as fp16 {hi[4], lo[4]} groups
+                wqkv_p=ops.lm_pack_weight(wqkv * in_w[None, :]),
+                wo_p=ops.lm_pack_weight(sd[p + "self_attn.o_proj.weight"]),
+                wg_p=ops.lm_pack_weight(wg * post_w[None, :]),
+                wu_p=ops.lm_pack_weight(wu * post_w[None, :]),
+                wd_p=ops.lm_pack_weight(sd[p + "mlp.down_proj.weight"])))
         self._w = dict(layers=layers, norm=sd["norm.weight"].contiguous(), head=Planes.from_f32(sd["output_head.weight"], True),
-                       head32=(sd["output_head.weight"] * sd["norm.weight"][None, :]).contiguous(), emb=sd["codec_embedding.weight"].contiguous(),
+                       head_p=ops.lm_pack_weight(sd["output_head.weight"] * sd["norm.weight"][None, :]),
+                       emb=sd["codec_embedding.weight"].contiguous(),
                        adapter=Planes.from_f32(sd["adapter.weight"], True), adapter_b=sd["adapter.bias"].contiguous(),
                        cos=None, sin=None, rope_rows=0)
-        self._w["head_p"] = ops.lm_pack_weight(self._w["head32"])
         self._ensure_rope(self.max_pos)
         return self._w
 
@@ -247,13 +241,12 @@ class LLM_SFT(nn.Module):
 
     def _decode_layers(self, x: torch.Tensor, B: int, cache: StaticKVCache):
         W = self._prepare()
-        if self.decode_kernel == "tc":
-            ops.lm_set_att_unroll(self.att_unroll)
+        ops.lm_set_att_unroll(self.att_unroll)
         H, heads, inter = self.hidden, self.heads, 4 * self.hidden
         qb, ab, mb = self._buf("dq", (B, H)), self._buf("da", (B, H)), self._buf("dm", (B, inter))
-        layer = ops.lm_decode_layer_tc if self.decode_kernel == "tc" else ops.lm_decode_layer
         for i, Lw in enumerate(W["layers"]):
-            layer(x, B, H, heads, inter, Lw, cache.k[i], cache.v[i], cache.Lmax, cache.pos, W["cos"], W["sin"], qb, ab, mb)
+            ops.lm_decode_layer_tc(x, B, H, heads, inter, Lw, cache.k[i], cache.v[i], cache.Lmax, cache.pos, W["cos"], W["sin"],
+                                   qb, ab, mb)
 
     @torch.no_grad()
     def llm_forward(self, inputs_embeds, attention_mask=None, past_key_values: Optional[StaticKVCache] = None,
@@ -360,8 +353,6 @@ class LLM_SFT(nn.Module):
         reference's arg-max does (filters never remove the arg-max, llm.py:263-287)."""
         sampling = None
         if do_sample:
-            if self.decode_kernel != "tc":
-                raise NotImplementedError("sampled decoding runs on the tensor-core decode path only (QB_LM_DECODE=tc)")
             if not (0.0 < temperature <= 1.0):
                 raise AssertionError("0 < temperature <= 1.0 (llm.py:278)")
             if top_k <= 0 or top_k > 1024:
@@ -436,7 +427,7 @@ class LLM_SFT(nn.Module):
         samp_key = None if sampling is None else (sampling["temperature"], sampling["top_k"], sampling["top_p"])
         # Decode state (KV cache, counters, output ids) and the captured graphs are kept per shape: capturing and
         # instantiating ~560 kernel nodes costs the host 10-50 ms, as much as the whole generation takes on the device.
-        key = (B, P, n_steps, bool(use_graph), self.decode_kernel, int(self.graph_steps), str(dev), samp_key)
+        key = (B, P, n_steps, bool(use_graph), int(self.graph_steps), str(dev), samp_key)
         st = self._gen_state.get(key)
         if st is None:
             self._gen_state.clear()                    # one shape at a time (the cache is ~0.9 GB at B=32)
@@ -468,17 +459,14 @@ class LLM_SFT(nn.Module):
                 ops.lm_head_sample_tc(xs, B, H, W["head_p"], rng, max_cols, W["emb"], xs, out_ids, n_steps, cache.pos, slot, pv, pi,
                                       st["logits"], sampling["temperature"], sampling["top_k"], sampling["top_p"], st["seed"],
                                       st["dbg"])
-            elif self.decode_kernel == "tc":
+            else:
                 ops.lm_head_argmax_tc(xs, B, H, W["head_p"], rng, max_cols, W["emb"], xs, out_ids, n_steps, cache.pos, slot,
                                       pv, pi)
-            else:
-                ops.lm_head_argmax(xs, B, H, W["norm"], W["head32"], rng, max_cols, W["emb"], xs, out_ids, n_steps, cache.pos,
-                                   slot, pv, pi)
 
         # All decode state is on the device, so a graph may hold any number of consecutive steps: one single-step graph
         # plus one of `graph_steps` steps (fewer replays per generation).
         K = max(1, int(self.graph_steps))
-        if use_graph and not st["captured"] and not (self.decode_kernel == "persistent" and sampling is None):
+        if use_graph and not st["captured"]:
             # warm-up outside capture (one-time cudaFuncSetAttribute calls), then restore the mutated state
             xs.copy_(W["emb"][self.global_sos_token_id][None].expand(B, H))
             step()
@@ -495,23 +483,8 @@ class LLM_SFT(nn.Module):
             cache.pos.fill_(cache.length)
             slot.zero_()
         g1, gk = (st["g1"], st["gk"]) if use_graph else (None, None)
-        persistent = (self.decode_kernel == "persistent" and sampling is None and H == 512 and self.n_layers <= 16 and max_cols % 16 == 0)
-        if persistent and "ptrs" not in st:
-            Ls = W["layers"]
-            st["ptrs"] = dict(n=self.n_layers, wqkv=ops.ptr_array([l["wqkv_p"] for l in Ls]), wo=ops.ptr_array([l["wo_p"] for l in Ls]),
-                              wg=ops.ptr_array([l["wg_p"] for l in Ls]), wu=ops.ptr_array([l["wu_p"] for l in Ls]),
-                              wd=ops.ptr_array([l["wd_p"] for l in Ls]), k=ops.ptr_array(cache.k), v=ops.ptr_array(cache.v))
-            st["bar"] = torch.zeros(4, dtype=torch.int32, device=dev)
-            st["dbuf"] = (torch.zeros(B, H, device=dev), torch.zeros(B, H, device=dev), torch.zeros(B, 4 * H, device=dev))
-
-        def run_persistent(n):
-            qb, ab, mb = st["dbuf"]
-            ops.lm_decode_steps(xs, B, H, self.heads, 4 * H, st["ptrs"], cache.Lmax, W["head_p"], rng, max_cols, W["emb"], W["cos"], W["sin"],
-                                qb, ab, mb, pv, pi, out_ids, n_steps, cache.pos, slot, n, st["bar"])
 
         def run(n):
-            if persistent:
-                return run_persistent(n)
             while n > 0:
                 if gk is not None and n >= K:
                     gk.replay()

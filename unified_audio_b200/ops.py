@@ -292,19 +292,6 @@ def lm_flash_attn(q16, kc, vc, B, L, heads, pos0, Lmax, out: Planes):
                                             _stream()))
 
 
-def lm_decode_layer(x, B, hidden, heads, inter, L, kc, vc, Lmax, pos, cos, sin, q_buf, attn_buf, mlp_buf):
-    _lib.check(_lib.load().qb_lm_decode_layer(_p(x), B, hidden, heads, inter, _p(L["in_w"]), _p(L["wqkv32"]), _p(L["wo32"]),
-                                              _p(L["post_w"]), _p(L["wg32"]), _p(L["wu32"]), _p(L["wd32"]), _p(kc), _p(vc),
-                                              Lmax, _p(pos), _p(cos), _p(sin), _p(q_buf), _p(attn_buf), _p(mlp_buf),
-                                              _stream()))
-
-
-def lm_head_argmax(x, B, hidden, final_norm, w_head, rng, max_cols, emb, x_next, out_ids, out_stride, pos, slot, pv, pi):
-    _lib.check(_lib.load().qb_lm_head_argmax(_p(x), B, hidden, _p(final_norm), _p(w_head), _p(rng), max_cols, _p(emb),
-                                             _p(x_next), _p(out_ids), out_stride, _p(pos), _p(slot), _p(pv), _p(pi),
-                                             _stream()))
-
-
 def lm_pack_weight(w: torch.Tensor) -> torch.Tensor:
     """fp32 [n,k] -> fp16 [n,2k] groups of {hi[4], lo[4]} (decode B-fragment layout, include/quark_b200.h)."""
     w = w.float().contiguous()
@@ -381,21 +368,6 @@ def pad_wav(x, left, T_out, wrap=False):
     out = torch.empty(B, T_out, device=x.device)
     _lib.check(_lib.load().qb_pad_wav(_p(x), B, T, left, T_out, int(wrap), _p(out), _stream()))
     return out
-
-
-def ptr_array(tensors):
-    """host array of device pointers (kept alive by the caller)"""
-    return (C.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
-
-
-def lm_decode_steps(x, B, hidden, heads, inter, layer_ptrs, Lmax, w_head_p, rng, max_cols, emb, cos, sin, q_buf, attn_buf, mlp_buf, pv, pi,
-                    out_ids, out_stride, pos, slot, n_steps, barrier):
-    """layer_ptrs: dict of ctypes pointer arrays wqkv / wo / wg / wu / wd / k / v (ptr_array)"""
-    L = layer_ptrs
-    _lib.check(_lib.load().qb_lm_decode_steps(_p(x), B, hidden, heads, inter, L["n"], L["wqkv"], L["wo"], L["wg"], L["wu"], L["wd"], L["k"], L["v"],
-                                              Lmax, _p(w_head_p), _p(rng), max_cols, _p(emb), _p(cos), _p(sin), _p(q_buf), _p(attn_buf),
-                                              _p(mlp_buf), _p(pv), _p(pi), _p(out_ids), out_stride, _p(pos), _p(slot), n_steps, _p(barrier),
-                                              _stream()))
 
 
 def lm_loss(logits, ld, M, V, targets, label_smoothing):
