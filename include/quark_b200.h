@@ -151,22 +151,15 @@ int qb_groupnorm_apply(const float* x, const float* stats, const float* w, const
                        int64_t ld, int64_t rows_per_batch, int64_t row_off, void* stream);
 
 /* ---------------------------------------------------------------- spectral front / back end */
-/* wav [B,T] fp32 -> hop-blocked planes [B, T/hop + 1, hop] with (n_fft-hop)/2 zeros each side
- * (vq/codec_encoder.py:65-66; frame f = hop blocks f, f+1 when n_fft == 2*hop). */
-int qb_wav_to_hopblocks(const float* wav, int64_t B, int64_t T, int32_t hop, qb_half* hi, qb_half* lo,
-                        void* stream);
-/* spec [M, ld_spec] fp32 = [re_0..re_{nf-1}, im_0..im_{nf-1}] -> log(clip(|S|,1e-5)), angle/pi planes
- * [B, rows_per_batch, ld] (channels: mag 0..nf-1, phase nf..2nf-1, zero pad); imag of DC/Nyquist
- * forced to +0 (vq/codec_encoder.py:68-71). */
-int qb_stft_post(const float* spec, int64_t ld_spec, int64_t B, int64_t frames, int32_t nf, qb_half* hi,
-                 qb_half* lo, int64_t ld, int64_t rows_per_batch, int64_t row_off, void* stream);
-/* Two-stage STFT (n_fft = P*Q; P <= 64, Q <= 64): the same spectrum as the one-GEMM form above with MMA chains of 4 / 8
- * instead of n_fft/16 - the tensor core truncates on every accumulate, and at K = 1920 that bias is 25x an fp32 FFT's error
- * (csrc/elementwise.cu).   gather -> qb_gemm [.., 64] x W_A[2P, 64] -> twiddle -> qb_gemm [.., 128] x W_B[2*(nf/P+1), 128] -> post2.
+/* Two-stage STFT (n_fft = P*Q; P <= 64, Q <= 64) of the padded, windowed frames (vq/codec_encoder.py:65-71): MMA chains of
+ * 4 / 8 instead of the n_fft/16 of one K = n_fft DFT GEMM - the tensor core truncates on every accumulate, and at K = 1920 that
+ * bias is 25x an fp32 FFT's error (csrc/elementwise.cu).
+ * gather -> qb_gemm [.., 64] x W_A[2P, 64] -> twiddle -> qb_gemm [.., 128] x W_B[2*(nf/P+1), 128] -> post2.
  * qb_stft_gather: planes [(B*F*Q), 64], row (clip, f, b) col a = pad(wav)[hop f + Q a + b] * window[Q a + b].
  * qb_stft_twiddle: Y [(frames_total*Q), ldY] (cols 2 k1, 2 k1 + 1 = re, im) x twiddle[b*P + k1] = (cos, -sin)(2 pi k1 b / n_fft)
  *   -> planes [(frames_total*P), 128] (cols b = re, Q + b = im).
- * qb_stft_post2: as qb_stft_post with X[k] = row (clip, f, k % P), cols 2 (k / P), 2 (k / P) + 1 of X [.., ldX]. */
+ * qb_stft_post2: X[k] = row (clip, f, k % P), cols 2 (k / P), 2 (k / P) + 1 of X [.., ldX] -> log(clip(|X|,1e-5)), angle/pi
+ *   planes [B, rows_per_batch, ld] (channels: mag 0..nf-1, phase nf..2nf-1, zero pad); imag of DC/Nyquist forced to +0. */
 int qb_stft_gather(const float* wav, int64_t B, int64_t T, int32_t hop, int32_t n_fft, int32_t P, int32_t Q, const float* window,
                    qb_half* hi, qb_half* lo, void* stream);
 int qb_stft_twiddle(const float* Y, int64_t ldY, int64_t frames_total, int32_t P, int32_t Q, const float* twiddle, qb_half* hi,

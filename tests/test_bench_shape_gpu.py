@@ -124,7 +124,7 @@ def test_h2_index_identity_full_batch(lib):
         assert a["tokens"] == int(ok.sum()) * 125 and a["explained"], f"{tag}: unexplained index difference {a}"
         # RVQ kernel alone on the ORACLE's embedding: bit-exact on every one of the clips*125*16 decisions (all clips)
         allrows = o.float().transpose(1, 2).reshape(B * N, D)
-        qz = model.engine().rvq(0 if q == "quantizer" else 1) if model._use_engine() else (model.quantizer if q == "quantizer" else model.semantic_quantizer)
+        qz = model.engine().rvq(0 if q == "quantizer" else 1)
         idx, _ = qz.encode_rows(allrows.cuda())
         same = torch.equal(idx.cpu().reshape(B, N, -1).transpose(1, 2), want)
         if not same:

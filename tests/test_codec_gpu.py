@@ -139,24 +139,28 @@ def test_h2_full_config_vs_oracle(lib):
 
 
 def test_h2_ragged_sizes_vs_oracle(lib):
-    """odd batch / token counts (partial M tiles, LSTM groups with < 32 rows, CTA-pair fallbacks)"""
+    """odd batch / token counts (partial M tiles, LSTM groups with < 32 rows, CTA-pair fallbacks), at the small config and at
+    a mid-width one (512 channels, 16 quantisers of 1024 codes)"""
     from oracle import hcodec2, weights
-    cfg = weights.h2_small()
-    model, sd = build(cfg, 5, "mixed")
-    for B, ntok in ((1, 1), (3, 5), (33, 2)):
-        wav, feat = weights.synth_inputs(cfg, B, ntok, 77 + B)
-        oa, os_ = hcodec2.codec_encode(sd, cfg, wav, feat)
-        emb = hcodec2.encoder_forward(sd, cfg["encoder_config"], wav)
-        taps = {}
-        ac, sc = model.encode(wav.cuda(), feat.cuda(), taps=taps)
-        rec = model.decode(oa.cuda(), os_.cuda())
-        torch.cuda.synchronize()
-        ref = hcodec2.codec_decode(sd, cfg, oa, os_)
-        print(f"[ragged B={B} N={ntok}] emb rel {rel(taps['enc.out'], emb):.2e} wav rel {rel(rec, ref):.2e} "
-              f"code match {float((ac.cpu() == oa).float().mean()):.4f}")
-        assert rel(taps["enc.out"], emb) < TOL and rel(rec, ref) < TOL and rec.shape == (B, ntok * 3840)
-        with pytest.raises(ValueError):
-            model.encode(wav[:, :-1].cuda(), feat.cuda())          # length not a multiple of 3840 (pad_wav contract)
+    for widths, shapes in ((dict(), ((1, 1), (3, 5), (33, 2))),
+                           (dict(dim=512, inter=1536, enc_layers=3, dec_layers=4, tf_layers=2, sem_ch=512, nq=16, cb=1024, qdim=512),
+                            ((1, 4),))):
+        cfg = weights.h2_small(**widths)
+        model, sd = build(cfg, 5, "mixed")
+        for B, ntok in shapes:
+            wav, feat = weights.synth_inputs(cfg, B, ntok, 77 + B)
+            oa, os_ = hcodec2.codec_encode(sd, cfg, wav, feat)
+            emb = hcodec2.encoder_forward(sd, cfg["encoder_config"], wav)
+            taps = {}
+            ac, sc = model.encode(wav.cuda(), feat.cuda(), taps=taps)
+            rec = model.decode(oa.cuda(), os_.cuda())
+            torch.cuda.synchronize()
+            ref = hcodec2.codec_decode(sd, cfg, oa, os_)
+            print(f"[ragged dim={cfg['encoder_config']['dim']} B={B} N={ntok}] emb rel {rel(taps['enc.out'], emb):.2e} "
+                  f"wav rel {rel(rec, ref):.2e} code match {float((ac.cpu() == oa).float().mean()):.4f}")
+            assert rel(taps["enc.out"], emb) < TOL and rel(rec, ref) < TOL and rec.shape == (B, ntok * 3840)
+            with pytest.raises(ValueError):
+                model.encode(wav[:, :-1].cuda(), feat.cuda())          # length not a multiple of 3840 (pad_wav contract)
 
 
 def test_h2_full_size_properties(lib):

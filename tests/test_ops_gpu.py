@@ -267,22 +267,45 @@ def test_spectral(lib):
     from unified_audio_b200 import ops
     B, F_, n_fft = 2, 7, 1920
     hop, nf = n_fft // 2, n_fft // 2 + 1
-    T = F_ * hop
+    P, Q = 64, 30                                  # two-stage STFT factors of n_fft (include/quark_b200.h)
+    T, M = F_ * hop, B * F_
+    # gather: row (clip, f, b), col a = pad(wav)[hop f + Q a + b] * window[Q a + b]
     wav = _mk((B, T), 51, 0.1)
-    hb = ops.Planes.zeros((B, F_ + 1, hop), True, DEV)
-    ops.wav_to_hopblocks(wav, hop, hb)
+    win = _mk((n_fft,), 55).abs()
+    ga = ops.Planes.zeros((M * Q, 64), True, DEV)
+    ops.stft_gather(wav, hop, n_fft, P, Q, win, ga)
     torch.cuda.synchronize()
-    padded = torch.nn.functional.pad(wav, (hop // 2, hop // 2))
-    assert relerr(planes_ref(hb).reshape(B, -1), padded) < 1e-6
-    spec = _mk((B * F_, 2 * nf), 52)
+    pad = (n_fft - hop) // 2
+    xw = torch.nn.functional.pad(wav.double(), (pad, pad)).unfold(1, n_fft, hop) * win.double()       # [B, F, n_fft]
+    assert xw.shape[1] == F_
+    assert relerr(planes_ref(ga), xw.reshape(B, F_, P, Q).transpose(2, 3).reshape(M * Q, P)) < 1e-6
+    # twiddle: row (clip-frame, k1), cols b / Q + b = re / im of Y[(clip-frame, b), k1] * (cos, -sin)(2 pi k1 b / n_fft)
+    Y = _mk((M * Q, 2 * P), 52)
+    ang = 2 * math.pi * torch.arange(Q, dtype=torch.float64)[:, None] * torch.arange(P, dtype=torch.float64)[None] / n_fft
+    tw = torch.stack([torch.cos(ang), -torch.sin(ang)], -1).reshape(Q * P, 2).float().to(DEV)
+    Z = ops.Planes.zeros((M * P, 128), True, DEV)
+    ops.stft_twiddle(Y, 2 * P, M, P, Q, tw, Z)
+    torch.cuda.synchronize()
+    yc = torch.view_as_complex(Y.double().reshape(M, Q, P, 2).contiguous())
+    z = (yc * torch.view_as_complex(tw.double().reshape(Q, P, 2).contiguous())).transpose(1, 2)            # [M, P, Q]
+    got = planes_ref(Z).reshape(M, P, 128)
+    assert relerr(got[..., :Q], z.real) < 1e-6 and relerr(got[..., Q:2 * Q], z.imag) < 1e-6
+    # post2: X[k] at row (clip, f, k % P), cols 2 (k / P), 2 (k / P) + 1 -> log(clip(|X|, 1e-5)), angle / pi, zero pad columns
+    K2 = (nf - 1) // P + 1
+    ldX = (2 * K2 + 3) // 4 * 4
+    X = _mk((M * P, ldX), 56)
     dst = ops.Planes.zeros((B, F_ + 2, 1984), True, DEV)
-    ops.stft_post(spec, 2 * nf, B, F_, nf, dst, 1984, F_ + 2, 1)
+    dst.hi.fill_(1.0)
+    dst.lo.fill_(1.0)                              # the padding columns must be written, not left as they were
+    ops.stft_post2(X, ldX, B, F_, nf, P, dst, 1984, F_ + 2, 1)
     torch.cuda.synchronize()
-    re, im = spec[:, :nf].double(), spec[:, nf:].double().clone()
+    k = torch.arange(nf)
+    Xr = X.double().reshape(M, P, ldX)
+    re, im = Xr[:, k % P, 2 * (k // P)], Xr[:, k % P, 2 * (k // P) + 1].clone()
     im[:, 0] = 0; im[:, -1] = 0
     mag = torch.log(torch.clip(torch.sqrt(re * re + im * im), min=1e-5))
     ph = torch.atan2(im, re) / math.pi
-    got = planes_ref(dst)[:, 1:-1].reshape(B * F_, 1984)
+    got = planes_ref(dst)[:, 1:-1].reshape(M, 1984)
     assert relerr(got[:, :nf], mag) < 1e-5 and relerr(got[:, nf:2 * nf], ph) < 1e-5
     assert float(got[:, 2 * nf:].abs().max()) == 0
     head = _mk((B * F_, 2 * nf), 53)

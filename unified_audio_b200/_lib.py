@@ -72,8 +72,6 @@ SIGNATURES = {
     "qb_groupnorm_stats": (C.c_int, [_vp, _i64, _i64, _i64, _i32, _f32, _vp, _vp]),
     "qb_groupnorm_apply": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _i64, _i64,
                                       _i64, _vp]),
-    "qb_wav_to_hopblocks": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _vp, _vp]),
-    "qb_stft_post": (C.c_int, [_vp, _i64, _i64, _i64, _i32, _vp, _vp, _i64, _i64, _i64, _vp]),
     "qb_stft_gather": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "qb_stft_twiddle": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _vp]),
     "qb_stft_post2": (C.c_int, [_vp, _i64, _i64, _i64, _i32, _i32, _vp, _vp, _i64, _i64, _i64, _vp]),

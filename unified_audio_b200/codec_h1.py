@@ -9,19 +9,23 @@ state_dict keys are the reference's, including the old-style weight-norm pairs `
 SEANet encoder = strided / reflect-padded conv stack (encoder_modules/seanet.py:121-208): every conv runs as a
 TMA-im2col GEMM over a reflect-filled channel-last plane buffer; decoder = sub-pixel x2 up-sampler (vq/conv.py:60-93)
 + the H-Codec-2.0 block set at width 768 (8 heads of 96) + ISTFT(1280, hop 320).
+
+This face is orchestrated from Python: `encode` / `decode` launch the libquark_b200 kernels op by op on the current CUDA
+stream, from weights repacked here at first use.  `CodecH15` (codec_h15.py) builds on it.  The H-Codec-2.0 `Codec`
+(codec.py) is backed by the C engine instead.  There is no PyTorch / CPU fallback.
 """
 from __future__ import annotations
 
 import math
+import os
 from typing import Dict
 
 import torch
 
 from . import ops
-from .codec import Codec, _Tree, _pad_to, _planes_from_f64, PRECISION_POLICIES
-from .ops import ACT_ELU, ACT_NONE, Planes, rowmap
+from .codec import _CodecFace, _Tree, _pad_to, PRECISION_POLICIES
+from .ops import ACT_ELU, ACT_GELU, ACT_NONE, ACT_SWIGLU, Planes, rowmap
 from .rvq import ResidualVQ
-from torch import nn
 
 RATIOS = [2, 4, 5, 8]          # SEANetEncoder reverses ratios=[8,5,4,2] (seanet.py:111)
 H1 = dict(n_filters=32, dimension=512, dec_dim=768, dec_inter=2304, dec_layers=12, n_fft=1280, hop=320, nq=4,
@@ -114,10 +118,10 @@ def h1_spec(c) -> Dict[str, Dict[str, tuple]]:
     return dict(encoder=enc, decoder=dec, semantic_encoder=sem)
 
 
-class CodecH1(Codec):
+class CodecH1(_CodecFace):
     def __init__(self, encoder_kwargs: dict = None, decoder_kwargs: dict = None, quantizer_kwargs: dict = None,
                  precision: str = "mixed", _cfg: dict = None):
-        nn.Module.__init__(self)
+        super().__init__()
         c = dict(_cfg or H1)
         self.c = c
         sp = h1_spec(c)
@@ -131,9 +135,12 @@ class CodecH1(Codec):
                             channel_ratios=[1] * len(c["sem_strides"]))
         self.dec_cfg = dict(dim=c["dec_dim"], intermediate_dim=c["dec_inter"])
         self.policy = dict(PRECISION_POLICIES[precision])
-        self._w, self._ws = None, {}
-        self.precision, self.engine_mode, self._engine = precision, "python", None     # H-Codec-1.0 is orchestrated from this file
+        self._w, self._ws = None, {}        # repacked weights (device planes), workspace cache
+        self.precision = precision
         self.eval()
+
+    def _drop_prepared(self):
+        self._w, self._ws = None, {}
 
     # ------------------------------------------------------------------ weight repack
     def _prepare(self):
@@ -160,8 +167,6 @@ class CodecH1(Codec):
                         cout=v.shape[0], cin=v.shape[1])
 
         f32 = lambda k: sd[k].float().contiguous()
-        # reuse the H-Codec-2.0 block packers through a temporary view of this module as its `sd`
-        base = Codec.__new__(Codec)
         stages = []
         idx = 1
         for r in c.get("ratios", RATIOS):
@@ -245,6 +250,91 @@ class CodecH1(Codec):
                 w2=lw(sd[p + "mlp.w2.weight"], "mlp")))
         return layers
 
+    # ------------------------------------------------------------------ workspace
+    def _buf(self, name, shape, dtype=torch.float32):
+        key = (name, tuple(shape), dtype)
+        t = self._ws.get(key)
+        if t is None:
+            t = torch.zeros(shape, dtype=dtype, device=next(self.parameters()).device)
+            self._ws[key] = t
+        return t
+
+    def _planes(self, name, shape, split):
+        key = ("P", name, tuple(shape), bool(split))
+        p = self._ws.get(key)
+        if p is None:
+            p = Planes.zeros(shape, split, next(self.parameters()).device)
+            self._ws[key] = p
+        return p
+
+    def _rope(self, T, D=64):
+        key = ("rope", T, D)
+        r = self._ws.get(key)
+        if r is None:
+            inv = 1.0 / (10000.0 ** (torch.arange(0, D, 2, dtype=torch.int64).float() / D))
+            fr = torch.arange(T).float()[:, None] * inv[None, :]
+            emb = torch.cat((fr, fr), dim=-1)
+            dev = next(self.parameters()).device
+            r = (emb.cos().to(dev).contiguous(), emb.sin().to(dev).contiguous())
+            self._ws[key] = r
+        return r
+
+    # ------------------------------------------------------------------ blocks
+    def _linear(self, a, w, n, M, K, **kw):
+        ops.gemm(a, w, n, a_batch=1, a_rows_per_batch=M, a_ld=K, m_per_batch=M, **kw)
+
+    def _convnext(self, blocks, x, B, F, C, I):
+        M = B * F
+        pol = self.policy["convnext"]
+        t1 = self._planes("cnx_t1", (M, C), pol)
+        hid = self._planes("cnx_hid", (M, I), pol)
+        xm = rowmap(x, C, M, 0)
+        for blk in blocks:
+            ops.dwconv7_ln(x, blk["dw_w"], blk["dw_b"], blk["ln_w"], blk["ln_b"], B, F, C, t1)
+            self._linear(t1, blk["w1"], I, M, C, bias=blk["b1"], act=ACT_GELU, out_planes=hid, out_planes_map=(I, M, 0))
+            self._linear(hid, blk["w2"], C, M, I, bias=blk["b2"], gamma=blk["gamma"], residual=xm, out_f32=xm)
+
+    def _transformer(self, layers, x, B, F, C, heads=None):
+        """encoder_modules/transformer.py:367-393 per layer; x [B*F, C] fp32 updated in place."""
+        heads = heads or C // 64
+        hd = C // heads
+        M, I = B * F, min(4 * C, 4096)
+        pa, pm = self.policy["lstm_attn"], self.policy["mlp"]
+        t_a = self._planes("tf_a", (M, C), pa)
+        t_b = self._planes("tf_b", (M, C), pa)
+        t_m = self._planes("tf_m", (M, C), pm)
+        hid = self._planes("tf_hid", (M, I), pm)
+        xp = self._buf("tf_xp", (M, 4 * C))
+        qkv = self._buf("tf_qkv", (M, 3 * C))
+        use_tc = layers[0]["whh_perm"] is not None and B <= 256
+        ws = self._buf("lstm_ws", (max(ops.lstm_workspace_bytes(B, C), ops.lstm_tc_workspace_bytes(B, C)),), torch.uint8)
+        lstm_u = ops.lstm_tc_units(C) if use_tc else 0
+        cos, sin = self._rope(F, hd)
+        legacy = os.environ.get("QB_ATTENTION", "umma") == "legacy"
+        umma = (not legacy) and hd in (64, 128)          # wgmma attention (csrc/attention_umma.cu), both precision policies
+        tc_att = (not umma) and (not pa) and hd == 64
+        att_ws = (self._buf("att5_ws", (ops.attention_umma_workspace_bytes(B, F, heads, hd, pa),), torch.uint8) if umma else
+                  self._buf("att_ws", (ops.attention_tc_workspace_bytes(B, F, heads),), torch.uint8) if tc_att else None)
+        xm = rowmap(x, C, M, 0)
+        for L in layers:
+            ops.rmsnorm(x, L["in_w"], M, C, t_a)
+            self._linear(t_a, L["wih"], 4 * C, M, C, bias=L["b_ih"], out_f32=rowmap(xp, 4 * C, M, 0))
+            if use_tc:
+                ops.lstm_tc(xp, L["whh_perm"], lstm_u, B, F, C, t_b, ws)
+            else:
+                ops.lstm(xp, L["whh"], B, F, C, t_b, ws)
+            self._linear(t_b, L["wqkv"], 3 * C, M, C, bias=L["bqkv"], out_f32=rowmap(qkv, 3 * C, M, 0))
+            if umma:
+                ops.attention_umma(qkv, B, F, heads, hd, cos, sin, t_a, att_ws, split=pa)
+            elif tc_att:   # legacy: single-pass fp16 policy, head_dim 64: mma.sync flash attention
+                ops.attention_tc(qkv, B, F, heads, cos, sin, t_a, att_ws)
+            else:        # split-precision policy or head_dim 96: fp32 SIMT attention
+                ops.attention_hd(qkv, B, F, heads, hd, cos, sin, t_a)
+            self._linear(t_a, L["wo"], C, M, C, residual=xm, out_f32=xm)
+            ops.rmsnorm(x, L["post_w"], M, C, t_m)
+            self._linear(t_m, L["w13"], 2 * I, M, C, act=ACT_SWIGLU, out_planes=hid, out_planes_map=(I, M, 0))
+            self._linear(hid, L["w2"], C, M, I, residual=xm, out_f32=xm)
+
     # ------------------------------------------------------------------ SEANet encoder
     def _sconv(self, src: Planes, cw, B, T_in, stride, *, src_rpb, bias=True, residual=None, out_f32=None, out=None,
                out_map=(0, 0, 0), act2=ACT_NONE):
@@ -318,7 +408,67 @@ class CodecH1(Codec):
             taps["enc.out"] = emb.reshape(B, N, ch).transpose(1, 2).clone()
         return emb, N
 
+    def _encode_sem(self, feat: torch.Tensor, taps=None):
+        """vq/semantic_module.py:196-201 -> [B*N, out_channels] fp32."""
+        W = self._prepare()
+        S, cfg = W["sem"], self.sem_cfg
+        B, Cin, F = feat.shape
+        Cs, Co = cfg["encode_channels"], cfg["out_channels"]
+        pc = self.policy["conv"]
+        cin_pad = _pad_to(Cin, 64)
+        fin = self._planes("sem_in", (B, F + 2, cin_pad), pc)
+        ops.bct_to_planes(feat.float().contiguous(), fin, cin_pad, F + 2, 1)
+        Tc = F
+        sx = self._buf(f"sem_x{Tc}", (B * Tc, Cs))
+        pe = self._planes(f"sem_pe{Tc}", (B, Tc + 2, Cs), pc)
+        ops.gemm(fin, S["conv"], Cs, a_batch=B, a_rows_per_batch=F + 2, a_ld=cin_pad, m_per_batch=F, taps=3,
+                 out_f32=rowmap(sx, Cs, Tc, 0), out_planes=pe, out_planes_map=(Cs, Tc + 2, 1), act2=ACT_ELU)
+        nb = len(S["blocks"])
+        for bi, blk in enumerate(S["blocks"]):
+            pu = self._planes(f"sem_pu{Tc}", (B, Tc, Cs), pc)
+            for u, un in enumerate(blk["units"]):
+                ops.gemm(pe, un["c1"], Cs, a_batch=B, a_rows_per_batch=Tc + 2, a_ld=Cs, m_per_batch=Tc, taps=3,
+                         act=ACT_ELU, out_planes=pu, out_planes_map=(Cs, Tc, 0))
+                ops.gemm(pu, un["c2"], Cs, a_batch=B, a_rows_per_batch=Tc, a_ld=Cs, m_per_batch=Tc,
+                         residual=rowmap(sx, Cs, Tc, 0), out_f32=rowmap(sx, Cs, Tc, 0), out_planes=pe,
+                         out_planes_map=(Cs, Tc + 2, 1), act2=ACT_ELU if u == 0 else ACT_NONE)
+            st, k = blk["stride"], blk["k"]
+            pad = (k - 1) // 2
+            if pad != 1 or (Tc + 2) % st != 0:
+                raise ValueError(f"semantic encoder: {Tc} frames cannot be strided by {st} with kernel {k} (frame count must be even)")
+            Tn = (Tc + 2 * pad - k) // st + 1
+            sx2 = self._buf(f"sem_x{Tn}_{bi}", (B * Tn, Cs))
+            pe2 = self._planes(f"sem_pe{Tn}_{bi}", (B, Tn + 2, Cs), pc)
+            ops.gemm(pe, blk["conv"], Cs, a_batch=B, a_rows_per_batch=Tc + 2, a_ld=Cs, m_per_batch=Tn, taps=k, stride=st,
+                     bias=blk["conv_b"], out_f32=rowmap(sx2, Cs, Tn, 0), out_planes=pe2, out_planes_map=(Cs, Tn + 2, 1),
+                     act2=ACT_ELU if bi + 1 < nb else ACT_NONE)
+            sx, pe, Tc = sx2, pe2, Tn
+            if taps is not None:
+                taps[f"sem.block{bi}"] = sx.reshape(B, Tc, Cs).transpose(1, 2).clone()
+        out = self._buf("sem_out", (B * Tc, Co))
+        ops.gemm(pe, S["conv2"], Co, a_batch=B, a_rows_per_batch=Tc + 2, a_ld=Cs, m_per_batch=Tc, taps=3,
+                 out_f32=rowmap(out, Co, Tc, 0))
+        if taps is not None:
+            taps["sem.out"] = out.reshape(B, Tc, Co).transpose(1, 2).clone()
+        return out, Tc
+
     # ------------------------------------------------------------------ decoder
+    def _resnet(self, R, x, B, F, C):
+        """vq/conv.py:286-303."""
+        M = B * F
+        pc = self.policy["conv"]
+        stats = self._buf("gn_stats", (B, 32, 2))
+        pr = self._planes("res_pr", (B, F + 2, C), pc)
+        h = self._buf("res_h", (M, C))
+        ops.groupnorm_stats(x, B, F, C, stats)
+        ops.groupnorm_apply(x, stats, R["n1w"], R["n1b"], B, F, C, True, out=pr, ld=C, rows_per_batch=F + 2, row_off=1)
+        ops.gemm(pr, R["c1"], C, a_batch=B, a_rows_per_batch=F + 2, a_ld=C, m_per_batch=F, taps=3, bias=R["c1b"],
+                 out_f32=rowmap(h, C, F, 0))
+        ops.groupnorm_stats(h, B, F, C, stats)
+        ops.groupnorm_apply(h, stats, R["n2w"], R["n2b"], B, F, C, True, out=pr, ld=C, rows_per_batch=F + 2, row_off=1)
+        ops.gemm(pr, R["c2"], C, a_batch=B, a_rows_per_batch=F + 2, a_ld=C, m_per_batch=F, taps=3, bias=R["c2b"],
+                 residual=rowmap(x, C, F, 0), out_f32=rowmap(x, C, F, 0))
+
     def _decode_z(self, z: torch.Tensor, B: int, N: int, taps=None):
         """vq/codec_decoder.py:54-66 -> wav [B, N*640]."""
         W = self._prepare()
@@ -363,3 +513,34 @@ class CodecH1(Codec):
         wav = torch.empty(B, F * hop, device=z.device)
         ops.istft_ola(frames, D["window"], B, F, n_fft, wav, hop)
         return wav
+
+    # ------------------------------------------------------------------ public surface
+    @torch.no_grad()
+    def encode(self, x, feat, taps=None):
+        """vq/codec.py:165-174: x [B,1,T] fp32, feat [B,768,T/320] fp32 -> (acoustic, semantic) int64 [B,nq,N]."""
+        emb, N = self._encode_emb(x, taps)
+        sem, Ns = self._encode_sem(feat, taps)
+        if Ns != N:
+            raise ValueError(f"semantic stream has {Ns} frames but the acoustic stream has {N}")
+        B = x.shape[0]
+        ia, _ = self.quantizer.encode_rows(emb, want_quantized=False)
+        isem, _ = self.semantic_quantizer.encode_rows(sem, want_quantized=False)
+        return (ia.reshape(B, N, -1).transpose(1, 2).contiguous(), isem.reshape(B, N, -1).transpose(1, 2).contiguous())
+
+    @torch.no_grad()
+    def decode(self, acoustic_codes, semantic_codes, taps=None):
+        """vq/codec.py:177-186: int64 [B,nq,N] x2 -> wav [B, N*640]."""
+        B, nq, N = acoustic_codes.shape
+        Dq = self.quantizer.dim
+        z = self._buf("dec_z", (B * N, 2 * Dq))
+        ia = acoustic_codes.transpose(1, 2).reshape(B * N, nq).long().contiguous()
+        isem = semantic_codes.transpose(1, 2).reshape(B * N, nq).long().contiguous()
+        self.quantizer.decode_rows(ia, z, 2 * Dq, 0)
+        self.semantic_quantizer.decode_rows(isem, z, 2 * Dq, Dq)
+        return self._decode_z(z, B, N, taps)
+
+
+def _planes_from_f64(w: torch.Tensor, split: bool) -> Planes:
+    hi = w.clamp(-65504.0, 65504.0).half()
+    lo = (w - hi.double()).half() if split else None
+    return Planes(hi.contiguous(), lo.contiguous() if lo is not None else None)

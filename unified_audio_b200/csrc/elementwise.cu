@@ -347,34 +347,6 @@ __global__ void groupnorm_apply_kernel(const float* __restrict__ x, const float*
 }
 
 // ------------------------------------------------------------------ spectral
-__global__ void wav_to_hopblocks_kernel(const float* __restrict__ wav, long long T, int hop, int pad,
-                                        __half* __restrict__ hi, __half* __restrict__ lo, long long per_batch) {
-  const int b = blockIdx.y;
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= per_batch) return;
-  long long src = i - pad;
-  float v = (src >= 0 && src < T) ? wav[(long long)b * T + src] : 0.f;
-  store_planes(hi, lo, (long long)b * per_batch + i, v);
-}
-
-__global__ void stft_post_kernel(const float* __restrict__ spec, long long ld_spec, int frames, int nf,
-                                 __half* __restrict__ hi, __half* __restrict__ lo, long long ld, long long rpb,
-                                 long long off) {
-  const int f = blockIdx.x, b = blockIdx.y;
-  const float* sp = spec + ((long long)b * frames + f) * ld_spec;
-  const long long o = ((long long)b * rpb + off + f) * ld;
-  for (int k = threadIdx.x; k < ld; k += blockDim.x) {
-    if (k < nf) {
-      float re = sp[k], im = (k == 0 || k == nf - 1) ? 0.f : sp[nf + k];
-      float mag = hypotf(re, im);
-      store_planes(hi, lo, o + k, logf(fmaxf(mag, 1e-5f)));
-      store_planes(hi, lo, o + nf + k, atan2f(im, re) * 0.31830988618379067154f);
-    } else if (k >= 2 * nf) {
-      store_planes(hi, lo, o + k, 0.f);
-    }
-  }
-}
-
 __global__ void istft_pre_kernel(const float* __restrict__ head, long long ld_in, int nf, __half* __restrict__ hi,
                                  __half* __restrict__ lo, long long ld) {
   const long long m = blockIdx.x;
@@ -753,25 +725,6 @@ extern "C" int qb_groupnorm_apply(const float* x, const float* stats, const floa
   dim3 grid((unsigned)T, (unsigned)B);
   groupnorm_apply_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, stats, w, b, (int)T, (int)C, groups, swish, out_f32,
                                                                 (__half*)hi, (__half*)lo, ld, rows_per_batch, row_off);
-  QB_LAUNCH_END();
-}
-
-extern "C" int qb_wav_to_hopblocks(const float* wav, int64_t B, int64_t T, int32_t hop, qb_half* hi, qb_half* lo,
-                                   void* stream) {
-  QB_REQUIRE(wav && hi && T % hop == 0, "wav_to_hopblocks: T must be a multiple of hop");
-  const long long per_batch = T + hop;
-  dim3 grid((unsigned)ceil_div(per_batch, 256), (unsigned)B);
-  wav_to_hopblocks_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(wav, T, hop, hop / 2, (__half*)hi, (__half*)lo,
-                                                                 per_batch);
-  QB_LAUNCH_END();
-}
-
-extern "C" int qb_stft_post(const float* spec, int64_t ld_spec, int64_t B, int64_t frames, int32_t nf, qb_half* hi,
-                            qb_half* lo, int64_t ld, int64_t rows_per_batch, int64_t row_off, void* stream) {
-  QB_REQUIRE(spec && hi && 2 * nf <= ld && 2 * nf <= ld_spec && row_off + frames <= rows_per_batch, "stft_post: bad args");
-  dim3 grid((unsigned)frames, (unsigned)B);
-  stft_post_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(spec, ld_spec, (int)frames, nf, (__half*)hi, (__half*)lo, ld,
-                                                          rows_per_batch, row_off);
   QB_LAUNCH_END();
 }
 

@@ -319,7 +319,7 @@ struct qb_codec {
   void* tap_user = nullptr;
   // geometry
   int nf, feat_ld, spec_ld, kin, lstm_u;
-  PlanesD dft_fwd, dft_inv;
+  PlanesD dft_inv;
   const float* istft_window;
   // two-stage STFT (n_fft = P*Q): stage matrices, twiddle table, analysis window
   int stft_P = 0, stft_Q = 0, stft_nB = 0, stft_ldX = 0;
@@ -564,30 +564,20 @@ static int encode_emb(qb_codec* c, const float* wav, int64_t B, int64_t T, float
   QB_REQUIRE(T > 0 && T % ((int64_t)hop * stride) == 0, "codec_encode: waveform length %lld must be a multiple of %d (pad_wav, audio_tokenizer.py:63-66)",
              (long long)T, hop * stride);
   const int64_t F = T / hop, N = F / stride, M = B * F;
-  PlanesD hb, feat, fin;
-  float *spec, *x0, *x, *emb;
+  PlanesD feat, fin, ga, Z;
+  float *Y, *X, *x0, *x, *emb;
   QB_TRY(c->ws.planes(&feat, "enc_feat", (size_t)B * (F + 2) * c->feat_ld, c->pol.conv));
-  if (c->stft_P) {
-    // two-stage DFT: gather -> P-point DFTs (GEMM, K = 64) -> twiddle -> Q-point DFTs (GEMM, K = 128) -> log-magnitude / phase
-    const int P = c->stft_P, Q = c->stft_Q;
-    PlanesD ga, Z;
-    float *Y, *X;
-    QB_TRY(c->ws.planes(&ga, "enc_sg", (size_t)M * Q * 64, true));
-    QB_TRY(qb_stft_gather(wav, B, T, hop, g.n_fft, P, Q, c->stft_window, (qb_half*)ga.hi, (qb_half*)ga.lo, st));
-    QB_TRY(c->ws.f32(&Y, "enc_sy", (size_t)M * Q * 2 * P));
-    QB_TRY(lin(ga, M * Q, 64, c->stft_wA, 2 * P).out32(Y, 2 * P, M * Q, 0).run(st));
-    QB_TRY(c->ws.planes(&Z, "enc_sz", (size_t)M * P * 128, true));
-    QB_TRY(qb_stft_twiddle(Y, 2 * P, M, P, Q, c->stft_tw, (qb_half*)Z.hi, (qb_half*)Z.lo, st));
-    QB_TRY(c->ws.f32(&X, "enc_sx", (size_t)M * P * c->stft_ldX));
-    QB_TRY(lin(Z, M * P, 128, c->stft_wB, c->stft_nB).out32(X, c->stft_ldX, M * P, 0).run(st));
-    QB_TRY(qb_stft_post2(X, c->stft_ldX, B, F, nf, P, (qb_half*)feat.hi, (qb_half*)feat.lo, c->feat_ld, F + 2, 1, st));
-  } else {
-    QB_TRY(c->ws.planes(&hb, "enc_hb", (size_t)B * (F + 1) * hop, c->pol.dft));
-    QB_TRY(qb_wav_to_hopblocks(wav, B, T, hop, (qb_half*)hb.hi, (qb_half*)hb.lo, st));
-    QB_TRY(c->ws.f32(&spec, "enc_spec", (size_t)M * c->spec_ld));
-    QB_TRY(G(hb, B, F + 1, hop, F, c->dft_fwd, 2 * nf, 2).out32(spec, c->spec_ld, F, 0).run(st));
-    QB_TRY(qb_stft_post(spec, c->spec_ld, B, F, nf, (qb_half*)feat.hi, (qb_half*)feat.lo, c->feat_ld, F + 2, 1, st));
-  }
+  // two-stage DFT: gather -> P-point DFTs (GEMM, K = 64) -> twiddle -> Q-point DFTs (GEMM, K = 128) -> log-magnitude / phase
+  const int P = c->stft_P, Q = c->stft_Q;
+  QB_TRY(c->ws.planes(&ga, "enc_sg", (size_t)M * Q * 64, true));
+  QB_TRY(qb_stft_gather(wav, B, T, hop, g.n_fft, P, Q, c->stft_window, (qb_half*)ga.hi, (qb_half*)ga.lo, st));
+  QB_TRY(c->ws.f32(&Y, "enc_sy", (size_t)M * Q * 2 * P));
+  QB_TRY(lin(ga, M * Q, 64, c->stft_wA, 2 * P).out32(Y, 2 * P, M * Q, 0).run(st));
+  QB_TRY(c->ws.planes(&Z, "enc_sz", (size_t)M * P * 128, true));
+  QB_TRY(qb_stft_twiddle(Y, 2 * P, M, P, Q, c->stft_tw, (qb_half*)Z.hi, (qb_half*)Z.lo, st));
+  QB_TRY(c->ws.f32(&X, "enc_sx", (size_t)M * P * c->stft_ldX));
+  QB_TRY(lin(Z, M * P, 128, c->stft_wB, c->stft_nB).out32(X, c->stft_ldX, M * P, 0).run(st));
+  QB_TRY(qb_stft_post2(X, c->stft_ldX, B, F, nf, P, (qb_half*)feat.hi, (qb_half*)feat.lo, c->feat_ld, F + 2, 1, st));
   QB_TRY(tap_planes(c, "enc.feat", feat, B, F, 2 * nf, c->feat_ld, F + 2, 1, st));
   QB_TRY(c->ws.f32(&x0, "enc_x0", (size_t)M * C));
   QB_TRY(G(feat, B, F + 2, c->feat_ld, F, c->e_embed, C, 3).bias(c->e_embed_b).out32(x0, C, F, 0).run(st));
@@ -771,8 +761,10 @@ extern "C" int qb_rvq_decode_rows(qb_rvq* q, const int64_t* idx, int64_t M, floa
 
 extern "C" int qb_codec_load(qb_handle* h, const qb_codec_cfg* cfg, const qb_tensor* named, int32_t n, qb_codec** out) {
   QB_REQUIRE(h && cfg && named && out && n > 0, "codec_load: bad args");
-  QB_REQUIRE(cfg->n_fft == 2 * cfg->hop_length && cfg->hop_length % 64 == 0,
-             "codec_load: the STFT/ISTFT kernels assume n_fft == 2*hop and hop %% 64 == 0 (shipped config)");
+  // n_fft <= 4096: the two-stage STFT needs n_fft = P*Q with P, Q <= 64
+  QB_REQUIRE(cfg->n_fft == 2 * cfg->hop_length && cfg->hop_length % 64 == 0 && cfg->n_fft <= 4096,
+             "codec_load: the STFT/ISTFT kernels assume n_fft == 2*hop, hop %% 64 == 0 and n_fft <= 4096 (n_fft = P*Q with P, Q <= 64); "
+             "got n_fft %d, hop %d", cfg->n_fft, cfg->hop_length);
   QB_REQUIRE(cfg->dim % 256 == 0 && cfg->dimension % 64 == 0 && cfg->sem_n_blocks >= 0 && cfg->sem_n_blocks <= 8, "codec_load: unsupported widths");
   QB_CHECK_CUDA(cudaSetDevice(h->device));
   WeightTable wt;
@@ -789,58 +781,44 @@ extern "C" int qb_codec_load(qb_handle* h, const qb_codec_cfg* cfg, const qb_ten
     const qb_tensor *we, *wd;
     QB_TRY(L.get(&we, "encoder.stft.window", 1));
     QB_TRY(L.get(&wd, "decoder.head.istft.window", 1));
-    std::vector<float> win_e(n_fft), win_d(n_fft);
-    QB_CHECK_CUDA(cudaMemcpy(win_e.data(), we->data, (size_t)n_fft * 4, cudaMemcpyDeviceToHost));
+    std::vector<float> win_d(n_fft);
     QB_CHECK_CUDA(cudaMemcpy(win_d.data(), wd->data, (size_t)n_fft * 4, cudaMemcpyDeviceToHost));
     const double two_pi = 6.283185307179586476925286766559;
     std::vector<double> cs(n_fft), sn(n_fft);
     for (int r = 0; r < n_fft; ++r) { cs[r] = cos(two_pi * r / n_fft); sn[r] = sin(two_pi * r / n_fft); }
-    std::vector<double> fwd((size_t)2 * nf * n_fft);        // rows [re_0..re_nf-1, im_0..im_nf-1], K = n_fft
-    for (int k = 0; k < nf; ++k)
-      for (int s = 0; s < n_fft; ++s) {
-        const int r = (int)(((long long)k * s) % n_fft);
-        fwd[(size_t)k * n_fft + s] = cs[r] * (double)win_e[s];
-        fwd[(size_t)(nf + k) * n_fft + s] = -sn[r] * (double)win_e[s];
+    // two-stage factorisation n_fft = P*Q with P = 64, Q = n_fft/64 <= 64 (checked above): chains of 4 / 8 MMAs instead of n_fft/16
+    const int P = 64, Q = n_fft / 64, K2 = (nf - 1) / P + 1;
+    c->stft_P = P; c->stft_Q = Q;
+    c->stft_nB = 2 * K2; c->stft_ldX = (int)pad_to(2 * K2, 4);
+    std::vector<double> wA((size_t)2 * P * 64, 0.0), wB((size_t)2 * K2 * 128, 0.0);
+    for (int k1 = 0; k1 < P; ++k1)
+      for (int a = 0; a < P; ++a) {
+        const double ang = two_pi * ((k1 * a) % P) / P;
+        wA[(size_t)(2 * k1) * 64 + a] = cos(ang);
+        wA[(size_t)(2 * k1 + 1) * 64 + a] = -sin(ang);
       }
-    QB_TRY(L.planes_from_f64(&c->dft_fwd, fwd));
-    // two-stage factorisation n_fft = P*Q (P <= 64 as large as possible, Q <= 64): chains of 4 / 8 MMAs instead of n_fft/16
-    const char* stft_env = getenv("QB_STFT");
-    if (!(stft_env && std::string(stft_env) == "gemm"))
-      for (int P = 64; P >= 1; --P)
-        if (n_fft % P == 0 && n_fft / P <= 64) { c->stft_P = P; c->stft_Q = n_fft / P; break; }
-    if (c->stft_P) {
-      const int P = c->stft_P, Q = c->stft_Q, K2 = (nf - 1) / P + 1;
-      c->stft_nB = 2 * K2; c->stft_ldX = (int)pad_to(2 * K2, 4);
-      std::vector<double> wA((size_t)2 * P * 64, 0.0), wB((size_t)2 * K2 * 128, 0.0);
-      for (int k1 = 0; k1 < P; ++k1)
-        for (int a = 0; a < P; ++a) {
-          const double ang = two_pi * ((k1 * a) % P) / P;
-          wA[(size_t)(2 * k1) * 64 + a] = cos(ang);
-          wA[(size_t)(2 * k1 + 1) * 64 + a] = -sin(ang);
-        }
-      for (int k2 = 0; k2 < K2; ++k2)
-        for (int b = 0; b < Q; ++b) {
-          const double ang = two_pi * ((k2 * b) % Q) / Q;
-          wB[(size_t)(2 * k2) * 128 + b] = cos(ang);
-          wB[(size_t)(2 * k2) * 128 + Q + b] = sin(ang);
-          wB[(size_t)(2 * k2 + 1) * 128 + b] = -sin(ang);
-          wB[(size_t)(2 * k2 + 1) * 128 + Q + b] = cos(ang);
-        }
-      QB_TRY(L.planes_from_f64(&c->stft_wA, wA));
-      QB_TRY(L.planes_from_f64(&c->stft_wB, wB));
-      std::vector<float> tw((size_t)Q * P * 2);
-      for (int b = 0; b < Q; ++b)
-        for (int k1 = 0; k1 < P; ++k1) {
-          const double ang = two_pi * ((b * k1) % n_fft) / n_fft;
-          tw[((size_t)b * P + k1) * 2] = (float)cos(ang);
-          tw[((size_t)b * P + k1) * 2 + 1] = (float)(-sin(ang));
-        }
-      float* dtw;
-      QB_TRY(c->arena.alloc((void**)&dtw, tw.size() * 4, false));
-      QB_CHECK_CUDA(cudaMemcpy(dtw, tw.data(), tw.size() * 4, cudaMemcpyHostToDevice));
-      c->stft_tw = dtw;
-      QB_TRY(L.f32(&c->stft_window, "encoder.stft.window"));
-    }
+    for (int k2 = 0; k2 < K2; ++k2)
+      for (int b = 0; b < Q; ++b) {
+        const double ang = two_pi * ((k2 * b) % Q) / Q;
+        wB[(size_t)(2 * k2) * 128 + b] = cos(ang);
+        wB[(size_t)(2 * k2) * 128 + Q + b] = sin(ang);
+        wB[(size_t)(2 * k2 + 1) * 128 + b] = -sin(ang);
+        wB[(size_t)(2 * k2 + 1) * 128 + Q + b] = cos(ang);
+      }
+    QB_TRY(L.planes_from_f64(&c->stft_wA, wA));
+    QB_TRY(L.planes_from_f64(&c->stft_wB, wB));
+    std::vector<float> tw((size_t)Q * P * 2);
+    for (int b = 0; b < Q; ++b)
+      for (int k1 = 0; k1 < P; ++k1) {
+        const double ang = two_pi * ((b * k1) % n_fft) / n_fft;
+        tw[((size_t)b * P + k1) * 2] = (float)cos(ang);
+        tw[((size_t)b * P + k1) * 2 + 1] = (float)(-sin(ang));
+      }
+    float* dtw;
+    QB_TRY(c->arena.alloc((void**)&dtw, tw.size() * 4, false));
+    QB_CHECK_CUDA(cudaMemcpy(dtw, tw.data(), tw.size() * 4, cudaMemcpyHostToDevice));
+    c->stft_tw = dtw;
+    QB_TRY(L.f32(&c->stft_window, "encoder.stft.window"));
     std::vector<double> inv((size_t)n_fft * c->kin, 0.0);    // [n_fft, kin]: 1/N, Hermitian weights, synthesis window folded in
     for (int s = 0; s < n_fft; ++s)
       for (int k = 0; k < nf; ++k) {

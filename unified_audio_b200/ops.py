@@ -170,16 +170,6 @@ def groupnorm_apply(x, stats, w, b, B, T, Cc, swish, out_f32=None, out: Optional
                                               _p(hi), _p(lo), ld, rows_per_batch, row_off, _stream()))
 
 
-def wav_to_hopblocks(wav, hop, out: Planes):
-    B, T = wav.shape
-    _lib.check(_lib.load().qb_wav_to_hopblocks(_p(wav), B, T, hop, _p(out.hi), _p(out.lo), _stream()))
-
-
-def stft_post(spec, ld_spec, B, frames, nf, out: Planes, ld, rows_per_batch, row_off):
-    _lib.check(_lib.load().qb_stft_post(_p(spec), ld_spec, B, frames, nf, _p(out.hi), _p(out.lo), ld, rows_per_batch,
-                                        row_off, _stream()))
-
-
 def stft_gather(wav, hop, n_fft, P, Q, window, out: Planes):
     B, T = wav.shape
     _lib.check(_lib.load().qb_stft_gather(_p(wav), B, T, hop, n_fft, P, Q, _p(window), _p(out.hi), _p(out.lo), _stream()))
