@@ -137,6 +137,13 @@ __device__ __forceinline__ void mbar_wait_parked(uint64_t* bar, uint32_t parity)
   }
 }
 
+// Warpgroup register reallocation (sm_90a): every thread of the warpgroup executes it; the block's pool is fixed at launch by
+// the kernel's register count, so the decreases of some warpgroups must free what the increases of the others take.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 __device__ __forceinline__ void prefetch_tmap(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
 }

@@ -1,12 +1,12 @@
 // Dense contraction kernels: wgmma/TMA persistent GEMM (product path) and a SIMT
 // cross-check.  Both evaluate the same qb_gemm_desc (include/quark_b200.h).
 //
-// Tile: 128 (rows) x 128 (cols) x 64 (K) per pipeline stage, fp16 planes K-major in shared memory
-// with the 128-byte TMA/wgmma swizzle; accumulators live in registers.  Warp roles (384 threads):
-//   warpgroup 0     TMA producer (one thread)
-//   warpgroups 1-2  wgmma m64n128k16 on rows [0, 64) / [64, 128) of the tile, then the epilogue
+// Tile: 128 (rows) x BN (cols, 256 or 128) x 64 (K) per pipeline stage, fp16 planes K-major in shared
+// memory with the 128-byte TMA/wgmma swizzle; accumulators live in registers.  Warp roles (384 threads):
+//   warpgroup 0     TMA producer (one thread), shrunk to 40 registers by setmaxnreg
+//   warpgroups 1-2  wgmma m64nBNk16 on rows [0, 64) / [64, 128) of the tile, then the epilogue
 //                   (bias/act/gamma/residual -> global) straight from the accumulator registers;
-//                   the producer already fills the stages of the next tile meanwhile.
+//                   the producer already fills the stages of the next tile meanwhile.  232 registers each.
 // Convolutions are expressed as `taps` shifted K-panels over a zero-padded channel-last buffer:
 // the A tensor map views the buffer as [batch][rows/stride][stride*C], so tap t of output row m is
 // the box at (x = (t % stride)*C + c, y = m + t / stride) - TMA-staged im2col without an im2col
@@ -45,6 +45,13 @@ static int current_device() {
 #define QB_PARK 1
 #endif
 
+// What the epilogue of a launch does, decided on the host so that the consumer branches once per tile:
+//   EPI_HI      (bias) (GELU) -> fp16 hi plane, one half2 store per accumulator pair (ConvNeXt pwconv1)
+//   EPI_F32     (bias) (* gamma) (+ residual) -> fp32, one float2 store per pair (pwconv2, o-proj, w2, residual convs)
+//   EPI_GENERIC every other combination, element by element through epilogue_pair
+// The two fast kinds need an even N and even pitches / 8-byte aligned bases, so that every in-range pair is one aligned vector.
+enum EpiKind : int { EPI_GENERIC = 0, EPI_HI = 1, EPI_F32 = 2 };
+
 struct RowMapD {
   void* ptr;
   long long ld, rpb, off;
@@ -60,6 +67,7 @@ struct GemmParams {
   const float* act2_p;   // per-column parameter of `act2`
   RowMapD res, o32, ohi, olo;
   int act, act2;
+  int epi;               // EpiKind, classified once per launch by fill_params
   // SIMT path only
   const __half *a_hi, *a_lo, *w_hi, *w_lo;
   long long a_rpb;
@@ -160,15 +168,68 @@ __device__ __forceinline__ void epilogue_pair(const GemmParams& p, int b, int m,
   if (has1) epi_finish_scalar(p, b, m, n + 1, v1);
 }
 
-constexpr int GEMM_BM = 128, GEMM_BN = 128, GEMM_BK = 64;
+constexpr int GEMM_BM = 128, GEMM_BK = 64;
 constexpr int GEMM_THREADS = 3 * 128;           // warpgroup 0: TMA producer; warpgroups 1-2: MMA + epilogue, 64 rows each
+// register split after setmaxnreg: 128 * 40 + 256 * 232 = 64512 of the SM's 65536 (the launch reserves 384 * 168)
+constexpr int GEMM_PRODUCER_REGS = 40, GEMM_CONSUMER_REGS = 232;
 
-template <int NTERMS, int STAGES>
+// Fast epilogue kinds: accumulator pair (rows r, r + 8; columns n, n + 1 for n = c + 8j) -> one vector store each.
+// Same arithmetic, in the same order, as the vectorised branches of epilogue_pair.
+template <int BN>
+__device__ __forceinline__ void epilogue_hi(const GemmParams& p, int b, int r, int c, const float (&acc)[BN / 2]) {
+  const __half2 hmax = __float2half2_rn(65504.f), hmin = __float2half2_rn(-65504.f);
+  const bool gelu = p.act == QB_ACT_GELU;
+  __half* base = (__half*)p.ohi.ptr + ((long long)b * p.ohi.rpb + p.ohi.off + r) * p.ohi.ld;
+  const long long row8 = 8 * p.ohi.ld;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = c + 8 * j;
+    if (n >= p.N) break;
+    const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.f, 0.f);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (r + 8 * h >= p.m_per_batch) continue;
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      if (p.bias) { v0 += bb.x; v1 += bb.y; }
+      if (gelu) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
+      *reinterpret_cast<__half2*>(base + h * row8 + n) = __hmax2(__hmin2(__floats2half2_rn(v0, v1), hmax), hmin);
+    }
+  }
+}
+
+template <int BN>
+__device__ __forceinline__ void epilogue_f32(const GemmParams& p, int b, int r, int c, const float (&acc)[BN / 2]) {
+  float* base = (float*)p.o32.ptr + ((long long)b * p.o32.rpb + p.o32.off + r) * p.o32.ld;
+  const float* rbase = p.res.ptr ? (const float*)p.res.ptr + ((long long)b * p.res.rpb + p.res.off + r) * p.res.ld : nullptr;
+  const long long row8 = 8 * p.o32.ld, rrow8 = 8 * p.res.ld;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = c + 8 * j;
+    if (n >= p.N) break;
+    const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.f, 0.f);
+    const float2 g = p.gamma ? __ldg(reinterpret_cast<const float2*>(p.gamma + n)) : make_float2(1.f, 1.f);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (r + 8 * h >= p.m_per_batch) continue;
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      if (p.bias) { v0 += bb.x; v1 += bb.y; }
+      if (p.gamma) { v0 *= g.x; v1 *= g.y; }
+      if (rbase) {
+        const float2 rv = *reinterpret_cast<const float2*>(rbase + h * rrow8 + n);
+        v0 += rv.x; v1 += rv.y;
+      }
+      *reinterpret_cast<float2*>(base + h * row8 + n) = make_float2(v0, v1);
+    }
+  }
+}
+
+// One kernel for every qb_gemm: BM x BN x 64 tiles, BN = 256 (wgmma m64n256k16, 128 accumulators per thread) or 128.
+template <int NTERMS, int BN, int STAGES>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
                const GemmParams p) {
-  constexpr int BM = GEMM_BM, BN = GEMM_BN, BK = GEMM_BK;
+  constexpr int BM = GEMM_BM, BK = GEMM_BK;
   constexpr int NPL = (NTERMS == 1) ? 1 : 2;
   constexpr uint32_t A_BYTES = BM * BK * 2, W_BYTES = BN * BK * 2;
   constexpr uint32_t STAGE_BYTES = NPL * (A_BYTES + W_BYTES);
@@ -191,6 +252,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   __syncthreads();
 
   if (wg == 0) {
+    setmaxnreg_dec<GEMM_PRODUCER_REGS>();
     if (threadIdx.x == 0) {
       uint32_t stage = 0, phase = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
@@ -212,6 +274,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       }
     }
   } else {
+    setmaxnreg_inc<GEMM_CONSUMER_REGS>();
     const int cw = wg - 1, wq = warp & 3;      // consumer warpgroup: rows [cw * 64, +64) of the tile
     uint32_t stage = 0, phase = 0;
     float acc[BN / 2];
@@ -243,10 +306,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       wgmma_fence_regs(acc);
       if (lane == 0) mbar_arrive(&empty[prev_stage]);
       const int r = m0 + cw * 64 + wq * 16 + (lane >> 2), c = n0 + 2 * (lane & 3);
+      if (p.epi == EPI_HI) {
+        epilogue_hi<BN>(p, b, r, c, acc);
+      } else if (p.epi == EPI_F32) {
+        epilogue_f32<BN>(p, b, r, c, acc);
+      } else {
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        epilogue_pair(p, b, r, c + 8 * j, acc[4 * j], acc[4 * j + 1]);
-        epilogue_pair(p, b, r + 8, c + 8 * j, acc[4 * j + 2], acc[4 * j + 3]);
+        for (int j = 0; j < BN / 8; ++j) {
+          epilogue_pair(p, b, r, c + 8 * j, acc[4 * j], acc[4 * j + 1]);
+          epilogue_pair(p, b, r + 8, c + 8 * j, acc[4 * j + 2], acc[4 * j + 3]);
+        }
       }
     }
   }
@@ -326,6 +395,21 @@ static int make_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t
 
 static RowMapD to_rm(const qb_rowmap& r) { return RowMapD{r.ptr, (long long)r.ld, (long long)r.rows_per_batch, (long long)r.row_off}; }
 
+static bool aligned(const void* ptr, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(ptr) & (bytes - 1)) == 0; }
+
+// The conditions are those under which epilogue_pair takes its vectorised branch for every in-range pair (plus an 8-byte
+// aligned bias, loaded as float2), so each kind computes what epilogue_pair would.
+static int classify_epilogue(const GemmParams& p) {
+  if (p.N % 2 != 0 || p.act2 != QB_ACT_NONE || !aligned(p.bias, 8)) return EPI_GENERIC;
+  if (p.ohi.ptr && !p.olo.ptr && !p.o32.ptr && !p.res.ptr && !p.gamma && (p.act == QB_ACT_NONE || p.act == QB_ACT_GELU) &&
+      (p.ohi.ld & 1) == 0 && aligned(p.ohi.ptr, 4))
+    return EPI_HI;
+  if (p.o32.ptr && !p.ohi.ptr && p.act == QB_ACT_NONE && (p.o32.ld & 1) == 0 && aligned(p.o32.ptr, 8) &&
+      (!p.res.ptr || ((p.res.ld & 1) == 0 && aligned(p.res.ptr, 8))) && aligned(p.gamma, 8))
+    return EPI_F32;
+  return EPI_GENERIC;
+}
+
 static int fill_params(const qb_gemm_desc* d, GemmParams* p, int BN) {
   QB_REQUIRE(d && d->a_hi && d->w_hi, "gemm: null operand");
   QB_REQUIRE((d->a_lo == nullptr) == (d->w_lo == nullptr), "gemm: a_lo and w_lo must both be given or both be NULL");
@@ -355,12 +439,12 @@ static int fill_params(const qb_gemm_desc* d, GemmParams* p, int BN) {
   p->a_hi = (const __half*)d->a_hi; p->a_lo = (const __half*)d->a_lo;
   p->w_hi = (const __half*)d->w_hi; p->w_lo = (const __half*)d->w_lo;
   p->a_rpb = d->a_rows_per_batch; p->a_batch = (int)d->a_batch;
+  p->epi = classify_epilogue(*p);
   return 0;
 }
 
-template <int NTERMS, int STAGES>
+template <int NTERMS, int BN, int STAGES>
 static int launch_tc(const qb_gemm_desc* d, cudaStream_t st, int num_sms) {
-  constexpr int BN = GEMM_BN;
   GemmParams p;
   if (int e = fill_params(d, &p, BN)) return e;
   CUtensorMap mA_hi, mA_lo, mW_hi, mW_lo;
@@ -383,7 +467,7 @@ static int launch_tc(const qb_gemm_desc* d, cudaStream_t st, int num_sms) {
   constexpr int NPL = NTERMS == 1 ? 1 : 2;
   constexpr size_t smem = (size_t)STAGES * NPL * (GEMM_BM * 64 * 2 + BN * 64 * 2) + 1024 + 256;
   static_assert(smem <= 227 * 1024, "GEMM pipeline exceeds the 227 KB of shared memory a block may use");
-  auto kern = gemm_tc_kernel<NTERMS, STAGES>;
+  auto kern = gemm_tc_kernel<NTERMS, BN, STAGES>;
   static bool attr_set[QB_MAX_DEVICES] = {};          // the opt-in shared-memory limit is per-device state
   const int dev = current_device();
   if (!attr_set[dev]) {
@@ -416,17 +500,22 @@ extern "C" int qb_version(void) { return 100; }
 extern "C" int64_t qb_launch_count(void) { return (int64_t)g_launches.load(); }
 extern "C" void qb_launch_count_reset(void) { g_launches = 0; }
 
-// One tile shape (128 x 128 x 64) for every problem: single pass with 6 pipeline stages (192 KB), hi + lo split with 3.
+// Three instantiations of one kernel, every stage 128 rows x 64 K, 192 KB of pipeline each:
+//   single pass, n > 128:  128 x 256 tiles, 4 stages (48 KB)
+//   single pass, n <= 128: 128 x 128 tiles, 6 stages (32 KB) - a 256-wide tile would be at least half padding
+//   hi + lo split:         128 x 128 tiles, 3 stages (64 KB)
 extern "C" const char* qb_gemm_kernel_name(int64_t m_per_batch, int64_t n, int32_t split) {
-  (void)m_per_batch; (void)n;
-  return split ? "gemm_tc_kernel<3,3>" : "gemm_tc_kernel<1,6>";
+  (void)m_per_batch;
+  if (split) return "gemm_tc_kernel<3,128,3>";
+  return n > 128 ? "gemm_tc_kernel<1,256,4>" : "gemm_tc_kernel<1,128,6>";
 }
 
 extern "C" int qb_gemm(const qb_gemm_desc* d, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   QB_REQUIRE(d != nullptr, "gemm: null desc");
   const int sms = num_sms_cached();
-  return d->a_lo != nullptr ? launch_tc<3, 3>(d, st, sms) : launch_tc<1, 6>(d, st, sms);
+  if (d->a_lo != nullptr) return launch_tc<3, 128, 3>(d, st, sms);
+  return d->n > 128 ? launch_tc<1, 256, 4>(d, st, sms) : launch_tc<1, 128, 6>(d, st, sms);
 }
 
 extern "C" int qb_gemm_simt(const qb_gemm_desc* d, void* stream) {
