@@ -86,12 +86,22 @@ def test_gemm_conv1d(lib, split, k, s, Cin, Cout, T, B):
 
 
 def test_gemm_epilogues(lib):
+    """the 3-term <3,128,3> kernel against the fp64 product of the fp32 operands"""
+    _gemm_epilogues(True)
+
+
+def test_gemm_epilogues_single_pass(lib):
+    """the same epilogues on the single-pass 256-wide tile (N = 512) against the fp64 product of the fp16 operands it reads"""
+    _gemm_epilogues(False)
+
+
+def _gemm_epilogues(split):
     import torch.nn.functional as F
     from unified_audio_b200 import ops
     M, N, K = 260, 512, 256
     x, w, bias, gamma, res = _mk((M, K), 11), _mk((N, K), 12, K ** -0.5), _mk((N,), 13), _mk((N,), 14), _mk((M, N), 15)
-    a, wp = ops.Planes.from_f32(x, True), ops.Planes.from_f32(w, True)
-    acc = (x.double() @ w.double().t())
+    a, wp = ops.Planes.from_f32(x, split), ops.Planes.from_f32(w, split)
+    acc = (x.double() @ w.double().t()) if split else planes_ref(a) @ planes_ref(wp).t()
     # GELU -> planes
     outp = ops.Planes.zeros((M, N), True, DEV)
     ops.gemm(a, wp, N, a_batch=1, a_rows_per_batch=M, a_ld=K, m_per_batch=M, bias=bias, act=ops.ACT_GELU,

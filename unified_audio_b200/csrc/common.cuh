@@ -56,11 +56,15 @@ __device__ __forceinline__ float sigmoid_acc(float x) { return 1.0f / (1.0f + ex
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + expf(-x)); }
 __device__ __forceinline__ float elu_f(float x) { return x > 0.f ? x : expm1f(x); }
 
-// fp32 -> (hi, lo) fp16 planes.  hi = rn(x) saturated to the fp16 range, lo = rn(x - hi).
+// fp32 -> fp16 rounded to nearest and saturated to +-65504 (infinities included), NaN kept as NaN: one cvt .satfinite.
+// (A clamp with fminf / fmaxf, or __hmin2 / __hmax2, returns the non-NaN operand and would turn a NaN into a finite value; the
+// half2 stores of the GEMM epilogue clamp with __hmin2_nan / __hmax2_nan.)
 __device__ __forceinline__ __half f2h_sat(float x) {
-  x = fminf(fmaxf(x, -65504.f), 65504.f);
-  return __float2half_rn(x);
+  unsigned short h;
+  asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(x));
+  return __ushort_as_half(h);
 }
+// fp32 -> (hi, lo) fp16 planes.  hi = rn(x) saturated to the fp16 range, lo = rn(x - hi).
 __device__ __forceinline__ void split_f16(float x, __half& hi, __half& lo) {
   hi = f2h_sat(x);
   lo = __float2half_rn(x - __half2float(hi));

@@ -139,7 +139,7 @@ __device__ __forceinline__ void epilogue_pair(const GemmParams& p, int b, int m,
       if (p.act == QB_ACT_GELU) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
       const __half2 hmax = __float2half2_rn(65504.f), hmin = __float2half2_rn(-65504.f);
       *reinterpret_cast<__half2*>((__half*)p.ohi.ptr + ((long long)b * p.ohi.rpb + p.ohi.off + m) * p.ohi.ld + n) =
-          __hmax2(__hmin2(__floats2half2_rn(v0, v1), hmax), hmin);
+          __hmax2_nan(__hmin2_nan(__floats2half2_rn(v0, v1), hmax), hmin);     // saturated, NaN kept (as f2h_sat)
       return;
     }
     if (p.o32.ptr && !p.ohi.ptr && p.act == QB_ACT_NONE && (p.o32.ld & 1) == 0 && (reinterpret_cast<uintptr_t>(p.o32.ptr) & 7) == 0 &&
@@ -192,7 +192,7 @@ __device__ __forceinline__ void epilogue_hi(const GemmParams& p, int b, int r, i
       float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
       if (p.bias) { v0 += bb.x; v1 += bb.y; }
       if (gelu) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
-      *reinterpret_cast<__half2*>(base + h * row8 + n) = __hmax2(__hmin2(__floats2half2_rn(v0, v1), hmax), hmin);
+      *reinterpret_cast<__half2*>(base + h * row8 + n) = __hmax2_nan(__hmin2_nan(__floats2half2_rn(v0, v1), hmax), hmin);
     }
   }
 }
