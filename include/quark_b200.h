@@ -40,7 +40,7 @@ int64_t qb_launch_count(void);
 void qb_launch_count_reset(void);
 
 /* activation codes for the GEMM epilogue */
-enum { QB_ACT_NONE = 0, QB_ACT_GELU = 1, QB_ACT_SWIGLU = 2, QB_ACT_ELU = 3, QB_ACT_TANH = 4, QB_ACT_SNAKE = 5 };
+enum { QB_ACT_NONE = 0, QB_ACT_GELU = 1, QB_ACT_SWIGLU = 2, QB_ACT_ELU = 3, QB_ACT_TANH = 4, QB_ACT_SNAKE = 5, QB_ACT_RELU = 6 };
 
 /* Row mapping of an output / residual tensor: GEMM row (batch b, row m) lives at
  * ptr + ((b * rows_per_batch + row_off + m) * ld + n).  Lets a GEMM write straight into the
@@ -62,6 +62,8 @@ typedef struct {
  *            out_f32 <- v;   out planes <- split_fp16(act2(v))
  * QB_ACT_SWIGLU pairs columns (2j, 2j+1) -> silu(v[2j]) * v[2j+1] at output column j
  * (encoder_modules/transformer.py:218-226 with w1/w3 rows interleaved).
+ * QB_ACT_RELU with gamma and a broadcast residual row (residual.ld = rows_per_batch = 0, row_off = 0: address ptr + n) is an
+ * eval-mode conv -> ReLU -> BatchNorm1d (ecapa_tdnn.py:90-109): gamma = w / sqrt(var + eps), residual = b - mean * gamma.
  */
 typedef struct {
   const qb_half* a_hi;      /* [a_batch, a_rows_per_batch, a_ld] */
@@ -334,6 +336,42 @@ int qb_ssl_compress(const float* x, int64_t B, int64_t T, int32_t C, float power
 /* out[b, i] = x[b, i - left] (zero outside, or wrapped modulo T_in when wrap != 0): pad_wav (audio_tokenizer.py:63-66),
  * F.pad(wavs, (160, 160)) (:51), wrap padding of UniSE segments (QuarkAudio-UniSE/model/model.py:175-181). */
 int qb_pad_wav(const float* x, int64_t B, int64_t T_in, int64_t left, int64_t T_out, int32_t wrap, float* out, void* stream);
+
+/* ---------------------------------------------------------------- BiCodec global (speaker) tokens (SURVEY 8f.1, csrc/speaker.cu)
+ * BiCodec.get_global_tokens (QuarkAudio-UniSE/model/bicodec/bicodec.py:174-178): MelSpectrogram -> ECAPA-TDNN latent ->
+ * PerceiverResampler -> ResidualFSQ indices.  Convolutions and linears run on qb_gemm (Conv1dReluBn as QB_ACT_RELU + gamma + a
+ * broadcast residual row); the DFT is the two-stage one of the STFT above (qb_stft_twiddle).
+ * qb_mel_gather: torch.stft(center=True, pad_mode="reflect") framing of wav [B, L], 1 + L / hop frames, in qb_stft_gather's layout
+ *   (torchaudio MelSpectrogram, bicodec.py:201-221; window [n_fft] = the win_length window zero-padded to the middle of n_fft).
+ * qb_spec_magnitude: |X[k]|, k < nf, of the second DFT stage (layout of qb_stft_post2) -> planes [M, ld], zero past nf. */
+int qb_mel_gather(const float* wav, int64_t B, int64_t L, int32_t hop, int32_t n_fft, int32_t P, int32_t Q, const float* window,
+                  qb_half* hi, qb_half* lo, void* stream);
+int qb_spec_magnitude(const float* X, int64_t ldX, int64_t M, int32_t nf, int32_t P, qb_half* hi, qb_half* lo, int64_t ld, void* stream);
+/* x [B*T rows, pitch ldx] (+ y [B*T rows, pitch ldy], or NULL) over C channels -> planes of a padded buffer [B, rows_per_batch, ld]
+ * at row_off, channels C..ld-1 zeroed: Res2Conv1dReluBn's sp + spx[i] (modules/speaker/ecapa_tdnn.py:68-83). */
+int qb_add_planes(const float* x, int64_t ldx, const float* y, int64_t ldy, int64_t B, int64_t T, int64_t C, qb_half* hi, qb_half* lo,
+                  int64_t ld, int64_t rows_per_batch, int64_t row_off, void* stream);
+/* SE_Connect (ecapa_tdnn.py:116-129): s [B, C] = sigmoid(W2 relu(W1 mean_t z + b1) + b2), z [B, T, C]; W1 [R, C], W2 [C, R]; the
+ * time mean is a fixed-order fp64 sum.  qb_se_apply: x + z * s (ecapa_tdnn.py:150) -> fp32 out [B*T, C] and / or planes at column
+ * col_off of rows of ld channels (the block's slice of the 3 x C concat, ecapa_tdnn.py:203). */
+int qb_se_gate(const float* z, int64_t B, int64_t T, int32_t C, const float* w1, const float* b1, int32_t R, const float* w2,
+               const float* b2, float* s, void* stream);
+int qb_se_apply(const float* z, const float* s, const float* x, int64_t B, int64_t T, int32_t C, float* out, qb_half* hi, qb_half* lo,
+                int64_t ld, int64_t col_off, void* stream);
+/* GEGLU (perceiver_encoder.py:232-235): h [rows, 2*inner] fp32 (value | gate, the reference's chunk order) -> planes [rows, ld] =
+ * gelu_erf(gate) * value, zero past inner.  A kernel rather than a GEMM epilogue: an epilogue variant grew the GEMM kernels' code by a
+ * fifth and measurably slowed the H-Codec path that never uses it. */
+int qb_geglu_planes(const float* h, int64_t rows, int32_t inner, qb_half* hi, qb_half* lo, int64_t ld, void* stream);
+/* fp32 cross attention, head_dim 64, scale 1/8 (perceiver_encoder.py:135-178,280-294): q [B, Nq, heads*64], kv [B, Nk, 2*heads*64]
+ * (keys | values) -> planes [B*Nq, heads*64].  Nk <= 3072. */
+int qb_cross_attention(const float* q, const float* kv, int64_t B, int64_t Nq, int64_t Nk, int32_t heads, qb_half* out_hi,
+                       qb_half* out_lo, void* stream);
+/* RMSNorm F.normalize(x) * sqrt(dim) * gamma (perceiver_encoder.py:195-214) -> project_in (W [n_levels, dim], b) -> FSQ bound,
+ * round half to even, codes_to_indices (finite_scalar_quantization.py:126-157; residual_fsq.py:158-252 with one quantizer):
+ * x [rows, dim] fp32 -> idx [rows] int32; z [rows, n_levels] (project_in output) and xn [rows, dim] (normed rows) if not NULL.
+ * `levels` is a HOST array of n_levels <= 8 entries; num_quantizers other than 1 is refused. */
+int qb_fsq_tokenize(const float* x, int64_t rows, int32_t dim, const float* gamma, const float* w_in, const float* b_in, int32_t n_levels,
+                    const int32_t* levels, int32_t num_quantizers, int32_t* idx, float* z, float* xn, void* stream);
 
 /* ---------------------------------------------------------------- H-Codec-1.5 adaptive frame-rate primitives (SURVEY 8f.4)
  * FlexiCodec._perform_similarity_alignment_vectorized (HCodec-1.5/adaptive/modeling_flexicodec_new.py:828-921): h [B, T, D] fp32 ->

@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("QB_LIB") or os.path.join(_HERE, "lib", "libquark_b200.so")     # QB_LIB: A/B builds for experiments
 
-ACT_NONE, ACT_GELU, ACT_SWIGLU, ACT_ELU, ACT_TANH, ACT_SNAKE = 0, 1, 2, 3, 4, 5
+ACT_NONE, ACT_GELU, ACT_SWIGLU, ACT_ELU, ACT_TANH, ACT_SNAKE, ACT_RELU = 0, 1, 2, 3, 4, 5, 6
 
 
 class RowMap(C.Structure):
@@ -109,6 +109,14 @@ SIGNATURES = {
     "qb_axpy": (C.c_int, [_vp, _f32, _i64, _i32, _vp, _vp]),
     "qb_ssl_compress": (C.c_int, [_vp, _i64, _i64, _i32, _f32, _i32, _vp, _vp]),
     "qb_pad_wav": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _i32, _vp, _vp]),
+    "qb_mel_gather": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "qb_spec_magnitude": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _vp, _vp, _i64, _vp]),
+    "qb_add_planes": (C.c_int, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "qb_se_gate": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp]),
+    "qb_se_apply": (C.c_int, [_vp, _vp, _vp, _i64, _i64, _i32, _vp, _vp, _vp, _i64, _i64, _vp]),
+    "qb_geglu_planes": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i64, _vp]),
+    "qb_cross_attention": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp, _vp]),
+    "qb_fsq_tokenize": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _vp, _i32, C.POINTER(C.c_int32), _i32, _vp, _vp, _vp, _vp]),
     "qb_similarity_alignment": (C.c_int, [_vp, _i64, _i64, _i32, _f32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "qb_alignment_matrix": (C.c_int, [_vp, _i64, _i64, _i64, _vp, _vp]),
     "qb_pack_lengths": (C.c_int, [_vp, _vp, _i64, _i32, _i64, _i32, _vp, _vp]),

@@ -5,7 +5,17 @@ Mirrors QuarkAudio-UniSE/model/bicodec/bicodec.py:182-199:
 state_dict keys are the reference's (`quantizer.*`, `speaker_encoder.*`, `prenet.*`, `decoder.*`, old-style weight-norm
 `weight_g / weight_v` pairs); keys of the tokenize side (`encoder.*`, `postnet.*`, ECAPA / perceiver, `mel_transformer.*`,
 `quantizer.in_project.*`) are accepted at load and ignored.  The reference ships no `config.yaml` (it comes with the
-Spark-TTS-0.5B checkpoint, U/README.md:57-74); BICODEC_CONFIG restates that published configuration.
+Spark-TTS-0.5B checkpoint, U/README.md:57-74); BICODEC_CONFIG and MEL_PARAMS restate that published configuration.
+
+With `global_tokens=True` the module also holds the global-token path, bicodec.py:174-178:
+    BiCodec.get_global_tokens({"ref_wav": [B, L]}) -> int32 [B, 1, token_num]
+and a strict load requires its keys (`speaker_encoder.speaker_encoder.{layer1..layer4,conv}.*` with BatchNorm running statistics,
+`speaker_encoder.perceiver_sampler.*`, `speaker_encoder.quantizer.project_in.*`).  Still ignored: the semantic tokenize side, the
+x-vector branch the reference computes and discards (`speaker_encoder.speaker_encoder.{pool,bn,linear}.*`), BatchNorm's
+`num_batches_tracked` and `mel_transformer.*` (window and filter bank are rebuilt from MEL_PARAMS).  Mapping: MelSpectrogram =
+centred reflect framing + two-stage DFT GEMMs + |X| + the slaney filter bank as a GEMM; Conv1dReluBn = one GEMM with a ReLU
+epilogue and the eval BatchNorm folded into gamma + a broadcast residual row; squeeze-excitation, the perceiver's cross attention
+RMSNorm + FSQ and the feed-forward's GEGLU are kernels of csrc/speaker.cu.  Every contraction is a 3-term split.
 
 How the path maps onto the library (every arithmetic op is a libquark_b200 kernel; channel-last activations):
   * FactorizedVectorQuantize.detokenize (modules/vq/factorized_vector_quantize.py:154-167) and the residual-FSQ de-quantiser
@@ -20,6 +30,7 @@ How the path maps onto the library (every arithmetic op is a libquark_b200 kerne
 """
 from __future__ import annotations
 
+import math
 from typing import Dict
 
 import torch
@@ -27,7 +38,7 @@ from torch import nn
 
 from . import ops
 from .codec import _Tree, _pad_to
-from .ops import ACT_GELU, ACT_SNAKE, ACT_TANH, Planes, rowmap
+from .ops import ACT_GELU, ACT_RELU, ACT_SNAKE, ACT_TANH, Planes, rowmap
 
 BICODEC_CONFIG = dict(
     sample_rate=16000, hop=320,
@@ -37,6 +48,11 @@ BICODEC_CONFIG = dict(
                 condition_dim=1024, sample_ratios=[1, 1], use_tanh_at_final=False),
     decoder=dict(input_channel=1024, channels=1536, rates=[8, 5, 4, 2], kernel_sizes=[16, 11, 8, 4]),
 )
+
+# BiCodec's `mel_params` (bicodec.py:201-221): the published Spark-TTS-0.5B values, restated like BICODEC_CONFIG and likewise not
+# verifiable offline.  A config without a "mel_params" entry uses these.
+MEL_PARAMS = dict(sample_rate=16000, n_fft=1024, win_length=640, hop_length=320, mel_fmin=10, mel_fmax=None, num_mels=128)
+ECAPA_C, ECAPA_SCALE, ECAPA_OUT, HEADS = 512, 8, 1536, 8   # ECAPA_TDNN_GLOB_c512, dim_context = 512 * 3, 8 heads x 64 (fixed)
 
 # 3-term split (True) or single-pass fp16 (False) per GEMM group; "accurate" is the default until the error budget of the
 # 26-conv generator is mapped (DESIGN.md)
@@ -111,30 +127,110 @@ def bicodec_spec(c) -> Dict[str, tuple]:
     return out
 
 
+def speaker_spec(c) -> Dict[str, tuple]:
+    """Reference state-dict keys -> shapes of the global-token path (SpeakerEncoder.tokenize, speaker_encoder.py:104-109)
+    without the x-vector branch it discards (pool / bn / linear) and without BatchNorm's num_batches_tracked."""
+    out: Dict[str, tuple] = {}
+    s, nm, w = c["speaker"], c.get("mel_params", MEL_PARAMS)["num_mels"], ECAPA_C // ECAPA_SCALE
+    E = "speaker_encoder.speaker_encoder."
+
+    def bn(p, ch):
+        for k in ("weight", "bias", "running_mean", "running_var"):
+            out[p + k] = (ch,)
+
+    def crb(p, cin, cout, k):
+        out[p + "conv.weight"], out[p + "conv.bias"] = (cout, cin, k), (cout,)
+        bn(p + "bn.", cout)
+
+    crb(E + "layer1.", nm, ECAPA_C, 5)
+    for k in (2, 3, 4):
+        p = f"{E}layer{k}.se_res2block."
+        crb(p + "0.", ECAPA_C, ECAPA_C, 1)
+        for i in range(ECAPA_SCALE - 1):
+            out[f"{p}1.convs.{i}.weight"], out[f"{p}1.convs.{i}.bias"] = (w, w, 3), (w,)
+            bn(f"{p}1.bns.{i}.", w)
+        crb(p + "2.", ECAPA_C, ECAPA_C, 1)
+        out[p + "3.linear1.weight"], out[p + "3.linear1.bias"] = (128, ECAPA_C), (128,)
+        out[p + "3.linear2.weight"], out[p + "3.linear2.bias"] = (ECAPA_C, 128), (ECAPA_C,)
+    out[E + "conv.weight"], out[E + "conv.bias"] = (ECAPA_OUT, 3 * ECAPA_C, 1), (ECAPA_OUT,)
+    P, dim, inner = "speaker_encoder.perceiver_sampler.", s["latent_dim"], int(s["latent_dim"] * 4 * 2 / 3)
+    if dim != ECAPA_OUT:
+        out[P + "proj_context.weight"], out[P + "proj_context.bias"] = (dim, ECAPA_OUT), (dim,)
+    out[P + "latents"] = (s["token_num"], dim)
+    for layer in range(2):
+        q = f"{P}layers.{layer}."
+        out[q + "0.to_q.weight"], out[q + "0.to_kv.weight"] = (HEADS * 64, dim), (2 * HEADS * 64, dim)
+        out[q + "0.to_out.weight"] = (dim, HEADS * 64)
+        out[q + "1.0.weight"], out[q + "1.0.bias"] = (2 * inner, dim), (2 * inner,)
+        out[q + "1.2.weight"], out[q + "1.2.bias"] = (dim, inner), (dim,)
+    out[P + "norm.gamma"] = (dim,)
+    out["speaker_encoder.quantizer.project_in.weight"] = (len(s["fsq_levels"]), dim)
+    out["speaker_encoder.quantizer.project_in.bias"] = (len(s["fsq_levels"]),)
+    return out
+
+
 _IGNORED = ("encoder.", "postnet.", "mel_transformer.", "speaker_encoder.speaker_encoder.", "speaker_encoder.perceiver_sampler.",
             "speaker_encoder.quantizer.project_in.", "quantizer.in_project.", "quantizer.cluster_size")
+# with global_tokens=True: the semantic tokenize side, the mel transformer's buffers (rebuilt from mel_params) and the x-vector
+# branch the reference computes and discards (speaker_encoder.py:104-109)
+_IGNORED_GLOBAL = ("encoder.", "postnet.", "mel_transformer.", "quantizer.in_project.", "quantizer.cluster_size",
+                   "speaker_encoder.speaker_encoder.pool.", "speaker_encoder.speaker_encoder.bn.", "speaker_encoder.speaker_encoder.linear.")
+
+
+def hann_window(mp) -> torch.Tensor:
+    """torch.hann_window(win_length) (periodic) zero-padded to the middle of n_fft, as torch.stft applies it; fp64"""
+    n, win = mp["n_fft"], mp["win_length"]
+    k = torch.arange(win, dtype=torch.float64)
+    out = torch.zeros(n, dtype=torch.float64)
+    out[(n - win) // 2:(n - win) // 2 + win] = 0.5 - 0.5 * torch.cos(2 * math.pi * k / win)
+    return out
+
+
+def mel_filterbank(mp) -> torch.Tensor:
+    """Slaney-scale, slaney-normalised triangular filters (torchaudio melscale_fbanks) [n_fft // 2 + 1, num_mels]; fp64"""
+    def hz_to_mel(f):
+        return 15.0 + math.log(f / 1000.0) / (math.log(6.4) / 27.0) if f >= 1000.0 else 3.0 * f / 200.0
+
+    sr, n_fft, n_mels = mp["sample_rate"], mp["n_fft"], mp["num_mels"]
+    f_max = float(mp["mel_fmax"]) if mp["mel_fmax"] is not None else sr / 2
+    freqs = torch.linspace(0, sr // 2, n_fft // 2 + 1, dtype=torch.float64)
+    m = torch.linspace(hz_to_mel(float(mp["mel_fmin"])), hz_to_mel(f_max), n_mels + 2, dtype=torch.float64)
+    f = torch.where(m >= 15.0, 1000.0 * torch.exp(math.log(6.4) / 27.0 * (m - 15.0)), 200.0 * m / 3.0)
+    slopes = f[None, :] - freqs[:, None]
+    fb = torch.clamp(torch.minimum(-slopes[:, :-2] / (f[1:-1] - f[:-2]), slopes[:, 2:] / (f[2:] - f[1:-1])), min=0.0)
+    return fb * (2.0 / (f[2:] - f[:-2]))[None, :]
 
 
 class BiCodec(nn.Module):
-    def __init__(self, config: dict = None, precision: str = "accurate"):
+    """`global_tokens=True` adds the global-token path (`mel_spectrogram`, `get_global_tokens`): its reference keys become part of
+    the module and are required by a strict load.  The default object is the detokenize path alone."""
+
+    def __init__(self, config: dict = None, precision: str = "accurate", global_tokens: bool = False):
         super().__init__()
         self.cfg = dict(config or BICODEC_CONFIG)
         self.policy = PRECISION[precision]
-        tree = _Tree.build(bicodec_spec(self.cfg))
+        self.global_tokens = bool(global_tokens)
+        spec = bicodec_spec(self.cfg)
+        if self.global_tokens:
+            spec.update(speaker_spec(self.cfg))
+        tree = _Tree.build(spec)
         for name, child in tree.named_children():
             self.add_module(name, child)
-        self._w, self._ws = None, {}
+        self._w, self._wg, self._ws = None, None, {}
         self.eval()
 
     # ------------------------------------------------------------------ state
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
-        sd = {k: v for k, v in state_dict.items() if not k.startswith(_IGNORED)}
+        if self.global_tokens:
+            sd = {k: v for k, v in state_dict.items() if not k.startswith(_IGNORED_GLOBAL) and not k.endswith(".num_batches_tracked")}
+        else:
+            sd = {k: v for k, v in state_dict.items() if not k.startswith(_IGNORED)}
         r = super().load_state_dict(sd, strict=strict, assign=assign)
-        self._w = None
+        self._w, self._wg = None, None
         return r
 
     def _apply(self, fn, *a, **k):
-        self._w, self._ws = None, {}
+        self._w, self._wg, self._ws = None, None, {}
         return super()._apply(fn, *a, **k)
 
     def _dev(self):
@@ -425,6 +521,218 @@ class BiCodec(nn.Module):
         wav = torch.empty(B, 1, Tc, device=dev)
         self._conv(af, G["conv_f"], 1, B, Tc + 6, cpf, Tc, 7, bias=G["conv_f_b"], act=ACT_TANH, out_f32=rowmap(wav, 1, Tc, 0))
         return wav
+
+    # ------------------------------------------------------------------ global (speaker) tokens
+    def _mel_params(self):
+        return self.cfg.get("mel_params", MEL_PARAMS)
+
+    def _prepare_global(self):
+        if self._wg is not None:
+            return self._wg
+        if not self.global_tokens:
+            raise RuntimeError("this BiCodec was built without the global-token path: construct it with BiCodec(..., global_tokens=True)")
+        dev = self._dev()
+        if dev.type != "cuda":
+            raise RuntimeError("unified_audio_b200.BiCodec runs on CUDA only (no CPU fallback): call .cuda() first")
+        keys = speaker_spec(self.cfg)
+        sd = {k: v.detach().double().cpu() for k, v in self.state_dict().items() if k in keys}
+        mp, s = self._mel_params(), self.cfg["speaker"]
+        n_fft, nf = mp["n_fft"], mp["n_fft"] // 2 + 1
+        if n_fft % 64 or n_fft > 4096 or mp["win_length"] > n_fft:
+            raise ValueError("mel_params: the two-stage DFT needs n_fft a multiple of 64, at most 4096, and win_length <= n_fft")
+        if s["fsq_num_quantizers"] != 1:
+            raise NotImplementedError("residual FSQ with more than one quantizer (the shipped speaker encoder uses one)")
+
+        def pl(w):
+            return Planes.from_f32(w.float().to(dev), True)
+
+        def conv_pack(w):          # [Cout, Cin, k] -> [Cout, k * Cin_pad], tap-major K
+            co, ci, k = w.shape
+            out = torch.zeros(co, k, _pad_to(ci, 64), dtype=torch.float64)
+            out[:, :, :ci] = w.permute(0, 2, 1)
+            return pl(out.reshape(co, -1))
+
+        def pad_k(w, kp):          # [N, K] -> [N, kp]
+            out = torch.zeros(w.shape[0], kp, dtype=torch.float64)
+            out[:, :w.shape[1]] = w
+            return pl(out)
+
+        def f32(t):
+            return t.float().contiguous().to(dev)
+
+        def crb(p, w, b):          # Conv1dReluBn: conv -> ReLU -> eval BatchNorm as the GEMM's gamma and broadcast residual row
+            g = sd[p + "bn.weight"] / torch.sqrt(sd[p + "bn.running_var"] + 1e-5)
+            return dict(w=w, b=f32(b), g=f32(g), t=f32(sd[p + "bn.bias"] - sd[p + "bn.running_mean"] * g))
+
+        G: dict = {}
+        # ---- mel: two-stage DFT n_fft = P * Q (P = 64) on the GEMM, as the H-Codec STFT (csrc/elementwise.cu)
+        P, Q = 64, n_fft // 64
+        K2 = (nf - 1) // P + 1
+        ang = lambda num, den: 2 * math.pi * (num % den).double() / den
+        a, k1 = torch.arange(P)[None, :], torch.arange(P)[:, None]
+        wA = torch.zeros(2 * P, 64, dtype=torch.float64)
+        wA[0::2, :P], wA[1::2, :P] = torch.cos(ang(k1 * a, P)), -torch.sin(ang(k1 * a, P))
+        b_, k2 = torch.arange(Q)[None, :], torch.arange(K2)[:, None]
+        wB = torch.zeros(2 * K2, 128, dtype=torch.float64)
+        wB[0::2, :Q], wB[0::2, Q:2 * Q] = torch.cos(ang(k2 * b_, Q)), torch.sin(ang(k2 * b_, Q))
+        wB[1::2, :Q], wB[1::2, Q:2 * Q] = -torch.sin(ang(k2 * b_, Q)), torch.cos(ang(k2 * b_, Q))
+        bb, kk = torch.arange(Q)[:, None], torch.arange(P)[None, :]
+        tw = torch.stack([torch.cos(ang(bb * kk, n_fft)), -torch.sin(ang(bb * kk, n_fft))], -1)       # [b, k1, (cos, -sin)]
+        fp = _pad_to(nf, 64)
+        G.update(P=P, Q=Q, K2=K2, ldX=_pad_to(2 * K2, 4), fp=fp, wA=pl(wA), wB=pl(wB), tw=f32(tw), window=f32(hann_window(mp)),
+                 fb=pad_k(mel_filterbank(mp).t(), fp))
+        # ---- ECAPA-TDNN up to its latent
+        E = "speaker_encoder.speaker_encoder."
+        G["l1"] = crb(E + "layer1.", conv_pack(sd[E + "layer1.conv.weight"]), sd[E + "layer1.conv.bias"])
+        G["blocks"] = []
+        for k in (2, 3, 4):
+            p = f"{E}layer{k}.se_res2block."
+            res2 = []
+            for i in range(ECAPA_SCALE - 1):
+                g = sd[f"{p}1.bns.{i}.weight"] / torch.sqrt(sd[f"{p}1.bns.{i}.running_var"] + 1e-5)
+                res2.append(dict(w=conv_pack(sd[f"{p}1.convs.{i}.weight"]), b=f32(sd[f"{p}1.convs.{i}.bias"]), g=f32(g),
+                                 t=f32(sd[f"{p}1.bns.{i}.bias"] - sd[f"{p}1.bns.{i}.running_mean"] * g)))
+            G["blocks"].append(dict(
+                dil=k, res2=res2,
+                c0=crb(p + "0.", pl(sd[p + "0.conv.weight"][:, :, 0]), sd[p + "0.conv.bias"]),
+                c2=crb(p + "2.", pl(sd[p + "2.conv.weight"][:, :, 0]), sd[p + "2.conv.bias"]),
+                se=[f32(sd[p + n]) for n in ("3.linear1.weight", "3.linear1.bias", "3.linear2.weight", "3.linear2.bias")]))
+        G["conv"], G["conv_b"] = pl(sd[E + "conv.weight"][:, :, 0]), f32(sd[E + "conv.bias"])
+        # ---- perceiver: K padded to a multiple of 64
+        Pp, dim = "speaker_encoder.perceiver_sampler.", s["latent_dim"]
+        dp, inner = _pad_to(dim, 64), int(dim * 4 * 2 / 3)
+        if dim == ECAPA_OUT:
+            raise NotImplementedError("latent_dim == 1536 (PerceiverResampler without proj_context)")
+        G.update(dim=dim, dp=dp, inner=inner, ip=_pad_to(inner, 64), proj=pl(sd[Pp + "proj_context.weight"]),
+                 proj_b=f32(sd[Pp + "proj_context.bias"]), latents=f32(sd[Pp + "latents"]), layers=[])
+        for layer in range(2):
+            q = f"{Pp}layers.{layer}."
+            G["layers"].append(dict(wq=pad_k(sd[q + "0.to_q.weight"], dp), wkv=pad_k(sd[q + "0.to_kv.weight"], dp),
+                                    wo=pl(sd[q + "0.to_out.weight"]), w1=pad_k(sd[q + "1.0.weight"], dp), b1=f32(sd[q + "1.0.bias"]),
+                                    w2=pad_k(sd[q + "1.2.weight"], _pad_to(inner, 64)), b2=f32(sd[q + "1.2.bias"])))
+        G.update(gamma=f32(sd[Pp + "norm.gamma"]), w_in=f32(sd["speaker_encoder.quantizer.project_in.weight"]),
+                 b_in=f32(sd["speaker_encoder.quantizer.project_in.bias"]))
+        self._wg = G
+        return G
+
+    def _check_wav(self, wav):
+        if not isinstance(wav, torch.Tensor) or wav.ndim not in (2, 3) or (wav.ndim == 3 and wav.shape[1] != 1):
+            raise ValueError("ref_wav must be [B, L] or [B, 1, L]")
+        if wav.device.type != "cuda":
+            raise RuntimeError("unified_audio_b200.BiCodec runs on CUDA only (no CPU fallback): ref_wav is on the CPU")
+        wav = wav.reshape(wav.shape[0], wav.shape[-1]).float().contiguous()
+        if wav.shape[-1] <= self._mel_params()["n_fft"] // 2:
+            raise ValueError(f"ref_wav needs more than n_fft / 2 = {self._mel_params()['n_fft'] // 2} samples (reflect padding)")
+        return wav
+
+    def _mel(self, G, wav):
+        """MelSpectrogram (bicodec.py:201-221) -> fp32 mel [B*T, num_mels] (channel-last) and the planes of layer1's input buffer"""
+        mp = self._mel_params()
+        B, L = wav.shape
+        T, M, nm = 1 + L // mp["hop_length"], B * (1 + L // mp["hop_length"]), mp["num_mels"]
+        P, Q, K2, ldX, fp = G["P"], G["Q"], G["K2"], G["ldX"], G["fp"]
+        ga = self._planes("mel_frames", (M * Q, 64), True)
+        ops.mel_gather(wav, mp["hop_length"], mp["n_fft"], P, Q, G["window"], ga)
+        Y = self._buf("mel_y", (M * Q, 2 * P))
+        ops.gemm(ga, G["wA"], 2 * P, a_batch=1, a_rows_per_batch=M * Q, a_ld=64, m_per_batch=M * Q, out_f32=rowmap(Y, 2 * P, M * Q, 0))
+        Z = self._planes("mel_z", (M * P, 128), True)
+        ops.stft_twiddle(Y, 2 * P, M, P, Q, G["tw"], Z)
+        X = self._buf("mel_x", (M * P, ldX))
+        ops.gemm(Z, G["wB"], 2 * K2, a_batch=1, a_rows_per_batch=M * P, a_ld=128, m_per_batch=M * P, out_f32=rowmap(X, ldX, M * P, 0))
+        mag = self._planes("mel_mag", (M, fp), True)
+        ops.spec_magnitude(X, ldX, M, mp["n_fft"] // 2 + 1, P, mag, fp)
+        cp = _pad_to(nm, 64)
+        x0 = self._planes("ecapa_in", (B, T + 4, cp), True)
+        mel = self._buf("mel", (M, nm))
+        ops.gemm(mag, G["fb"], nm, a_batch=B, a_rows_per_batch=T, a_ld=fp, m_per_batch=T, out_f32=rowmap(mel, nm, T, 0),
+                 out_planes=x0, out_planes_map=(cp, T + 4, 2))
+        return mel, x0, T
+
+    @torch.no_grad()
+    def mel_spectrogram(self, wav: torch.Tensor) -> torch.Tensor:
+        """The reference's mel_transformer(wav).squeeze(1): wav [B, L] or [B, 1, L] -> fp32 [B, num_mels, 1 + L // hop]"""
+        G = self._prepare_global()
+        wav = self._check_wav(wav)
+        mel, _, T = self._mel(G, wav)
+        return mel.reshape(wav.shape[0], T, -1).transpose(1, 2).contiguous()
+
+    def _crb(self, a, cw, n, **kw):
+        ops.gemm(a, cw["w"], n, bias=cw["b"], act=ACT_RELU, gamma=cw["g"], residual=rowmap(cw["t"], 0, 0, 0), **kw)
+
+    @torch.no_grad()
+    def get_global_tokens(self, batch, taps=None) -> torch.Tensor:
+        """bicodec.py:174-178: batch["ref_wav"] [B, L] (or [B, 1, L]) -> int32 [B, 1, token_num], the layout detokenize takes.
+        taps (a dict) receives channel-last fp32 copies: "mel" [B, T, num_mels], "latent" [B, T, 1536], "perceiver" [B, N, dim]
+        and "z" [B, N, len(fsq_levels)], the project_in output that the FSQ bound rounds."""
+        G = self._prepare_global()
+        wav = self._check_wav(batch["ref_wav"] if isinstance(batch, dict) else batch)
+        B = wav.shape[0]
+        mel, x0, T = self._mel(G, wav)
+        M, C, w = B * T, ECAPA_C, ECAPA_C // ECAPA_SCALE
+        # ---- ECAPA-TDNN (ecapa_tdnn.py:195-205): channel-last fp32 trunks, fp16 hi / lo planes for every contraction
+        cat = self._planes("ecapa_cat", (M, 3 * C), True)
+        trunk = [self._buf("ecapa_x0", (M, C)), self._buf("ecapa_x1", (M, C))]
+        inp = self._planes("ecapa_o1", (M, C), True)
+        self._crb(x0, G["l1"], C, a_batch=B, a_rows_per_batch=T + 4, a_ld=x0.hi.shape[-1], m_per_batch=T, taps=5,
+                  out_f32=rowmap(trunk[0], C, T, 0), out_planes=inp, out_planes_map=(C, T, 0))
+        in_ld, in_off = C, 0
+        y, z = self._buf("ecapa_y", (M, C)), self._buf("ecapa_z", (M, C))
+        yp, gate = self._planes("ecapa_yp", (M, C), True), self._buf("ecapa_se", (B, C))
+        for bi, blk in enumerate(G["blocks"]):
+            x_in, x_out, d = trunk[bi & 1], trunk[(bi + 1) & 1], blk["dil"]
+            self._crb(inp, blk["c0"], C, a_batch=1, a_rows_per_batch=M, a_ld=in_ld, a_cols=C, a_col_off=in_off, m_per_batch=M,
+                      out_f32=rowmap(y, C, M, 0))
+            # Res2Conv1dReluBn (ecapa_tdnn.py:68-83): chunk i's conv reads spx[i] + out[i - 1]; out[i] overwrites spx[i] in y
+            sp = self._planes(f"ecapa_sp{d}", (B, T + 2 * d, w), True)
+            for i, rw in enumerate(blk["res2"]):
+                ops.add_planes(y.view(-1)[w * i:], C, y.view(-1)[w * (i - 1):] if i else None, C, B, T, w, sp, w, T + 2 * d, d)
+                self._crb(sp, rw, w, a_batch=B, a_rows_per_batch=T + 2 * d, a_ld=w, m_per_batch=T, taps=3, dilation=d,
+                          out_f32=rowmap(y.view(-1)[w * i:], C, T, 0))
+            ops.split_f16(y, yp)
+            self._crb(yp, blk["c2"], C, a_batch=1, a_rows_per_batch=M, a_ld=C, m_per_batch=M, out_f32=rowmap(z, C, M, 0))
+            ops.se_gate(z, B, T, C, *blk["se"], gate)
+            ops.se_apply(z, gate, x_in, B, T, C, out=x_out, planes=cat, ld=3 * C, col_off=bi * C)
+            inp, in_ld, in_off = cat, 3 * C, bi * C
+        latp = self._planes("ecapa_latent_p", (M, ECAPA_OUT), True)
+        lat32 = self._buf("ecapa_latent", (M, ECAPA_OUT)) if taps is not None else None
+        ops.gemm(cat, G["conv"], ECAPA_OUT, a_batch=1, a_rows_per_batch=M, a_ld=3 * C, m_per_batch=M, bias=G["conv_b"], act=ACT_RELU,
+                 out_f32=rowmap(lat32, ECAPA_OUT, M, 0) if taps is not None else None, out_planes=latp, out_planes_map=(ECAPA_OUT, M, 0))
+        # ---- PerceiverResampler (perceiver_encoder.py:339-350); context rows 0..N-1 = the current latents, N.. = proj_context(x)
+        s = self.cfg["speaker"]
+        N, D, dp, ip = s["token_num"], G["dim"], G["dp"], G["ip"]
+        Nk, R = N + T, B * N
+        ctx = self._planes("pc_ctx", (B, Nk, dp), True)
+        ops.gemm(latp, G["proj"], D, a_batch=B, a_rows_per_batch=T, a_ld=ECAPA_OUT, m_per_batch=T, bias=G["proj_b"], out_planes=ctx,
+                 out_planes_map=(dp, Nk, N))
+        lat = self._buf("pc_lat", (R, D))
+        lat.view(B, N, D).copy_(G["latents"].expand(B, N, D))
+        lp, att = self._planes("pc_lat_p", (R, dp), True), self._planes("pc_att", (R, HEADS * 64), True)
+        q, kv = self._buf("pc_q", (R, HEADS * 64)), self._buf("pc_kv", (B * Nk, 2 * HEADS * 64))
+        hid, ffh = self._planes("pc_hid", (R, ip), True), self._buf("pc_ffh", (R, 2 * G["inner"]))
+        lm = rowmap(lat, D, R, 0)
+        for L in G["layers"]:
+            ops.rows_to_planes(lat, B, N, D, ctx, dp, Nk, 0)
+            ops.rows_to_planes(lat, 1, R, D, lp, dp, R, 0)
+            ops.gemm(lp, L["wq"], HEADS * 64, a_batch=1, a_rows_per_batch=R, a_ld=dp, m_per_batch=R, out_f32=rowmap(q, HEADS * 64, R, 0))
+            ops.gemm(ctx, L["wkv"], 2 * HEADS * 64, a_batch=1, a_rows_per_batch=B * Nk, a_ld=dp, m_per_batch=B * Nk,
+                     out_f32=rowmap(kv, 2 * HEADS * 64, B * Nk, 0))
+            ops.cross_attention(q, kv, B, N, Nk, HEADS, att)
+            ops.gemm(att, L["wo"], D, a_batch=1, a_rows_per_batch=R, a_ld=HEADS * 64, m_per_batch=R, residual=lm, out_f32=lm)
+            ops.rows_to_planes(lat, 1, R, D, lp, dp, R, 0)
+            ops.gemm(lp, L["w1"], 2 * G["inner"], a_batch=1, a_rows_per_batch=R, a_ld=dp, m_per_batch=R, bias=L["b1"],
+                     out_f32=rowmap(ffh, 2 * G["inner"], R, 0))
+            ops.geglu_planes(ffh, R, G["inner"], hid, ip)
+            ops.gemm(hid, L["w2"], D, a_batch=1, a_rows_per_batch=R, a_ld=ip, m_per_batch=R, bias=L["b2"], residual=lm, out_f32=lm)
+        # ---- RMSNorm + ResidualFSQ (one quantizer) -> int32 indices [B, 1, N]
+        idx = torch.empty(B, 1, N, dtype=torch.int32, device=wav.device)
+        nl = len(s["fsq_levels"])
+        zt = torch.empty(R, nl, device=wav.device) if taps is not None else None
+        xn = torch.empty(R, D, device=wav.device) if taps is not None else None
+        ops.fsq_tokenize(lat, R, D, G["gamma"], G["w_in"], G["b_in"], s["fsq_levels"], s["fsq_num_quantizers"], idx, zt, xn)
+        if taps is not None:
+            taps.update(mel=mel.clone().reshape(B, T, -1), latent=lat32.clone().reshape(B, T, ECAPA_OUT), perceiver=xn.reshape(B, N, D),
+                        z=zt.reshape(B, N, nl))
+        return idx
 
     def forward(self, *a, **k):
         raise RuntimeError("unified_audio_b200.BiCodec implements detokenize only (the decoder UniSE uses, model.py:193)")

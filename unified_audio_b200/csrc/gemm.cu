@@ -96,6 +96,7 @@ __device__ __forceinline__ float apply_act(int act, float v) {
   if (act == QB_ACT_GELU) return gelu_fast(v);
   if (act == QB_ACT_ELU) return elu_f(v);
   if (act == QB_ACT_TANH) return tanhf(v);
+  if (act == QB_ACT_RELU) return v < 0.f ? 0.f : v;      // NaN passes, as torch.relu
   return v;
 }
 

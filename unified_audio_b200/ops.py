@@ -9,7 +9,7 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import ACT_ELU, ACT_GELU, ACT_NONE, ACT_SNAKE, ACT_SWIGLU, ACT_TANH, GemmDesc, RowMap  # noqa: F401
+from ._lib import ACT_ELU, ACT_GELU, ACT_NONE, ACT_RELU, ACT_SNAKE, ACT_SWIGLU, ACT_TANH, GemmDesc, RowMap  # noqa: F401
 
 
 def _stream():
@@ -358,6 +358,46 @@ def pad_wav(x, left, T_out, wrap=False):
     out = torch.empty(B, T_out, device=x.device)
     _lib.check(_lib.load().qb_pad_wav(_p(x), B, T, left, T_out, int(wrap), _p(out), _stream()))
     return out
+
+
+def mel_gather(wav, hop, n_fft, P, Q, window, out: Planes):
+    B, L = wav.shape
+    _lib.check(_lib.load().qb_mel_gather(_p(wav), B, L, hop, n_fft, P, Q, _p(window), _p(out.hi), _p(out.lo), _stream()))
+
+
+def spec_magnitude(X, ldX, M, nf, P, out: Planes, ld):
+    _lib.check(_lib.load().qb_spec_magnitude(_p(X), ldX, M, nf, P, _p(out.hi), _p(out.lo), ld, _stream()))
+
+
+def add_planes(x, ldx, y, ldy, B, T, Cc, out: Planes, ld, rows_per_batch, row_off):
+    """x (+ y) over Cc channels of rows with pitches ldx / ldy -> planes of a padded buffer (y may be None)"""
+    _lib.check(_lib.load().qb_add_planes(_p(x), ldx, _p(y), ldy, B, T, Cc, _p(out.hi), _p(out.lo), ld, rows_per_batch, row_off,
+                                         _stream()))
+
+
+def se_gate(z, B, T, Cc, w1, b1, w2, b2, s):
+    _lib.check(_lib.load().qb_se_gate(_p(z), B, T, Cc, _p(w1), _p(b1), w1.shape[0], _p(w2), _p(b2), _p(s), _stream()))
+
+
+def se_apply(z, s, x, B, T, Cc, out=None, planes: Optional[Planes] = None, ld=0, col_off=0):
+    hi = planes.hi if planes is not None else None
+    lo = planes.lo if planes is not None else None
+    _lib.check(_lib.load().qb_se_apply(_p(z), _p(s), _p(x), B, T, Cc, _p(out), _p(hi), _p(lo), ld, col_off, _stream()))
+
+
+def geglu_planes(h, rows, inner, out: Planes, ld):
+    """h [rows, 2 * inner] (value | gate) -> planes [rows, ld] = gelu(gate) * value"""
+    _lib.check(_lib.load().qb_geglu_planes(_p(h), rows, inner, _p(out.hi), _p(out.lo), ld, _stream()))
+
+
+def cross_attention(q, kv, B, Nq, Nk, heads, out: Planes):
+    _lib.check(_lib.load().qb_cross_attention(_p(q), _p(kv), B, Nq, Nk, heads, _p(out.hi), _p(out.lo), _stream()))
+
+
+def fsq_tokenize(x, rows, dim, gamma, w_in, b_in, levels, num_quantizers, idx, z=None, xn=None):
+    lv = (C.c_int32 * len(levels))(*levels)
+    _lib.check(_lib.load().qb_fsq_tokenize(_p(x), rows, dim, _p(gamma), _p(w_in), _p(b_in), len(levels), lv, num_quantizers, _p(idx),
+                                           _p(z), _p(xn), _stream()))
 
 
 def lm_loss(logits, ld, M, V, targets, label_smoothing):

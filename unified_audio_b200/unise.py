@@ -23,6 +23,7 @@ from typing import Optional
 import torch
 from torch import nn
 
+from . import ops
 from .ssl import wrap_segments
 
 STFT_CONFIG = dict(hop_length=320, win_length=640, n_fft=640, n_mels=80)      # U/conf/config.yaml:124-128
@@ -30,12 +31,28 @@ SEG_LEN = 5 * 16000                                                            #
 
 
 class BiCodecTokenizer(nn.Module):
-    """audio_tokenizer.py:30-125, detokenize side.  `tokenize` (wav2vec2-large-xlsr-53 features + the BiCodec encoder) is only
-    called by the training / validation steps (model.py:96-99,139-142): out of scope, raises."""
+    """audio_tokenizer.py:30-125, detokenize side and `get_ref_clip`.  `tokenize` (wav2vec2-large-xlsr-53 features + the BiCodec
+    encoder) is only called by the training / validation steps (model.py:96-99,139-142): out of scope, raises.
+    ref_segment_length = int(sample_rate * ref_segment_duration) // latent_hop_length * latent_hop_length (audio_tokenizer.py:60-64):
+    96000 for the published 16 kHz, 6 s, 320-sample configuration."""
 
-    def __init__(self, model):
+    def __init__(self, model, ref_segment_length: int = 96000):
         super().__init__()
         self.model = model
+        self.ref_segment_length = int(ref_segment_length)
+
+    @torch.no_grad()
+    def get_ref_clip(self, wav: torch.Tensor) -> torch.Tensor:
+        """audio_tokenizer.py:54-72: wav [B, L] -> [B, ref_segment_length]; a shorter wav is repeated (torch.tile) and cut, i.e.
+        wrap-padded on the device (`qb_pad_wav`)."""
+        if wav.device.type != "cuda":
+            raise RuntimeError("unified_audio_b200.unise.BiCodecTokenizer runs on CUDA only (no CPU fallback)")
+        if wav.ndim != 2:
+            raise ValueError("wav must be [B, L]")
+        n = self.ref_segment_length
+        if n > wav.shape[-1]:
+            return ops.pad_wav(wav, 0, n, wrap=True)
+        return wav[:, :n].float().contiguous()
 
     def tokenize(self, wav):
         raise NotImplementedError("BiCodecTokenizer.tokenize is used by the training / validation steps only (model.py:96-99); "
