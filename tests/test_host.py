@@ -146,8 +146,7 @@ def test_state_dict_layout_matches_reference(name):
     assert torch.equal(m.state_dict()["encoder.out.conv.bias"], sd["encoder.out.conv.bias"])
 
 
-def test_product_path_refuses_cpu():
-    """No CPU / PyTorch fallback: the product path must fail loudly without a CUDA device."""
+def _codec_on_cpu():
     from oracle import weights
     from unified_audio_b200.codec import Codec
     cfg = weights.h2_small()
@@ -155,10 +154,64 @@ def test_product_path_refuses_cpu():
               cfg["semantic_decoder_config"])
     m.load_state_dict(weights.make_h2_state_dict(cfg, 1))
     wav, feat = weights.synth_inputs(cfg, 1, 1, 5)
-    with pytest.raises((RuntimeError, AssertionError)):
-        m.encode(wav, feat)
-    with pytest.raises(RuntimeError):
-        m(wav, feat)
+    return [lambda: m.encode(wav, feat), lambda: m.decode(torch.zeros(1, 4, 1, dtype=torch.long), torch.zeros(1, 4, 1, dtype=torch.long)),
+            lambda: m(wav, feat)]
+
+
+def _codec_h1_on_cpu(h15):
+    from oracle import hcodec1, hcodec15
+    from unified_audio_b200.codec_h1 import CodecH1
+    from unified_audio_b200.codec_h15 import CodecH15
+    if h15:
+        m = CodecH15(_cfg={k: v for k, v in hcodec15.h15_shallow().items() if k != "layer_scale"})
+    else:
+        m = CodecH1(_cfg=hcodec1.h1_small())
+    x, feat = torch.zeros(1, 1, 1280), torch.zeros(1, m.c["sem_in"], 4)
+    return [lambda: m.encode(x, feat), lambda: m(x, feat)]
+
+
+def _ssl_on_cpu(kind):
+    from oracle import hubert as oh
+    from oracle import wav2vec2 as ow
+    from unified_audio_b200.ssl import SSLFrontEnd
+    c = dict(hubert=oh.hubert_small, wavlm=oh.wavlm_small, wav2vec2=ow.wav2vec2_small)[kind]()
+    m = SSLFrontEnd(dict(c, kind=kind))
+    return [lambda: m(torch.zeros(1, 4000)), lambda: m.resample(torch.zeros(1, 4000))]
+
+
+def _lm_on_cpu():
+    from oracle import llama
+    from unified_audio_b200.llm import LLM_SFT
+    c = llama.lm_small()
+    m = LLM_SFT(num_tasks=c["num_tasks"], task_map=c["task_map"], feats_dim=c["feats_dim"], llm_base_config=c["llm_base_config"])
+    mix, ids = torch.zeros(1, 4, c["feats_dim"]), torch.zeros(1, 4, dtype=torch.long)
+    return [lambda: m.generate("se", None, None, mix, mix, do_sample=False),
+            lambda: m("se", None, None, mix, mix, ids, ids), lambda: m.llm_forward(torch.zeros(1, 4, c["llm_base_config"]["hidden_size"]))]
+
+
+def _bicodec_on_cpu(global_tokens):
+    from oracle import bicodec_global as og
+    from unified_audio_b200.bicodec import BiCodec
+    m = BiCodec(og.bicodec_global_small(), global_tokens=global_tokens)
+    calls = [lambda: m.detokenize(torch.zeros(1, 4, dtype=torch.long), torch.zeros(1, 1, 8, dtype=torch.long))]
+    if global_tokens:
+        calls += [lambda: m.get_global_tokens({"ref_wav": torch.zeros(1, 4000)}), lambda: m.mel_spectrogram(torch.zeros(1, 4000))]
+    return calls
+
+
+def test_product_path_refuses_cpu():
+    """No CPU / PyTorch fallback: the product path of every face, each at a small config, fails loudly without a CUDA device."""
+    faces = {"Codec": _codec_on_cpu, "CodecH1": lambda: _codec_h1_on_cpu(False), "CodecH15": lambda: _codec_h1_on_cpu(True),
+             "SSLFrontEnd hubert": lambda: _ssl_on_cpu("hubert"), "SSLFrontEnd wavlm": lambda: _ssl_on_cpu("wavlm"),
+             "SSLFrontEnd wav2vec2": lambda: _ssl_on_cpu("wav2vec2"), "LLM_SFT": _lm_on_cpu,
+             "BiCodec": lambda: _bicodec_on_cpu(False), "BiCodec global_tokens": lambda: _bicodec_on_cpu(True)}
+    for face, make in faces.items():
+        for i, call in enumerate(make()):
+            try:
+                call()
+            except RuntimeError:
+                continue
+            pytest.fail(f"{face}: entry point {i} ran on the CPU without raising RuntimeError")
 
 
 def test_product_does_not_import_oracle():

@@ -34,10 +34,9 @@ import math
 from typing import Dict
 
 import torch
-from torch import nn
 
 from . import ops
-from .codec import _Tree, _pad_to
+from .codec import _Face, _Tree, _pad_to
 from .ops import ACT_GELU, ACT_RELU, ACT_SNAKE, ACT_TANH, Planes, rowmap
 
 BICODEC_CONFIG = dict(
@@ -201,7 +200,7 @@ def mel_filterbank(mp) -> torch.Tensor:
     return fb * (2.0 / (f[2:] - f[:-2]))[None, :]
 
 
-class BiCodec(nn.Module):
+class BiCodec(_Face):
     """`global_tokens=True` adds the global-token path (`mel_spectrogram`, `get_global_tokens`): its reference keys become part of
     the module and are required by a strict load.  The default object is the detokenize path alone."""
 
@@ -216,49 +215,24 @@ class BiCodec(nn.Module):
         tree = _Tree.build(spec)
         for name, child in tree.named_children():
             self.add_module(name, child)
-        self._w, self._wg, self._ws = None, None, {}
+        self._wg = None                 # prepared weights of the global-token path
         self.eval()
 
     # ------------------------------------------------------------------ state
-    def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
+    def _ignored_key(self, key: str) -> bool:
         if self.global_tokens:
-            sd = {k: v for k, v in state_dict.items() if not k.startswith(_IGNORED_GLOBAL) and not k.endswith(".num_batches_tracked")}
-        else:
-            sd = {k: v for k, v in state_dict.items() if not k.startswith(_IGNORED)}
-        r = super().load_state_dict(sd, strict=strict, assign=assign)
-        self._w, self._wg = None, None
-        return r
+            return key.startswith(_IGNORED_GLOBAL) or key.endswith(".num_batches_tracked")
+        return key.startswith(_IGNORED)
 
-    def _apply(self, fn, *a, **k):
-        self._w, self._wg, self._ws = None, None, {}
-        return super()._apply(fn, *a, **k)
-
-    def _dev(self):
-        return self.quantizer.codebook.weight.device
-
-    def _buf(self, name, shape, dtype=torch.float32):
-        key = (name, tuple(shape), dtype)
-        t = self._ws.get(key)
-        if t is None:
-            t = torch.zeros(shape, dtype=dtype, device=self._dev())
-            self._ws[key] = t
-        return t
-
-    def _planes(self, name, shape, split):
-        key = ("P", name, tuple(shape), bool(split))
-        p = self._ws.get(key)
-        if p is None:
-            p = Planes.zeros(shape, split, self._dev())
-            self._ws[key] = p
-        return p
+    def _drop_prepared(self):
+        super()._drop_prepared()
+        self._wg = None
 
     # ------------------------------------------------------------------ load-time weight preparation
     def _prepare(self):
         if self._w is not None:
             return self._w
-        dev = self._dev()
-        if dev.type != "cuda":
-            raise RuntimeError("unified_audio_b200.BiCodec runs on CUDA only (no CPU fallback): call .cuda() first")
+        dev = self._require_cuda()
         sd = {k: v.detach().float() for k, v in self.state_dict().items()}
         c = self.cfg
         q, s, p, d = c["quantizer"], c["speaker"], c["prenet"], c["decoder"]
@@ -267,13 +241,6 @@ class BiCodec(nn.Module):
         def wnw(prefix):      # fold torch.nn.utils.weight_norm (dim 0): w = g * v / ||v||   (layers.py:24-29)
             v, g = sd[prefix + "weight_v"], sd[prefix + "weight_g"]
             return v * (g / v.reshape(v.shape[0], -1).norm(dim=1).reshape(g.shape))
-
-        def conv_pack(w, split):   # [Cout, Cin, k] -> planes [Cout, k * Cin_pad] (tap-major K, zero channel padding)
-            co, ci, k = w.shape
-            cp = _pad_to(ci, 64)
-            out = torch.zeros(co, k, cp, device=dev)
-            out[:, :, :ci] = w.permute(0, 2, 1)
-            return Planes.from_f32(out.reshape(co, k * cp), split)
 
         def convt_pack(w, s_, split):
             """ConvTranspose1d weight [Cin, Cout, k], stride s -> [s * Cout, J * Cin_pad], J = ceil(k / s):
@@ -320,7 +287,7 @@ class BiCodec(nn.Module):
                 if not cond:
                     blk.update(ln_w=sd[b + "norm.weight"].contiguous(), ln_b=sd[b + "norm.bias"].contiguous())
                 blocks.append(blk)
-            out = dict(embed=conv_pack(sd[prefix + "embed.weight"] * in_scale, sp_pre), embed_b=sd[prefix + "embed.bias"].contiguous(),
+            out = dict(embed=ops.conv_planes(sd[prefix + "embed.weight"] * in_scale, sp_pre), embed_b=sd[prefix + "embed.bias"].contiguous(),
                        blocks=blocks, fn_w=sd[prefix + "final_layer_norm.weight"].contiguous(),
                        fn_b=sd[prefix + "final_layer_norm.bias"].contiguous(), layers=layers)
             if not cond:
@@ -340,7 +307,7 @@ class BiCodec(nn.Module):
         W["lin_b"] = sd["prenet.linear.bias"].contiguous()
 
         # ---- WaveGenerator
-        G = dict(conv0=conv_pack(wnw("decoder.model.0."), sp_gen), conv0_b=sd["decoder.model.0.bias"].contiguous(), stages=[])
+        G = dict(conv0=ops.conv_planes(wnw("decoder.model.0."), sp_gen), conv0_b=sd["decoder.model.0.bias"].contiguous(), stages=[])
         ch = d["channels"]
         for i, (k, r) in enumerate(zip(d["kernel_sizes"], d["rates"])):
             cin, cout = ch // 2 ** i, ch // 2 ** (i + 1)
@@ -350,13 +317,13 @@ class BiCodec(nn.Module):
                       bt=sd[b + "1.bias"].repeat(r).contiguous(), units=[])
             for j, dil in enumerate((1, 3, 9)):
                 u = f"{b}{j + 2}.block."
-                st["units"].append(dict(dil=dil, a1=sd[u + "0.alpha"].reshape(-1).contiguous(), w1=conv_pack(wnw(u + "1."), sp_gen),
+                st["units"].append(dict(dil=dil, a1=sd[u + "0.alpha"].reshape(-1).contiguous(), w1=ops.conv_planes(wnw(u + "1."), sp_gen),
                                         b1=sd[u + "1.bias"].contiguous(), a2=sd[u + "2.alpha"].reshape(-1).contiguous(),
-                                        w2=conv_pack(wnw(u + "3."), sp_gen), b2=sd[u + "3.bias"].contiguous()))
+                                        w2=ops.conv_planes(wnw(u + "3."), sp_gen), b2=sd[u + "3.bias"].contiguous()))
             G["stages"].append(st)
         n = len(d["rates"])
         G["alpha_f"] = sd[f"decoder.model.{n + 1}.alpha"].reshape(-1).contiguous()
-        G["conv_f"] = conv_pack(wnw(f"decoder.model.{n + 2}."), sp_gen)
+        G["conv_f"] = ops.conv_planes(wnw(f"decoder.model.{n + 2}."), sp_gen)
         G["conv_f_b"] = sd[f"decoder.model.{n + 2}.bias"].contiguous()
         W["gen"] = G
         self._w = W
@@ -531,9 +498,7 @@ class BiCodec(nn.Module):
             return self._wg
         if not self.global_tokens:
             raise RuntimeError("this BiCodec was built without the global-token path: construct it with BiCodec(..., global_tokens=True)")
-        dev = self._dev()
-        if dev.type != "cuda":
-            raise RuntimeError("unified_audio_b200.BiCodec runs on CUDA only (no CPU fallback): call .cuda() first")
+        dev = self._require_cuda()
         keys = speaker_spec(self.cfg)
         sd = {k: v.detach().double().cpu() for k, v in self.state_dict().items() if k in keys}
         mp, s = self._mel_params(), self.cfg["speaker"]
@@ -543,22 +508,11 @@ class BiCodec(nn.Module):
         if s["fsq_num_quantizers"] != 1:
             raise NotImplementedError("residual FSQ with more than one quantizer (the shipped speaker encoder uses one)")
 
-        def pl(w):
-            return Planes.from_f32(w.float().to(dev), True)
-
-        def conv_pack(w):          # [Cout, Cin, k] -> [Cout, k * Cin_pad], tap-major K
-            co, ci, k = w.shape
-            out = torch.zeros(co, k, _pad_to(ci, 64), dtype=torch.float64)
-            out[:, :, :ci] = w.permute(0, 2, 1)
-            return pl(out.reshape(co, -1))
-
-        def pad_k(w, kp):          # [N, K] -> [N, kp]
-            out = torch.zeros(w.shape[0], kp, dtype=torch.float64)
-            out[:, :w.shape[1]] = w
-            return pl(out)
-
         def f32(t):
             return t.float().contiguous().to(dev)
+
+        def pl(w):
+            return Planes.from_f32(f32(w), True)
 
         def crb(p, w, b):          # Conv1dReluBn: conv -> ReLU -> eval BatchNorm as the GEMM's gamma and broadcast residual row
             g = sd[p + "bn.weight"] / torch.sqrt(sd[p + "bn.running_var"] + 1e-5)
@@ -580,17 +534,17 @@ class BiCodec(nn.Module):
         tw = torch.stack([torch.cos(ang(bb * kk, n_fft)), -torch.sin(ang(bb * kk, n_fft))], -1)       # [b, k1, (cos, -sin)]
         fp = _pad_to(nf, 64)
         G.update(P=P, Q=Q, K2=K2, ldX=_pad_to(2 * K2, 4), fp=fp, wA=pl(wA), wB=pl(wB), tw=f32(tw), window=f32(hann_window(mp)),
-                 fb=pad_k(mel_filterbank(mp).t(), fp))
+                 fb=ops.pad_k_planes(f32(mel_filterbank(mp).t()), fp))
         # ---- ECAPA-TDNN up to its latent
         E = "speaker_encoder.speaker_encoder."
-        G["l1"] = crb(E + "layer1.", conv_pack(sd[E + "layer1.conv.weight"]), sd[E + "layer1.conv.bias"])
+        G["l1"] = crb(E + "layer1.", ops.conv_planes(f32(sd[E + "layer1.conv.weight"])), sd[E + "layer1.conv.bias"])
         G["blocks"] = []
         for k in (2, 3, 4):
             p = f"{E}layer{k}.se_res2block."
             res2 = []
             for i in range(ECAPA_SCALE - 1):
                 g = sd[f"{p}1.bns.{i}.weight"] / torch.sqrt(sd[f"{p}1.bns.{i}.running_var"] + 1e-5)
-                res2.append(dict(w=conv_pack(sd[f"{p}1.convs.{i}.weight"]), b=f32(sd[f"{p}1.convs.{i}.bias"]), g=f32(g),
+                res2.append(dict(w=ops.conv_planes(f32(sd[f"{p}1.convs.{i}.weight"])), b=f32(sd[f"{p}1.convs.{i}.bias"]), g=f32(g),
                                  t=f32(sd[f"{p}1.bns.{i}.bias"] - sd[f"{p}1.bns.{i}.running_mean"] * g)))
             G["blocks"].append(dict(
                 dil=k, res2=res2,
@@ -607,9 +561,9 @@ class BiCodec(nn.Module):
                  proj_b=f32(sd[Pp + "proj_context.bias"]), latents=f32(sd[Pp + "latents"]), layers=[])
         for layer in range(2):
             q = f"{Pp}layers.{layer}."
-            G["layers"].append(dict(wq=pad_k(sd[q + "0.to_q.weight"], dp), wkv=pad_k(sd[q + "0.to_kv.weight"], dp),
-                                    wo=pl(sd[q + "0.to_out.weight"]), w1=pad_k(sd[q + "1.0.weight"], dp), b1=f32(sd[q + "1.0.bias"]),
-                                    w2=pad_k(sd[q + "1.2.weight"], _pad_to(inner, 64)), b2=f32(sd[q + "1.2.bias"])))
+            G["layers"].append(dict(wq=ops.pad_k_planes(f32(sd[q + "0.to_q.weight"]), dp), wkv=ops.pad_k_planes(f32(sd[q + "0.to_kv.weight"]), dp),
+                                    wo=pl(sd[q + "0.to_out.weight"]), w1=ops.pad_k_planes(f32(sd[q + "1.0.weight"]), dp), b1=f32(sd[q + "1.0.bias"]),
+                                    w2=ops.pad_k_planes(f32(sd[q + "1.2.weight"]), _pad_to(inner, 64)), b2=f32(sd[q + "1.2.bias"])))
         G.update(gamma=f32(sd[Pp + "norm.gamma"]), w_in=f32(sd["speaker_encoder.quantizer.project_in.weight"]),
                  b_in=f32(sd["speaker_encoder.quantizer.project_in.bias"]))
         self._wg = G

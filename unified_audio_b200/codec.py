@@ -10,7 +10,7 @@ codec.py:71) are accepted by load_state_dict and ignored.
 `encode` / `decode` are one call each into the C ABI (csrc/engine.cu through engine.py): the engine owns the repacked
 weights, the workspace and the ~340-kernel orchestration, with activations channel-last [B*T, C] end to end.  There is no
 PyTorch / CPU fallback.  H-Codec-1.0 / 1.5 (codec_h1.py, codec_h15.py) launch their kernels op by op from Python instead;
-they share `_CodecFace` with this class.
+they share `_CodecFace` with this class.  `_Face`, the base of every face of the package, is defined here too.
 """
 from __future__ import annotations
 
@@ -59,16 +59,27 @@ def _pad_to(n, m):
     return (n + m - 1) // m * m
 
 
-class _CodecFace(nn.Module):
-    """What the codec faces share: the checkpoint filter, dropping the prepared weights when the parameters or the device
-    change, CUDA-graph capture, the encode -> decode round trip and the refusal of the training forward.  Each face says in
-    `_drop_prepared` what it derives from its parameters."""
+class _Face(nn.Module):
+    """What every face over libquark_b200 shares.  `_w` holds the weights prepared from the parameters (None = not prepared
+    yet, or stale) and `_ws` the zero-initialised scratch buffers and shape-keyed tables.  Both are dropped whenever the
+    parameters or the device change (`load_state_dict`, `.to()` / `.cuda()` / `.half()`); a face that derives more state
+    from them drops it in `_drop_prepared`.  `load_state_dict` accepts the reference checkpoint's keys that the face does not
+    hold (`_ignored_key`)."""
+
+    _IGNORED_KEYS: tuple = ()          # checkpoint key prefixes accepted at load and not kept
+
+    def __init__(self):
+        super().__init__()
+        self._w, self._ws = None, {}
 
     def _drop_prepared(self):
-        raise NotImplementedError
+        self._w, self._ws = None, {}
+
+    def _ignored_key(self, key: str) -> bool:
+        return key.startswith(self._IGNORED_KEYS)
 
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
-        sd = {k: v for k, v in state_dict.items() if not k.startswith("semantic_decoder.")}
+        sd = {k: v for k, v in state_dict.items() if not self._ignored_key(k)}
         r = super().load_state_dict(sd, strict=strict, assign=assign)
         self._drop_prepared()
         return r
@@ -76,6 +87,37 @@ class _CodecFace(nn.Module):
     def _apply(self, fn, *a, **k):
         self._drop_prepared()
         return super()._apply(fn, *a, **k)
+
+    def _dev(self):
+        return next(self.parameters()).device
+
+    def _require_cuda(self):
+        dev = self._dev()
+        if dev.type != "cuda":
+            raise RuntimeError(f"unified_audio_b200.{type(self).__name__} runs on CUDA only (no CPU fallback): call .cuda() first")
+        return dev
+
+    def _cached(self, key, build):
+        """`_ws[key]`, built by `build()` on first use."""
+        v = self._ws.get(key)
+        if v is None:
+            v = self._ws[key] = build()
+        return v
+
+    def _buf(self, name, shape, dtype=torch.float32):
+        """Zero-initialised scratch tensor: kernels rely on the pad rows / columns they never write staying zero."""
+        return self._cached(("buf", name, tuple(shape), dtype), lambda: torch.zeros(shape, dtype=dtype, device=self._dev()))
+
+    def _planes(self, name, shape, split=True):
+        """Zero-initialised fp16 hi (+ lo if `split`) planes."""
+        return self._cached(("planes", name, tuple(shape), bool(split)), lambda: ops.Planes.zeros(shape, split, self._dev()))
+
+
+class _CodecFace(_Face):
+    """The codec faces add CUDA-graph capture, the encode -> decode round trip and the refusal of the training forward; their
+    checkpoints carry the training-only `semantic_decoder.*`."""
+
+    _IGNORED_KEYS = ("semantic_decoder.",)
 
     # ------------------------------------------------------------------ CUDA-graph replay of a fixed-shape call
     def graphed(self, fn_name: str, *example_inputs, warmup: int = 2) -> "GraphedCall":
@@ -116,15 +158,14 @@ class Codec(_CodecFace):
         self.eval()
 
     def _drop_prepared(self):
+        super()._drop_prepared()
         self._engine = None
 
     def engine(self):
         """The qb_codec handle of this model (built lazily from the current parameters)."""
         if self._engine is None:
             from .engine import CodecEngine
-            dev = next(self.parameters()).device
-            if dev.type != "cuda":
-                raise RuntimeError("unified_audio_b200.Codec runs on CUDA only (no CPU fallback): call .cuda() first")
+            dev = self._require_cuda()
             self._engine = CodecEngine(dev, self.enc_cfg, self.dec_cfg, dict(num_quantizers=self.quantizer.num_quantizers,
                                                                              codebook_size=self.quantizer.codebook_size),
                                        self.sem_cfg, self.precision, {k: v for k, v in self.state_dict().items()})

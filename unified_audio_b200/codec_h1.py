@@ -135,30 +135,20 @@ class CodecH1(_CodecFace):
                             channel_ratios=[1] * len(c["sem_strides"]))
         self.dec_cfg = dict(dim=c["dec_dim"], intermediate_dim=c["dec_inter"])
         self.policy = dict(PRECISION_POLICIES[precision])
-        self._w, self._ws = None, {}        # repacked weights (device planes), workspace cache
         self.precision = precision
         self.eval()
-
-    def _drop_prepared(self):
-        self._w, self._ws = None, {}
 
     # ------------------------------------------------------------------ weight repack
     def _prepare(self):
         if self._w is not None:
             return self._w
         sd = {k: v.detach() for k, v in self.state_dict().items()}
-        dev = next(self.parameters()).device
-        if dev.type != "cuda":
-            raise RuntimeError("unified_audio_b200.CodecH1 runs on CUDA only (no CPU fallback): call .cuda() first")
+        dev = self._require_cuda()
         pol, c = self.policy, self.c
         W: Dict[str, object] = {}
 
-        def pack(w, group):                                          # [Cout, Cin, k] -> planes [Cout, k*Cin_pad]
-            cout, cin, k = w.shape
-            cpad = _pad_to(cin, 64)
-            wp = torch.zeros(cout, k, cpad, device=dev)
-            wp[:, :, :cin] = w.float().permute(0, 2, 1)
-            return Planes.from_f32(wp.reshape(cout, k * cpad), pol[group])
+        def pack(w, group):
+            return ops.conv_planes(w.float(), pol[group])
 
         def wn(p):     # fold old-style weight norm: w = g * v / ||v||  (encoder_modules/conv.py:25-28)
             v = sd[p + "conv.conv.weight_v"].double()
@@ -250,35 +240,6 @@ class CodecH1(_CodecFace):
                 w2=lw(sd[p + "mlp.w2.weight"], "mlp")))
         return layers
 
-    # ------------------------------------------------------------------ workspace
-    def _buf(self, name, shape, dtype=torch.float32):
-        key = (name, tuple(shape), dtype)
-        t = self._ws.get(key)
-        if t is None:
-            t = torch.zeros(shape, dtype=dtype, device=next(self.parameters()).device)
-            self._ws[key] = t
-        return t
-
-    def _planes(self, name, shape, split):
-        key = ("P", name, tuple(shape), bool(split))
-        p = self._ws.get(key)
-        if p is None:
-            p = Planes.zeros(shape, split, next(self.parameters()).device)
-            self._ws[key] = p
-        return p
-
-    def _rope(self, T, D=64):
-        key = ("rope", T, D)
-        r = self._ws.get(key)
-        if r is None:
-            inv = 1.0 / (10000.0 ** (torch.arange(0, D, 2, dtype=torch.int64).float() / D))
-            fr = torch.arange(T).float()[:, None] * inv[None, :]
-            emb = torch.cat((fr, fr), dim=-1)
-            dev = next(self.parameters()).device
-            r = (emb.cos().to(dev).contiguous(), emb.sin().to(dev).contiguous())
-            self._ws[key] = r
-        return r
-
     # ------------------------------------------------------------------ blocks
     def _linear(self, a, w, n, M, K, **kw):
         ops.gemm(a, w, n, a_batch=1, a_rows_per_batch=M, a_ld=K, m_per_batch=M, **kw)
@@ -309,7 +270,7 @@ class CodecH1(_CodecFace):
         use_tc = layers[0]["whh_perm"] is not None and B <= 256
         ws = self._buf("lstm_ws", (max(ops.lstm_workspace_bytes(B, C), ops.lstm_tc_workspace_bytes(B, C)),), torch.uint8)
         lstm_u = ops.lstm_tc_units(C) if use_tc else 0
-        cos, sin = self._rope(F, hd)
+        cos, sin = self._cached(("rope", F, hd), lambda: ops.rope_tables(F, hd, self._dev()))
         legacy = os.environ.get("QB_ATTENTION", "umma") == "legacy"
         umma = (not legacy) and hd in (64, 128)          # wgmma attention (csrc/attention_umma.cu), both precision policies
         tc_att = (not umma) and (not pa) and hd == 64

@@ -138,16 +138,10 @@ class CodecH15(CodecH1):
 
     def _rope_mimi(self, L, hd):
         """module/rope.py:38-40, 57-58 in the rotate-half layout: cos / sin [L, hd] with column j and j + hd/2 = frequency j"""
-        key = ("rope_mimi", L, hd)
-        r = self._ws.get(key)
-        if r is None:
-            freqs = torch.exp(torch.arange(hd // 2, dtype=torch.float32) * (-math.log(10000.0) * 2 / hd))
-            ang = torch.arange(L, dtype=torch.float32)[:, None] * freqs[None]
-            emb = torch.cat((ang, ang), -1)
-            dev = next(self.parameters()).device
-            r = (emb.cos().to(dev).contiguous(), emb.sin().to(dev).contiguous())
-            self._ws[key] = r
-        return r
+        freqs = torch.exp(torch.arange(hd // 2, dtype=torch.float32) * (-math.log(10000.0) * 2 / hd))
+        ang = torch.arange(L, dtype=torch.float32)[:, None] * freqs[None]
+        emb = torch.cat((ang, ang), -1)
+        return emb.cos().to(self._dev()).contiguous(), emb.sin().to(self._dev()).contiguous()
 
     # ------------------------------------------------------------------ mimi transformer
     def _mimi(self, layers, x, B, L, t, split, taps=None, tap_name=None):
@@ -158,7 +152,7 @@ class CodecH15(CodecH1):
         t_b = self._planes("mm_b", (M, C), split)
         hid = self._planes("mm_hid", (M, FF), split)
         qkv = self._buf("mm_qkv", (M, 3 * C))
-        cos, sin = self._rope_mimi(L, hd)
+        cos, sin = self._cached(("rope_mimi", L, hd), lambda: self._rope_mimi(L, hd))
         umma = hd in (64, 128) and os.environ.get("QB_ATTENTION", "umma") != "legacy"      # wgmma attention (csrc/attention_umma.cu)
         tc_att = (not umma) and (not split) and hd == 64
         att_ws = (self._buf("att5_ws", (ops.attention_umma_workspace_bytes(B, L, heads, hd, split),), torch.uint8) if umma else

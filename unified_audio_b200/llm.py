@@ -22,10 +22,9 @@ import os
 from typing import Optional
 
 import torch
-from torch import nn
 
 from . import ops
-from .codec import _Tree
+from .codec import _Face, _Tree, _pad_to
 from .ops import ACT_SWIGLU, Planes, rowmap
 
 
@@ -83,7 +82,9 @@ class LMOutput:
     past_key_values: Optional[StaticKVCache] = None
 
 
-class LLM_SFT(nn.Module):
+class LLM_SFT(_Face):
+    _IGNORED_KEYS = ("cond_", "rotary_emb.")         # the conformer condition encoder is never executed
+
     def __init__(self, num_tasks: int = 1, task_map: dict = None, feats_dim: int = 768, llm_base_config: dict = None):
         super().__init__()
         b = dict(llm_base_config or {})
@@ -101,7 +102,6 @@ class LLM_SFT(nn.Module):
         tree = _Tree.build(lm_spec(b, num_tasks, feats_dim))
         for name, child in tree.named_children():
             self.add_module(name, child)
-        self._w, self._ws = None, {}
         self.graph_steps = int(os.environ.get("QB_LM_GRAPH_STEPS", "8"))     # decode steps per replayed CUDA graph
         self._gen_state = {}
         # generate() walks a batch in chunks of <= `chunk` sequences; `lanes` > 1 runs that many chunks CONCURRENTLY, each on its own
@@ -118,25 +118,14 @@ class LLM_SFT(nn.Module):
         self.eval()
 
     # ------------------------------------------------------------------ state
-    def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
-        sd = {k: v for k, v in state_dict.items() if not k.startswith(("cond_", "rotary_emb."))}
-        r = super().load_state_dict(sd, strict=strict, assign=assign)
-        self._w, self._gen_state, self._lane_views = None, {}, None          # captured graphs point at the old prepared weights
-        return r
-
-    def _apply(self, fn, *a, **k):
-        self._w, self._ws, self._gen_state, self._lane_views = None, {}, {}, None
-        return super()._apply(fn, *a, **k)
-
-    def _dev(self):
-        return self.norm.weight.device
+    def _drop_prepared(self):
+        super()._drop_prepared()
+        self._gen_state, self._lane_views = {}, None          # captured graphs point into the dropped weights and workspace
 
     def _prepare(self):
         if self._w is not None:
             return self._w
-        dev = self._dev()
-        if dev.type != "cuda":
-            raise RuntimeError("unified_audio_b200.LLM_SFT runs on CUDA only (no CPU fallback): call .cuda() first")
+        self._require_cuda()
         sd = {k: v.detach().float() for k, v in self.state_dict().items()}
         layers = []
         for i in range(self.n_layers):
@@ -158,8 +147,8 @@ class LLM_SFT(nn.Module):
         self._w = dict(layers=layers, norm=sd["norm.weight"].contiguous(), head=Planes.from_f32(sd["output_head.weight"], True),
                        head_p=ops.lm_pack_weight(sd["output_head.weight"] * sd["norm.weight"][None, :]),
                        emb=sd["codec_embedding.weight"].contiguous(),
-                       adapter=Planes.from_f32(sd["adapter.weight"], True), adapter_b=sd["adapter.bias"].contiguous(),
-                       cos=None, sin=None, rope_rows=0)
+                       adapter=ops.pad_k_planes(sd["adapter.weight"], _pad_to(sd["adapter.weight"].shape[1], 64)),
+                       adapter_b=sd["adapter.bias"].contiguous(), cos=None, sin=None, rope_rows=0)
         self._ensure_rope(self.max_pos)
         return self._w
 
@@ -172,27 +161,9 @@ class LLM_SFT(nn.Module):
         if W["rope_rows"] >= n_positions:
             return
         rows = max(self.max_pos, -(-n_positions // 1024) * 1024)
-        inv = 1.0 / (10000.0 ** (torch.arange(0, 64, 2, dtype=torch.int64).float() / 64))
-        fr = torch.arange(rows).float()[:, None] * inv[None, :]
-        emb = torch.cat((fr, fr), -1)
-        W["cos"], W["sin"], W["rope_rows"] = emb.cos().to(self._dev()).contiguous(), emb.sin().to(self._dev()).contiguous(), rows
+        W["cos"], W["sin"] = ops.rope_tables(rows, 64, self._dev())
+        W["rope_rows"] = rows
         self._gen_state = {}
-
-    def _buf(self, name, shape, dtype=torch.float32):
-        key = (name, tuple(shape), dtype)
-        t = self._ws.get(key)
-        if t is None:
-            t = torch.zeros(shape, dtype=dtype, device=self._dev())
-            self._ws[key] = t
-        return t
-
-    def _planes(self, name, shape):
-        key = ("P", name, tuple(shape))
-        p = self._ws.get(key)
-        if p is None:
-            p = Planes.zeros(shape, True, self._dev())
-            self._ws[key] = p
-        return p
 
     # ------------------------------------------------------------------ transformer stack
     def _prefill(self, x: torch.Tensor, B: int, L: int, cache: StaticKVCache):
@@ -290,16 +261,13 @@ class LLM_SFT(nn.Module):
     def _adapter(self, feats):
         W = self._prepare()
         B, T, Fd = feats.shape
-        fpad = (Fd + 63) // 64 * 64
+        if Fd != self.adapter.weight.shape[1]:
+            raise ValueError(f"features have {Fd} channels, the adapter takes {self.adapter.weight.shape[1]}")
+        fpad = W["adapter"].hi.shape[1]
         a = Planes.zeros((B * T, fpad), True, feats.device)
         ops.rows_to_planes(feats.float().contiguous(), 1, B * T, Fd, a, fpad, B * T, 0)
-        wpad = W.get("adapter_pad")
-        if wpad is None:
-            w = torch.zeros(self.hidden, fpad, device=feats.device)
-            w[:, :Fd] = self.adapter.weight.detach().float()
-            wpad = W["adapter_pad"] = Planes.from_f32(w, True)
         out = torch.empty(B * T, self.hidden, device=feats.device)
-        ops.gemm(a, wpad, self.hidden, a_batch=1, a_rows_per_batch=B * T, a_ld=fpad, m_per_batch=B * T, bias=W["adapter_b"],
+        ops.gemm(a, W["adapter"], self.hidden, a_batch=1, a_rows_per_batch=B * T, a_ld=fpad, m_per_batch=B * T, bias=W["adapter_b"],
                  out_f32=rowmap(out, self.hidden, B * T, 0))
         return out.reshape(B, T, self.hidden)
 

@@ -46,6 +46,30 @@ class Planes:
         return self.hi.float() + (self.lo.float() if self.lo is not None else 0.0)
 
 
+def conv_planes(w: torch.Tensor, split: bool = True) -> Planes:
+    """Conv1d weight [Cout, Cin, k] -> planes [Cout, k * pad64(Cin)], the convolution weight of qb_gemm_desc: tap-major K,
+    input channels zero-padded to a multiple of 64."""
+    co, ci, k = w.shape
+    out = w.new_zeros(co, k, (ci + 63) // 64 * 64)
+    out[:, :, :ci] = w.permute(0, 2, 1)
+    return Planes.from_f32(out.reshape(co, -1), split)
+
+
+def pad_k_planes(w: torch.Tensor, kp: int, split: bool = True) -> Planes:
+    """Dense weight [N, K] -> planes [N, kp], columns K..kp zero (K padded to the GEMM's multiple of 64)."""
+    out = w.new_zeros(w.shape[0], kp)
+    out[:, :w.shape[1]] = w
+    return Planes.from_f32(out, split)
+
+
+def rope_tables(T: int, D: int, device):
+    """RoPE cos / sin [T, D] in the rotate-half layout: columns j and j + D/2 hold position * 10000^(-2j / D)."""
+    inv = 1.0 / (10000.0 ** (torch.arange(0, D, 2, dtype=torch.int64).float() / D))
+    fr = torch.arange(T).float()[:, None] * inv[None, :]
+    emb = torch.cat((fr, fr), -1)
+    return emb.cos().to(device).contiguous(), emb.sin().to(device).contiguous()
+
+
 def rowmap(t: Optional[torch.Tensor], ld=0, rows_per_batch=0, row_off=0) -> RowMap:
     return RowMap(_p(t), ld, rows_per_batch, row_off)
 

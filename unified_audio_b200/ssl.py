@@ -35,7 +35,7 @@ import torch
 from torch import nn
 
 from . import ops
-from .codec import _Tree, _pad_to
+from .codec import _Face, _Tree, _pad_to
 from .ops import ACT_GELU, Planes, rowmap
 
 HUBERT_BASE = dict(conv_dim=[512] * 7, conv_kernel=[10, 3, 3, 3, 3, 2, 2], conv_stride=[5, 2, 2, 2, 2, 2, 2], hidden=768,
@@ -107,7 +107,9 @@ def resample_kernel(orig: int, new: int, lowpass_filter_width: int = 6, rolloff:
     return kern.float(), width, orig, new
 
 
-class SSLFrontEnd(nn.Module):
+class SSLFrontEnd(_Face):
+    _IGNORED_KEYS = ("masked_spec_embed",)          # pre-training only
+
     def __init__(self, config: Optional[dict] = None, in_rate: int = 16000, compress: bool = False):
         """config: HUBERT_BASE / WAVLM_BASE_PLUS / WAV2VEC2_XLSR53 (or a reduced dict of the same keys).  in_rate 48000 adds the
         tokenizer's Resample(48k -> 16k); compress adds sign(x)|x|^0.3 (H-Codec tokenizer) - UniSE and BiCodec use neither."""
@@ -121,56 +123,17 @@ class SSLFrontEnd(nn.Module):
         tree = _Tree.build(ssl_spec(self.cfg))
         for name, child in tree.named_children():
             self.add_module(name, child)
-        self._w, self._ws = None, {}
         self.eval()
-
-    def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
-        sd = {k: v for k, v in state_dict.items() if not k.startswith("masked_spec_embed")}
-        r = super().load_state_dict(sd, strict=strict, assign=assign)
-        self._w = None
-        return r
-
-    def _apply(self, fn, *a, **k):
-        self._w, self._ws = None, {}
-        return super()._apply(fn, *a, **k)
-
-    def _dev(self):
-        return self.encoder.layer_norm.weight.device
-
-    def _buf(self, name, shape, dtype=torch.float32):
-        key = (name, tuple(shape), dtype)
-        t = self._ws.get(key)
-        if t is None:
-            t = torch.zeros(shape, dtype=dtype, device=self._dev())
-            self._ws[key] = t
-        return t
-
-    def _planes(self, name, shape):
-        key = ("P", name, tuple(shape))
-        p = self._ws.get(key)
-        if p is None:
-            p = Planes.zeros(shape, True, self._dev())
-            self._ws[key] = p
-        return p
 
     # ------------------------------------------------------------------ weight repack
     def _prepare(self):
         if self._w is not None:
             return self._w
-        dev = self._dev()
-        if dev.type != "cuda":
-            raise RuntimeError("unified_audio_b200.SSLFrontEnd runs on CUDA only (no CPU fallback): call .cuda() first")
+        dev = self._require_cuda()
         c = self.cfg
         sd = {k: v.detach().float() for k, v in self.state_dict().items()}
         W: Dict[str, object] = {}
         f32 = lambda k: sd[k].contiguous()
-
-        def conv_w(w):                          # [Cout, Cin, k] -> [Cout, k * Cin_pad] planes
-            cout, cin, k = w.shape
-            cpad = _pad_to(cin, 64)
-            wp = torch.zeros(cout, k, cpad, device=dev)
-            wp[:, :, :cin] = w.permute(0, 2, 1)
-            return Planes.from_f32(wp.reshape(cout, k * cpad), True)
 
         if self.in_rate != 16000:
             kern, width, o, n = resample_kernel(self.in_rate, 16000)
@@ -188,13 +151,14 @@ class SSLFrontEnd(nn.Module):
         nconv = len(c["conv_dim"])
         W["conv0_w"] = f32("feature_extractor.conv_layers.0.conv.weight").reshape(c["conv_dim"][0], -1).contiguous()
         W["gn_w"], W["gn_b"] = f32("feature_extractor.conv_layers.0.layer_norm.weight"), f32("feature_extractor.conv_layers.0.layer_norm.bias")
-        W["convs"] = [conv_w(sd[f"feature_extractor.conv_layers.{i}.conv.weight"]) for i in range(1, nconv)]
+        W["convs"] = [ops.conv_planes(sd[f"feature_extractor.conv_layers.{i}.conv.weight"]) for i in range(1, nconv)]
         if w2v:
             W["conv_b"] = [f32(f"feature_extractor.conv_layers.{i}.conv.bias") for i in range(nconv)]
             W["conv_ln"] = [(f32(f"feature_extractor.conv_layers.{i}.layer_norm.weight"), f32(f"feature_extractor.conv_layers.{i}.layer_norm.bias"))
                             for i in range(nconv)]
         W["fp_ln_w"], W["fp_ln_b"] = f32("feature_projection.layer_norm.weight"), f32("feature_projection.layer_norm.bias")
-        W["fp_w"], W["fp_b"] = Planes.from_f32(sd["feature_projection.projection.weight"], True), f32("feature_projection.projection.bias")
+        W["fp_w"] = ops.pad_k_planes(sd["feature_projection.projection.weight"], _pad_to(c["conv_dim"][-1], 64))
+        W["fp_b"] = f32("feature_projection.projection.bias")
         # weight-normed grouped positional conv: w = g * v / ||v|| (norm over (out, in) per tap); per group [Cg, k * 64] planes
         g0, v = sd["encoder.pos_conv_embed.conv.parametrizations.weight.original0"], sd["encoder.pos_conv_embed.conv.parametrizations.weight.original1"]
         w = v * (g0 / v.pow(2).sum((0, 1), keepdim=True).sqrt())
@@ -230,30 +194,20 @@ class SSLFrontEnd(nn.Module):
     def _rel_table(self, T):
         """WavLMAttention.compute_bias / _relative_positions_bucket as a per-distance table [heads, 2T - 1]
         (entry (h, r + T - 1) = rel_attn_embed[bucket(r)][h], r = key - query); built once per length (load-time glue)."""
-        key = ("rel", T)
-        r = self._ws.get(key)
-        if r is None:
-            c = self.cfg
-            rel = torch.arange(-(T - 1), T)
-            nb = c["num_buckets"] // 2
-            bucket = (rel > 0).long() * nb
-            a = rel.abs()
-            max_exact = nb // 2
-            large = torch.log(a.float() / max_exact) / math.log(c["max_distance"] / max_exact) * (nb - max_exact)
-            large = torch.min((max_exact + large).long(), torch.full_like(a, nb - 1))
-            bucket = bucket + torch.where(a < max_exact, a, large)
-            emb = self._prepare()["rel_embed"]                       # [num_buckets, heads]
-            r = emb[bucket.to(emb.device)].t().contiguous()           # [heads, 2T - 1]
-            self._ws[key] = r
-        return r
+        c = self.cfg
+        rel = torch.arange(-(T - 1), T)
+        nb = c["num_buckets"] // 2
+        bucket = (rel > 0).long() * nb
+        a = rel.abs()
+        max_exact = nb // 2
+        large = torch.log(a.float() / max_exact) / math.log(c["max_distance"] / max_exact) * (nb - max_exact)
+        large = torch.min((max_exact + large).long(), torch.full_like(a, nb - 1))
+        bucket = bucket + torch.where(a < max_exact, a, large)
+        emb = self._prepare()["rel_embed"]                       # [num_buckets, heads]
+        return emb[bucket.to(emb.device)].t().contiguous()        # [heads, 2T - 1]
 
     def _identity_rope(self, T, D):
-        key = ("rope1", T, D)
-        r = self._ws.get(key)
-        if r is None:
-            r = (torch.ones(T, D, device=self._dev()), torch.zeros(T, D, device=self._dev()))
-            self._ws[key] = r
-        return r
+        return self._cached(("rope1", T, D), lambda: (torch.ones(T, D, device=self._dev()), torch.zeros(T, D, device=self._dev())))
 
     def _embed(self, feats: torch.Tensor, B: int, Tf: int, taps: Optional[dict] = None) -> torch.Tensor:
         """conv features [B * Tf, Cf] -> feature projection (LayerNorm -> Linear) -> x + GELU(positional conv(x)) [B * Tf, H]"""
@@ -267,14 +221,9 @@ class SSLFrontEnd(nn.Module):
         cfp = _pad_to(Cf, 64)
         pn = self._planes("fp_in", (M, cfp))
         ops.layernorm(feats, W["fp_ln_w"], W["fp_ln_b"], B, Tf, Cf, eps=c["eps"], out=pn, ld=cfp, rows_per_batch=Tf, row_off=0)
-        wfp = W.get("fp_w_pad")
-        if wfp is None:
-            w = torch.zeros(H, cfp, device=self._dev())
-            w[:, :Cf] = self.feature_projection.projection.weight.detach().float()
-            wfp = W["fp_w_pad"] = Planes.from_f32(w, True)
         xh = self._buf("x", (M, H))
         # projected features also go, group-padded, into the positional conv's zero-padded buffer
-        ops.gemm(pn, wfp, H, a_batch=1, a_rows_per_batch=M, a_ld=cfp, m_per_batch=M, bias=W["fp_b"], out_f32=rowmap(xh, H, M, 0))
+        ops.gemm(pn, W["fp_w"], H, a_batch=1, a_rows_per_batch=M, a_ld=cfp, m_per_batch=M, bias=W["fp_b"], out_f32=rowmap(xh, H, M, 0))
         # ---- positional conv embedding: x + GELU(conv_k128_g16(x))  (HubertPositionalConvEmbedding + SamePad)
         G, K = c["pos_groups"], c["pos_k"]
         cg = H // G
@@ -372,7 +321,7 @@ class SSLFrontEnd(nn.Module):
         umma = (not wavlm) and hd in (64, 128) and os.environ.get("QB_ATTENTION", "umma") != "legacy"
         att_ws = self._buf("att5_ws", (ops.attention_umma_workspace_bytes(B, Tf, heads, hd, True),), torch.uint8) if umma else None
         if wavlm:
-            rel_table = self._rel_table(Tf)
+            rel_table = self._cached(("rel", Tf), lambda: self._rel_table(Tf))
             gate = self._buf("gate", (B, heads, Tf))
         for li, L in enumerate(W["layers"]):
             ops.gemm(xp, L["wqkv"], 3 * H, a_batch=1, a_rows_per_batch=M, a_ld=H, m_per_batch=M, bias=L["bqkv"],
