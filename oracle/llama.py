@@ -209,7 +209,9 @@ def sample_filter(logits, temperature=0.8, top_k=50, top_p=0.95):
         kth = torch.topk(logits, top_k)[0][..., -1, None]
         logits[logits < kth] = float("-inf")
     if top_p < 1.0:
-        sorted_logits, sorted_indices = torch.sort(logits, descending=True)
+        # stable: when the cut falls inside a run of equal logits, the lower token ids are the ones kept, the order the
+        # device sampler defines (an unstable sort keeps an arbitrary subset of the run)
+        sorted_logits, sorted_indices = torch.sort(logits, descending=True, stable=True)
         cum = torch.cumsum(F.softmax(sorted_logits, dim=-1), dim=-1)
         rem = cum > top_p
         rem[..., 1:] = rem[..., :-1].clone()

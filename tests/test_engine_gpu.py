@@ -167,16 +167,19 @@ def test_lm_c_abi_against_oracle(lib):
     prefix = llama._prefix(sd, cfg, "se", None, mix)                     # [B, P, 512] (host-side embedding glue)
     ref_h, _ = llama.llm_forward(sd, cfg, prefix)
     _check(lib, lib.qb_kv_alloc(lm, B, 128, C.byref(kv)))
-    pre_d = prefix.cuda().contiguous()
-    hid = torch.empty(B, P, 512, device="cuda")
-    _check(lib, lib.qb_lm_prefill(lm, pre_d.data_ptr(), B, P, kv, hid.data_ptr(), stream))
+    # the prefix in two prefills on the same cache: the second continues it (lm_qkv_prep + lm_flash_attn at pos0 = 25)
+    P1 = 25
+    pre1, pre2 = prefix[:, :P1].cuda().contiguous(), prefix[:, P1:].cuda().contiguous()
+    hid1, hid2 = torch.empty(B, P1, 512, device="cuda"), torch.empty(B, P - P1, 512, device="cuda")
+    _check(lib, lib.qb_lm_prefill(lm, pre1.data_ptr(), B, P1, kv, hid1.data_ptr(), stream))
+    _check(lib, lib.qb_lm_prefill(lm, pre2.data_ptr(), B, P - P1, kv, hid2.data_ptr(), stream))
     goff, soff = 3, 3 + b["global_size"]
     gids = torch.empty(B, 33, dtype=torch.int64, device="cuda")
     sids = torch.empty(B, T, dtype=torch.int64, device="cuda")
     _check(lib, lib.qb_lm_decode_greedy(lm, kv, B, 0, 33, goff, goff + b["global_size"], gids.data_ptr(), stream))
     _check(lib, lib.qb_lm_decode_greedy(lm, kv, B, 1, T, soff, soff + b["semantic_size"], sids.data_ptr(), stream))
     torch.cuda.synchronize()
-    e_pre = rel(hid, ref_h)
+    e_pre = max(rel(hid1, ref_h[:, :P1]), rel(hid2, ref_h[:, P1:]))
     og, os_, margins = llama.sft_generate(sd, cfg, "se", None, mix, T, return_margins=True)
     got = torch.cat([gids.cpu() - goff, sids.cpu() - soff], 1)
     want = torch.cat([og, torch.zeros(B, 1, dtype=torch.long), os_], 1)

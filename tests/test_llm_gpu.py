@@ -120,6 +120,55 @@ def test_lm_decode_step_vs_oracle(lib, B):
     assert e_tc < TOL
 
 
+def test_lm_prefill_continuation_vs_oracle(lib):
+    """A prefill that continues a filled cache (lm_qkv_prep + lm_flash_attn at pos0 > 0), then cached decodes, against the oracle's
+    one-shot forward over all positions"""
+    from oracle import llama
+    cfg = llama.LM_FULL
+    m, sd = build(cfg, 5, 2.0)
+    g = torch.Generator().manual_seed(17)
+    B = 3
+    x = torch.randn(B, 74, 512, generator=g)
+    ref, _ = llama.llm_forward(sd, cfg, x)
+    out = m.llm_forward(x[:, :40].cuda(), use_cache=True)
+    cache = out.past_key_values
+    hs = [out.last_hidden_state, m.llm_forward(x[:, 40:70].cuda(), past_key_values=cache, use_cache=True).last_hidden_state]
+    assert cache.length == 70
+    for i in range(70, 74):
+        hs.append(m.llm_forward(x[:, i:i + 1].cuda(), past_key_values=cache, use_cache=True).last_hidden_state)
+    torch.cuda.synchronize()
+    got = torch.cat(hs, 1)
+    e_first, e_cont, e_dec = rel(got[:, :40], ref[:, :40]), rel(got[:, 40:70], ref[:, 40:70]), rel(got[:, 70:], ref[:, 70:])
+    print(f"prefill rel {e_first:.2e}, continuation prefill rel {e_cont:.2e}, decode after it rel {e_dec:.2e}")
+    assert e_first < TOL and e_cont < TOL and e_dec < TOL
+
+
+@pytest.mark.parametrize("ssize", [100, 128])
+def test_lm_generate_ranges_not_multiple_of_16(lib, ssize):
+    """Token ranges whose width is not a multiple of 16 (global 40; semantic 100 or 128): greedy tokens match the oracle under the
+    margin rule, and greedy and sampled tokens stay inside their ranges (the head's last CTA owns fewer than 16 columns)"""
+    from oracle import llama
+    cfg = llama.lm_small(gsize=40, ssize=ssize)
+    m, sd = build(cfg, 9, 2.0)
+    g = torch.Generator().manual_seed(ssize)
+    B, T = 5, 20
+    mix = torch.randn(B, T, cfg["feats_dim"], generator=g)
+    og, os_, margins = llama.sft_generate(sd, cfg, "se", None, mix, T, return_margins=True)
+    for graph in (False, True):
+        gg, ss = m.generate("se", None, None, mix.cuda(), mix.cuda(), do_sample=False, use_cuda_graph=graph)
+        torch.cuda.synchronize()
+        gg, ss = gg.cpu(), ss.cpu()
+        assert int(gg.min()) >= 0 and int(gg.max()) < 40 and int(ss.min()) >= 0 and int(ss.max()) < ssize
+        margins[:, 32] = 1.0
+        zero = torch.zeros(B, 1, dtype=torch.long)
+        compare_tokens(f"gsize 40 ssize {ssize} graph={graph}", torch.cat([gg, zero, ss], 1), torch.cat([og, zero, os_], 1), margins)
+    for seed in (1, 2, 3):
+        gs_, ss_ = m.generate("se", None, None, mix.cuda(), mix.cuda(), do_sample=True, seed=seed, top_k=1024, top_p=1.0,
+                              temperature=1.0)
+        torch.cuda.synchronize()
+        assert int(gs_.min()) >= 0 and int(gs_.max()) < 40 and int(ss_.min()) >= 0 and int(ss_.max()) < ssize
+
+
 def test_lm_sampled_generate_vs_oracle(lib):
     """do_sample=True with the reference's default arguments (temperature 0.8, top_k 50, top_p 0.95; llm_sft.py:93-107).
     The device sampler's tokens are replayed on the oracle along the device's own token path: at every step the token must

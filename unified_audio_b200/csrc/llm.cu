@@ -376,7 +376,7 @@ __global__ void lm_loss_reduce_kernel(const float* __restrict__ row_loss, const 
 // draw.  torch.multinomial's generator cannot be reproduced bit for bit, so the draw is defined here as the inverse CDF
 // over the kept tokens in descending-logit order (ties: ascending id) at u = Philox4x32-10(key = seed, counter =
 // {step, row, call, 0}).x * 2^-32 truncated to 24 bits: same distribution, replayable from (seed, call, step, row).
-constexpr int LS_MAX = 1024;             // survivors kept (top_k + ties); top_k <= LS_MAX enforced by the host
+constexpr int LS_MAX = 1024;             // survivors above the threshold kept (< top_k); top_k <= LS_MAX enforced by the host
 __device__ __forceinline__ uint32_t ls_key(float v) {     // monotone float -> uint32 (NaN sorts lowest)
   if (v != v) return 0u;
   const uint32_t u = __float_as_uint(v);
@@ -411,7 +411,7 @@ lm_sample_embed_kernel(const float* __restrict__ logits, int ld, const int* __re
   int* sidx = (int*)(skey + LS_MAX);              // [LS_MAX] survivors: column
   __shared__ int hist[256];
   __shared__ uint32_t sh_prefix;
-  __shared__ int sh_need, sh_cnt, sh_tok;
+  __shared__ int sh_need, sh_eq, sh_cnt, sh_tok, sh_rank;
   for (int i = tid; i < n; i += 256) keys[i] = ls_key(logits[(size_t)b * ld + i]);
   if (tid == 0) { sh_prefix = 0u; sh_need = top_k < n ? top_k : n; sh_cnt = 0; }
   __syncthreads();
@@ -433,20 +433,24 @@ lm_sample_embed_kernel(const float* __restrict__ logits, int ld, const int* __re
       }
       sh_need = need;
       sh_prefix = prefix | ((uint32_t)bin << shift);
+      if (shift == 0) sh_eq = hist[bin];          // keys equal to the threshold
     }
     __syncthreads();
   }
   const uint32_t thr = sh_prefix;
-  // ---- survivors (key >= threshold: ties at the k-th value stay, llm.py:263-264), then bitonic sort descending
+  // ---- survivors: every key >= threshold (ties at the k-th value stay, llm.py:263-264).  Those strictly above it (at most
+  // top_k - 1) are collected and bitonic-sorted descending; the n_eq tied ones, however many, share one value and follow them
+  // in ascending column order, so they are counted rather than stored.
+  const int n_gt = (top_k < n ? top_k : n) - sh_need, n_eq = sh_eq;
   for (int i = tid; i < n; i += 256) {
     const uint32_t k = keys[i];
-    if (k >= thr) {
+    if (k > thr) {
       const int s = atomicAdd(&sh_cnt, 1);
-      if (s < LS_MAX) { skey[s] = k; sidx[s] = i; }
+      skey[s] = k; sidx[s] = i;
     }
   }
   __syncthreads();
-  const int cnt = sh_cnt < LS_MAX ? sh_cnt : LS_MAX;
+  const int cnt = n_gt;
   int P = 1;
   while (P < cnt) P <<= 1;
   for (int i = cnt + tid; i < P; i += 256) { skey[i] = 0u; sidx[i] = 0x7fffffff; }
@@ -465,40 +469,78 @@ lm_sample_embed_kernel(const float* __restrict__ logits, int ld, const int* __re
       }
       __syncthreads();
     }
-  // ---- top-p cut, temperature, inverse-CDF draw (one thread: <= LS_MAX sequential fp32 adds, like torch.cumsum on a row)
+  // ---- top-p cut, temperature, inverse-CDF draw over the survivors in order: the cnt sorted ones one by one (sequential fp32 adds,
+  // like torch.cumsum on a row), then the tied tail in closed form (j tied tokens add j * their common term)
   if (tid == 0) {
-    const float m = ls_val(skey[0]);
-    int nk = cnt;
+    const float v = ls_val(thr), m = cnt > 0 ? ls_val(skey[0]) : v;
+    const int n_all = cnt + n_eq;
+    int nk = n_all;
     if (top_p < 1.0f) {
+      const float q = expf(v - m);
       float Z = 0.f;
       for (int i = 0; i < cnt; ++i) Z += expf(ls_val(skey[i]) - m);
+      Z += (float)n_eq * q;
       float cum = 0.f;
-      nk = 1;
-      for (int i = 1; i < cnt; ++i) {
+      nk = 0;
+      for (int i = 1; i <= cnt; ++i) {               // a token goes once the mass before it exceeds top_p
         cum += expf(ls_val(skey[i - 1]) - m) / Z;
-        if (cum > top_p) break;
-        nk = i + 1;
+        if (cum > top_p) { nk = i; break; }
+      }
+      if (nk == 0) {                                 // the cut falls in the tied tail: keep the first j of it, j >= 1
+        const float qz = q / Z;
+        int j = qz > 0.f ? (int)fminf(fmaxf(floorf((top_p - cum) / qz), 0.f), (float)n_eq) : n_eq;
+        while (j > 1 && cum + (float)(j - 1) * qz > top_p) --j;
+        while (j < n_eq && !(cum + (float)j * qz > top_p)) ++j;
+        nk = cnt + (j > 1 ? j : 1);
       }
     }
+    const int k_gt = nk < cnt ? nk : cnt, k_eq = nk - k_gt;
+    const float et = expf((v - m) * inv_temp);
     float S = 0.f;
-    for (int i = 0; i < nk; ++i) S += expf((ls_val(skey[i]) - m) * inv_temp);
+    for (int i = 0; i < k_gt; ++i) S += expf((ls_val(skey[i]) - m) * inv_temp);
+    S += (float)k_eq * et;
     const uint32_t r = philox_u32(seed[0], seed[1], (uint32_t)*slot, (uint32_t)b, seed[2], 0u);
     const float u = (float)(r >> 8) * (1.0f / 16777216.0f);
     const float target = u * S;
     float run = 0.f;
-    int pick = nk - 1;
-    for (int i = 0; i < nk; ++i) {
+    int pick = -1;
+    for (int i = 0; i < k_gt; ++i) {
       run += expf((ls_val(skey[i]) - m) * inv_temp);
       if (run > target) { pick = i; break; }
     }
-    int tok = lo + sidx[pick];
-    if (sidx[pick] == 0x7fffffff || m != m) tok = lo;          // all-NaN row: first column of the range (see arg-max kernel)
-    sh_tok = tok;
-    out_ids[(size_t)b * out_stride + *slot] = (int64_t)tok;
-    if (dbg) { dbg[b * 4 + 0] = u; dbg[b * 4 + 1] = (float)cnt; dbg[b * 4 + 2] = (float)nk; dbg[b * 4 + 3] = S; }
+    sh_rank = -1;
+    if (pick >= 0) {
+      sh_tok = lo + sidx[pick];
+    } else if (k_eq > 0) {                           // j-th tied token (0-based): the first j with run + (j + 1) et > target
+      int j = et > 0.f ? (int)fminf(fmaxf(floorf((target - run) / et), 0.f), (float)(k_eq - 1)) : k_eq - 1;
+      while (j > 0 && run + (float)j * et > target) --j;
+      while (j < k_eq - 1 && !(run + (float)(j + 1) * et > target)) ++j;
+      sh_rank = j;
+    } else {
+      sh_tok = lo + sidx[k_gt - 1];
+    }
+    if (m != m) { sh_tok = lo; sh_rank = -1; }      // all-NaN row: first column of the range (see arg-max kernel)
+    if (dbg) { dbg[b * 4 + 0] = u; dbg[b * 4 + 1] = (float)n_all; dbg[b * 4 + 2] = (float)nk; dbg[b * 4 + 3] = S; }
   }
   __syncthreads();
+  if (sh_rank >= 0) {                               // column of the rank-th tied key: block-wide prefix count over the row
+    int* cnt_of = hist;
+    const int per = (n + 255) / 256, i0 = tid * per, i1 = min(n, i0 + per);
+    int c = 0;
+    for (int i = i0; i < i1; ++i) c += keys[i] == thr;
+    cnt_of[tid] = c;
+    __syncthreads();
+    if (tid == 0)
+      for (int i = 0, s = 0; i < 256; ++i) { const int ci = cnt_of[i]; cnt_of[i] = s; s += ci; }
+    __syncthreads();
+    int rank = sh_rank - cnt_of[tid];
+    if (rank >= 0 && rank < c)
+      for (int i = i0; i < i1; ++i)
+        if (keys[i] == thr && rank-- == 0) { sh_tok = lo + i; break; }
+    __syncthreads();
+  }
   const int tok = sh_tok;
+  if (tid == 0) out_ids[(size_t)b * out_stride + *slot] = (int64_t)tok;
   for (int k = tid; k < Hd; k += 256) x_next[(size_t)b * Hd + k] = emb[(size_t)tok * Hd + k];
   __syncthreads();
   if (tid == 0) {
@@ -573,6 +615,7 @@ lm_skinny_kernel(const SkParams p) {
   const uint4* wrow[NT];
   bool cta_active = true;
   int row0 = 0, dd0 = 0, hh = 0, sec = 0;
+  int row_end = 1 << 30;        // HEAD: rows >= row0 + row_end lie past the range: no load, no candidate, no logit
   if (MODE == SK_QKV) {
     dd0 = (blockIdx.x & 3) * 8; hh = (blockIdx.x >> 2) % p.H; sec = blockIdx.x / (4 * p.H);
     row0 = sec * p.H * 64 + hh * 64 + dd0;
@@ -589,6 +632,7 @@ lm_skinny_kernel(const SkParams p) {
     const int lo = p.range[0], ncol = p.range[1] - lo;      // host-written before the graph launch, not by a kernel
     cta_active = (int)blockIdx.x * 16 < ncol;
     row0 = lo + (cta_active ? blockIdx.x * 16 : 0);
+    row_end = p.range[1] - row0;       // the last CTA of a range whose width is not a multiple of 16 owns fewer rows
     wrow[0] = p.W + (size_t)(row0 + g) * K4;
     if (NT > 1) wrow[NT - 1] = p.W + (size_t)(row0 + 8 + g) * K4;
   }
@@ -599,7 +643,8 @@ lm_skinny_kernel(const SkParams p) {
     const int step = warp * SPW + s;
     const bool ok = step < steps_total && cta_active;
 #pragma unroll
-    for (int nt = 0; nt < NT; ++nt) wv[nt][s] = ok ? __ldg(wrow[nt] + step * 4 + t) : make_uint4(0u, 0u, 0u, 0u);
+    for (int nt = 0; nt < NT; ++nt)
+      wv[nt][s] = ok && nt * 8 + g < row_end ? __ldg(wrow[nt] + step * 4 + t) : make_uint4(0u, 0u, 0u, 0u);
   }
   pdl_wait();
   float acc[2][NT][4];
@@ -687,13 +732,13 @@ lm_skinny_kernel(const SkParams p) {
   if (MODE == SK_HEAD) {
     float bv = -INFINITY;
     int bi = 0x7fffffff;
-    if (cta_active && b < p.B) {
+    if (cta_active && b < p.B && c < row_end) {
       bv = v0; bi = row0 + c;
-      if (v1 > bv) { bv = v1; bi = row0 + 8 + c; }
+      if (8 + c < row_end && v1 > bv) { bv = v1; bi = row0 + 8 + c; }
       if (p.logits) {
         float* lg = p.logits + (size_t)b * p.logits_ld + (row0 - p.range[0]);
         lg[c] = v0;
-        lg[8 + c] = v1;
+        if (8 + c < row_end) lg[8 + c] = v1;
       }
     }
 #pragma unroll

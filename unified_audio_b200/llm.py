@@ -391,7 +391,7 @@ class LLM_SFT(_Face):
         Lmax = -(-(P + n_steps) // 64) * 64
         self._ensure_rope(P + n_steps)
         W = self._w
-        max_cols = max(self.global_size, self.semantic_size)
+        max_cols = _pad_to(max(self.global_size, self.semantic_size), 16)     # the head runs 16 columns per CTA
         samp_key = None if sampling is None else (sampling["temperature"], sampling["top_k"], sampling["top_p"])
         # Decode state (KV cache, counters, output ids) and the captured graphs are kept per shape: capturing and
         # instantiating ~560 kernel nodes costs the host 10-50 ms, as much as the whole generation takes on the device.
