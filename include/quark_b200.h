@@ -238,6 +238,14 @@ int qb_rvq_encode(const float* x, const float* codebooks, const qb_half* cb_hi, 
  * summed q = 0..nq-1 in fp32 (codec.py:94-95). */
 int qb_rvq_decode(const int64_t* idx, const float* codebooks, int64_t M, int32_t D, int32_t K, int32_t nq,
                   float* out, int64_t out_ld, int64_t col_off, void* stream);
+/* Factorised VQ tokenize: BiCodec's semantic quantiser, FactorizedVectorQuantize.tokenize / in_project / decode_latents
+ * (QuarkAudio-UniSE/model/bicodec/modules/vq/factorized_vector_quantize.py:59-61,148-152,169-187).  Per row of z [M, D_in] fp32:
+ * z_e = W_in z + b_in (W_in [cdim, D_in] with the weight norm folded, fp64 sums), e = z_e / max(|z_e|, 1e-12) and
+ * idx = argmax_j (2 e.c_j - |c_j|^2) over codebook_n [K, cdim] fp64 = F.normalize(codebook) - the reference's argmax of -dist
+ * without the row constant |e|^2 - all in fp64, lowest index on exact ties.  idx [M] int64; z_e [M, cdim] fp32 (the in_project
+ * output, before normalisation) if not NULL.  1 <= cdim <= 16. */
+int qb_fvq_tokenize(const float* z, int64_t M, int32_t D_in, const float* w_in, const float* b_in, const double* codebook_n,
+                    int32_t K, int32_t cdim, int64_t* idx, float* z_e, void* stream);
 
 /* ---------------------------------------------------------------- UniSE AR-LM (decoder-only Llama-style LM)
  * Reference: QuarkAudio-UniSE/model/llm/llm.py:150-228 (llm_forward over HF Llama decoder layers),

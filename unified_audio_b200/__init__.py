@@ -6,12 +6,14 @@ Public surface mirrors the reference (alibaba/unified-audio):
   LLM_SFT          <- QuarkAudio-UniSE/model/llm/llm_sft.py:13 (llm_forward / forward / generate)
   CodecH1          <- QuarkAudio-HCodec/HCodec-1.0/vq/codec.py:21   (encode / decode)
   CodecH15         <- QuarkAudio-HCodec/HCodec-1.5/vq/codec_adaptive.py:32 (adaptive frame rate: encode / decode with length-packed codes)
-  BiCodec          <- QuarkAudio-UniSE/model/bicodec/bicodec.py:182 (detokenize)
-  SSLFrontEnd      <- HuBERT-base / WavLM-base-plus feature extraction as HCodecTokenizer.extract_ssl_features
-                      (HCodec-2.0/audio_tokenizer.py:47-61) and Model.extract_semantic_features (U/model/model.py:38-51) drive them
+  BiCodec          <- QuarkAudio-UniSE/model/bicodec/bicodec.py:151-199 (detokenize; get_global_tokens, get_semantic_tokens and
+                      tokenize with global_tokens=True / semantic_tokens=True)
+  SSLFrontEnd      <- HuBERT-base / WavLM-base-plus / wav2vec2-XLSR-53 feature extraction as HCodecTokenizer.extract_ssl_features
+                      (HCodec-2.0/audio_tokenizer.py:47-61), Model.extract_semantic_features (U/model/model.py:38-51) and
+                      BiCodecTokenizer.extract_wav2vec2_features (U/model/bicodec/audio_tokenizer.py:74-90) drive them
   HCodecTokenizer  <- QuarkAudio-HCodec/HCodec-2.0/audio_tokenizer.py:21-79 (pad_wav / tokenize / detokenize)
   unise.Model      <- QuarkAudio-UniSE/model/model.py:20-286 (extract_semantic_features / test_step: 'se', 'tse', 'ss') with
-                      unise.BiCodecTokenizer <- model/bicodec/audio_tokenizer.py:30-125 (detokenize)
+                      unise.BiCodecTokenizer <- model/bicodec/audio_tokenizer.py:30-125 (get_ref_clip / tokenize / detokenize)
 Kernels live in csrc/ behind the C ABI of include/quark_b200.h (lib/libquark_b200.so).
 """
 __version__ = "0.1.0"

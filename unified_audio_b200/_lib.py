@@ -93,6 +93,7 @@ SIGNATURES = {
     "qb_rvq_workspace_bytes": (C.c_int64, [_i64, _i32, _i32]),
     "qb_rvq_encode": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _f32, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "qb_rvq_decode": (C.c_int, [_vp, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _vp]),
+    "qb_fvq_tokenize": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "qb_lm_qkv_prep": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
     "qb_lm_flash_attn": (C.c_int, [_vp, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _vp, _vp, _vp]),
     "qb_lm_pack_weight": (C.c_int, [_vp, _i64, _i64, _vp, _vp]),

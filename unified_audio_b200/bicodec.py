@@ -3,19 +3,28 @@
 Mirrors QuarkAudio-UniSE/model/bicodec/bicodec.py:182-199:
     BiCodec(config).detokenize(semantic_tokens [B,T] int64, global_tokens [B,1,32] int64) -> wav [B,1,T*320] fp32
 state_dict keys are the reference's (`quantizer.*`, `speaker_encoder.*`, `prenet.*`, `decoder.*`, old-style weight-norm
-`weight_g / weight_v` pairs); keys of the tokenize side (`encoder.*`, `postnet.*`, ECAPA / perceiver, `mel_transformer.*`,
-`quantizer.in_project.*`) are accepted at load and ignored.  The reference ships no `config.yaml` (it comes with the
+`weight_g / weight_v` pairs); by default the keys of the tokenize side (`encoder.*`, `postnet.*`, ECAPA / perceiver,
+`mel_transformer.*`, `quantizer.in_project.*`) are accepted at load and ignored.  The reference ships no `config.yaml` (it comes with the
 Spark-TTS-0.5B checkpoint, U/README.md:57-74); BICODEC_CONFIG and MEL_PARAMS restate that published configuration.
 
 With `global_tokens=True` the module also holds the global-token path, bicodec.py:174-178:
     BiCodec.get_global_tokens({"ref_wav": [B, L]}) -> int32 [B, 1, token_num]
 and a strict load requires its keys (`speaker_encoder.speaker_encoder.{layer1..layer4,conv}.*` with BatchNorm running statistics,
-`speaker_encoder.perceiver_sampler.*`, `speaker_encoder.quantizer.project_in.*`).  Still ignored: the semantic tokenize side, the
-x-vector branch the reference computes and discards (`speaker_encoder.speaker_encoder.{pool,bn,linear}.*`), BatchNorm's
-`num_batches_tracked` and `mel_transformer.*` (window and filter bank are rebuilt from MEL_PARAMS).  Mapping: MelSpectrogram =
+`speaker_encoder.perceiver_sampler.*`, `speaker_encoder.quantizer.project_in.*`).  Still ignored: the x-vector branch the reference
+computes and discards (`speaker_encoder.speaker_encoder.{pool,bn,linear}.*`), BatchNorm's `num_batches_tracked` and
+`mel_transformer.*` (window and filter bank are rebuilt from MEL_PARAMS).  Mapping: MelSpectrogram =
 centred reflect framing + two-stage DFT GEMMs + |X| + the slaney filter bank as a GEMM; Conv1dReluBn = one GEMM with a ReLU
 epilogue and the eval BatchNorm folded into gamma + a broadcast residual row; squeeze-excitation, the perceiver's cross attention
 RMSNorm + FSQ and the feed-forward's GEGLU are kernels of csrc/speaker.cu.  Every contraction is a 3-term split.
+
+With `semantic_tokens=True` the module also holds the semantic-token path, bicodec.py:167-172:
+    BiCodec.get_semantic_tokens({"feat": [B, T, input_channels]}) -> int64 [B, T]
+and a strict load requires `encoder.*` (feat_encoder.py:29-90) and `quantizer.in_project.*`.  The Encoder's three Vocos backbones
+run on the same GEMM / ConvNeXt kernels as the prenet, SamplingBlock(1)'s 3 x folded into the downsample backbones' embed convs, and
+`project` is one GEMM; `qb_fvq_tokenize` (csrc/rvq.cu) does in_project, the normalisation and the codebook arg-max in fp64.  Every
+encoder contraction is a 3-term split whatever `precision` says (the tokens are discrete; `precision` governs detokenize).  With
+both flags, `tokenize(batch)` returns (semantic_tokens, global_tokens).  `postnet.*` (training only) and `quantizer.cluster_size`
+are always ignored.  ENCODER_PARAMS restates the published encoder section for a config without an "encoder" entry.
 
 How the path maps onto the library (every arithmetic op is a libquark_b200 kernel; channel-last activations):
   * FactorizedVectorQuantize.detokenize (modules/vq/factorized_vector_quantize.py:154-167) and the residual-FSQ de-quantiser
@@ -51,6 +60,10 @@ BICODEC_CONFIG = dict(
 # BiCodec's `mel_params` (bicodec.py:201-221): the published Spark-TTS-0.5B values, restated like BICODEC_CONFIG and likewise not
 # verifiable offline.  A config without a "mel_params" entry uses these.
 MEL_PARAMS = dict(sample_rate=16000, n_fft=1024, win_length=640, hop_length=320, mel_fmin=10, mel_fmax=None, num_mels=128)
+# BiCodec's `encoder` section (the feature Encoder, feat_encoder.py:29-90): the published Spark-TTS-0.5B values, restated like
+# MEL_PARAMS and likewise not verifiable offline.  A config without an "encoder" entry uses these.
+ENCODER_PARAMS = dict(input_channels=1024, vocos_dim=384, vocos_intermediate_dim=2048, vocos_num_layers=12, out_channels=1024,
+                      sample_ratios=[1, 1])
 ECAPA_C, ECAPA_SCALE, ECAPA_OUT, HEADS = 512, 8, 1536, 8   # ECAPA_TDNN_GLOB_c512, dim_context = 512 * 3, 8 heads x 64 (fixed)
 
 # 3-term split (True) or single-pass fp16 (False) per GEMM group; "accurate" is the default until the error budget of the
@@ -62,15 +75,40 @@ PRECISION = {
 }
 
 
+def _wn_spec(out, prefix, shape, n_out=None):
+    """old-style weight norm (layers.py:24-29): bias, weight_g [out, 1, ...], weight_v"""
+    out[prefix + "bias"] = (shape[0] if n_out is None else n_out,)
+    out[prefix + "weight_g"] = (shape[0],) + (1,) * (len(shape) - 1)
+    out[prefix + "weight_v"] = tuple(shape)
+
+
+def _backbone_spec(out, prefix, cin, dim, inter, layers, cond):
+    """VocosBackbone(input_channels=cin, dim, intermediate_dim=inter, num_layers=layers, condition_dim=cond) (vocos.py:273-335)"""
+    def norm(pp):
+        if cond:
+            out[pp + "scale.weight"] = (dim, cond); out[pp + "scale.bias"] = (dim,)
+            out[pp + "shift.weight"] = (dim, cond); out[pp + "shift.bias"] = (dim,)
+        else:
+            out[pp + "weight"] = (dim,); out[pp + "bias"] = (dim,)
+
+    out[prefix + "embed.weight"] = (dim, cin, 7)
+    out[prefix + "embed.bias"] = (dim,)
+    norm(prefix + "norm.")
+    for i in range(layers):
+        b = f"{prefix}convnext.{i}."
+        out[b + "gamma"] = (dim,)
+        out[b + "dwconv.weight"] = (dim, 1, 7); out[b + "dwconv.bias"] = (dim,)
+        norm(b + "norm.")
+        out[b + "pwconv1.weight"] = (inter, dim); out[b + "pwconv1.bias"] = (inter,)
+        out[b + "pwconv2.weight"] = (dim, inter); out[b + "pwconv2.bias"] = (dim,)
+    out[prefix + "final_layer_norm.weight"] = (dim,); out[prefix + "final_layer_norm.bias"] = (dim,)
+
+
 def bicodec_spec(c) -> Dict[str, tuple]:
     """Reference state-dict keys -> shapes of the detokenize path."""
     out: Dict[str, tuple] = {}
     q, s, p, d = c["quantizer"], c["speaker"], c["prenet"], c["decoder"]
-
-    def wn(prefix, shape, n_out=None):
-        out[prefix + "bias"] = (shape[0] if n_out is None else n_out,)
-        out[prefix + "weight_g"] = (shape[0],) + (1,) * (len(shape) - 1)
-        out[prefix + "weight_v"] = tuple(shape)
+    wn = lambda prefix, shape, n_out=None: _wn_spec(out, prefix, shape, n_out)
 
     out["quantizer.codebook.weight"] = (q["codebook_size"], q["codebook_dim"])
     wn("quantizer.out_project.", (q["input_dim"], q["codebook_dim"], 1))
@@ -79,33 +117,12 @@ def bicodec_spec(c) -> Dict[str, tuple]:
     out["speaker_encoder.project.weight"] = (s["out_dim"], s["latent_dim"] * s["token_num"])
     out["speaker_encoder.project.bias"] = (s["out_dim"],)
     dim, inter = p["vocos_dim"], p["vocos_intermediate_dim"]
-
-    def norm(pp, cond):
-        if cond:
-            out[pp + "scale.weight"] = (dim, cond); out[pp + "scale.bias"] = (dim,)
-            out[pp + "shift.weight"] = (dim, cond); out[pp + "shift.bias"] = (dim,)
-        else:
-            out[pp + "weight"] = (dim,); out[pp + "bias"] = (dim,)
-
-    def backbone(prefix, layers, cond):
-        out[prefix + "embed.weight"] = (dim, dim, 7)
-        out[prefix + "embed.bias"] = (dim,)
-        norm(prefix + "norm.", cond)
-        for i in range(layers):
-            b = f"{prefix}convnext.{i}."
-            out[b + "gamma"] = (dim,)
-            out[b + "dwconv.weight"] = (dim, 1, 7); out[b + "dwconv.bias"] = (dim,)
-            norm(b + "norm.", cond)
-            out[b + "pwconv1.weight"] = (inter, dim); out[b + "pwconv1.bias"] = (inter,)
-            out[b + "pwconv2.weight"] = (dim, inter); out[b + "pwconv2.bias"] = (dim,)
-        out[prefix + "final_layer_norm.weight"] = (dim,); out[prefix + "final_layer_norm.bias"] = (dim,)
-
     out["prenet.linear_pre.weight"] = (dim, p["input_channels"]); out["prenet.linear_pre.bias"] = (dim,)
     for i, r in enumerate(p["sample_ratios"]):
         if r != 1:
             raise NotImplementedError("prenet SamplingBlock ratios other than 1 (the shipped configuration uses [1, 1])")
-        backbone(f"prenet.downsample.{i}.1.", 2, None)
-    backbone("prenet.vocos_backbone.", p["vocos_num_layers"], p["condition_dim"])
+        _backbone_spec(out, f"prenet.downsample.{i}.1.", dim, dim, inter, 2, None)
+    _backbone_spec(out, "prenet.vocos_backbone.", dim, dim, inter, p["vocos_num_layers"], p["condition_dim"])
     out["prenet.linear.weight"] = (p["out_channels"], dim); out["prenet.linear.bias"] = (p["out_channels"],)
     ch = d["channels"]
     wn("decoder.model.0.", (ch, d["input_channel"], 7))
@@ -168,12 +185,34 @@ def speaker_spec(c) -> Dict[str, tuple]:
     return out
 
 
-_IGNORED = ("encoder.", "postnet.", "mel_transformer.", "speaker_encoder.speaker_encoder.", "speaker_encoder.perceiver_sampler.",
-            "speaker_encoder.quantizer.project_in.", "quantizer.in_project.", "quantizer.cluster_size")
-# with global_tokens=True: the semantic tokenize side, the mel transformer's buffers (rebuilt from mel_params) and the x-vector
-# branch the reference computes and discards (speaker_encoder.py:104-109)
-_IGNORED_GLOBAL = ("encoder.", "postnet.", "mel_transformer.", "quantizer.in_project.", "quantizer.cluster_size",
-                   "speaker_encoder.speaker_encoder.pool.", "speaker_encoder.speaker_encoder.bn.", "speaker_encoder.speaker_encoder.linear.")
+def encoder_spec(c) -> Dict[str, tuple]:
+    """Reference state-dict keys -> shapes of the semantic-token path: the feature Encoder (feat_encoder.py:29-90) and the
+    quantiser's in_project (factorized_vector_quantize.py:59-61)"""
+    out: Dict[str, tuple] = {}
+    e, q = c.get("encoder", ENCODER_PARAMS), c["quantizer"]
+    dim, inter = e["vocos_dim"], e["vocos_intermediate_dim"]
+    _backbone_spec(out, "encoder.encoder.", e["input_channels"], dim, inter, e["vocos_num_layers"], None)
+    for i, r in enumerate(e["sample_ratios"]):
+        if r != 1:
+            raise NotImplementedError("encoder SamplingBlock ratios other than 1 (the shipped configuration uses [1, 1])")
+        _backbone_spec(out, f"encoder.downsample.{i}.1.", dim, dim, inter, 2, None)
+    out["encoder.project.weight"] = (e["out_channels"], dim); out["encoder.project.bias"] = (e["out_channels"],)
+    _wn_spec(out, "quantizer.in_project.", (q["codebook_dim"], q["input_dim"], 1))
+    return out
+
+
+def _ignored_prefixes(global_tokens: bool, semantic_tokens: bool) -> tuple:
+    """Checkpoint keys a BiCodec face accepts at load and does not hold: the training-only postnet, the mel transformer's buffers
+    (rebuilt from mel_params), the FVQ usage statistics, the side of tokenize that is not built, and with the global-token path
+    the x-vector branch the reference computes and discards (speaker_encoder.py:104-109)."""
+    out = ("postnet.", "mel_transformer.", "quantizer.cluster_size")
+    if not semantic_tokens:
+        out += ("encoder.", "quantizer.in_project.")
+    if global_tokens:
+        out += ("speaker_encoder.speaker_encoder.pool.", "speaker_encoder.speaker_encoder.bn.", "speaker_encoder.speaker_encoder.linear.")
+    else:
+        out += ("speaker_encoder.speaker_encoder.", "speaker_encoder.perceiver_sampler.", "speaker_encoder.quantizer.project_in.")
+    return out
 
 
 def hann_window(mp) -> torch.Tensor:
@@ -200,33 +239,58 @@ def mel_filterbank(mp) -> torch.Tensor:
     return fb * (2.0 / (f[2:] - f[:-2]))[None, :]
 
 
-class BiCodec(_Face):
-    """`global_tokens=True` adds the global-token path (`mel_spectrogram`, `get_global_tokens`): its reference keys become part of
-    the module and are required by a strict load.  The default object is the detokenize path alone."""
+def _backbone_weights(sd, prefix, layers, cond, in_scale, split):
+    """A VocosBackbone's prepared weights: the embed conv as conv planes (times in_scale), the pointwise convs as planes, and the
+    fp32 vectors of the depthwise convs and norms (no norm affine when the backbone is conditioned)."""
+    dim = sd[prefix + "embed.bias"].shape[0]
+    blocks = []
+    for i in range(layers):
+        b = f"{prefix}convnext.{i}."
+        blk = dict(dw_w=sd[b + "dwconv.weight"].reshape(dim, 7).contiguous(), dw_b=sd[b + "dwconv.bias"].contiguous(),
+                   w1=Planes.from_f32(sd[b + "pwconv1.weight"], split), b1=sd[b + "pwconv1.bias"].contiguous(),
+                   w2=Planes.from_f32(sd[b + "pwconv2.weight"], split), b2=sd[b + "pwconv2.bias"].contiguous(),
+                   gamma=sd[b + "gamma"].contiguous())
+        if not cond:
+            blk.update(ln_w=sd[b + "norm.weight"].contiguous(), ln_b=sd[b + "norm.bias"].contiguous())
+        blocks.append(blk)
+    out = dict(embed=ops.conv_planes(sd[prefix + "embed.weight"] * in_scale, split), embed_b=sd[prefix + "embed.bias"].contiguous(),
+               blocks=blocks, fn_w=sd[prefix + "final_layer_norm.weight"].contiguous(),
+               fn_b=sd[prefix + "final_layer_norm.bias"].contiguous(), layers=layers)
+    if not cond:
+        out.update(n_w=sd[prefix + "norm.weight"].contiguous(), n_b=sd[prefix + "norm.bias"].contiguous())
+    return out
 
-    def __init__(self, config: dict = None, precision: str = "accurate", global_tokens: bool = False):
+
+class BiCodec(_Face):
+    """`global_tokens=True` adds the global-token path (`mel_spectrogram`, `get_global_tokens`) and `semantic_tokens=True` the
+    semantic-token path (`get_semantic_tokens`); with both, `tokenize` returns the pair.  Each flag makes its reference keys part of
+    the module, required by a strict load.  The default object is the detokenize path alone."""
+
+    def __init__(self, config: dict = None, precision: str = "accurate", global_tokens: bool = False, semantic_tokens: bool = False):
         super().__init__()
         self.cfg = dict(config or BICODEC_CONFIG)
         self.policy = PRECISION[precision]
-        self.global_tokens = bool(global_tokens)
+        self.global_tokens, self.semantic_tokens = bool(global_tokens), bool(semantic_tokens)
         spec = bicodec_spec(self.cfg)
         if self.global_tokens:
             spec.update(speaker_spec(self.cfg))
+        if self.semantic_tokens:
+            spec.update(encoder_spec(self.cfg))
         tree = _Tree.build(spec)
         for name, child in tree.named_children():
             self.add_module(name, child)
+        self._ignored = _ignored_prefixes(self.global_tokens, self.semantic_tokens)
         self._wg = None                 # prepared weights of the global-token path
+        self._we = None                 # prepared weights of the semantic-token path
         self.eval()
 
     # ------------------------------------------------------------------ state
     def _ignored_key(self, key: str) -> bool:
-        if self.global_tokens:
-            return key.startswith(_IGNORED_GLOBAL) or key.endswith(".num_batches_tracked")
-        return key.startswith(_IGNORED)
+        return key.startswith(self._ignored) or (self.global_tokens and key.endswith(".num_batches_tracked"))
 
     def _drop_prepared(self):
         super()._drop_prepared()
-        self._wg = None
+        self._wg = self._we = None
 
     # ------------------------------------------------------------------ load-time weight preparation
     def _prepare(self):
@@ -274,31 +338,11 @@ class BiCodec(_Face):
         W["spk_b"] = sd["speaker_encoder.project.bias"].contiguous()
 
         # ---- prenet
-        dim = p["vocos_dim"]
-
-        def backbone(prefix, layers, cond, in_scale):
-            blocks = []
-            for i in range(layers):
-                b = f"{prefix}convnext.{i}."
-                blk = dict(dw_w=sd[b + "dwconv.weight"].reshape(dim, 7).contiguous(), dw_b=sd[b + "dwconv.bias"].contiguous(),
-                           w1=Planes.from_f32(sd[b + "pwconv1.weight"], sp_pre), b1=sd[b + "pwconv1.bias"].contiguous(),
-                           w2=Planes.from_f32(sd[b + "pwconv2.weight"], sp_pre), b2=sd[b + "pwconv2.bias"].contiguous(),
-                           gamma=sd[b + "gamma"].contiguous())
-                if not cond:
-                    blk.update(ln_w=sd[b + "norm.weight"].contiguous(), ln_b=sd[b + "norm.bias"].contiguous())
-                blocks.append(blk)
-            out = dict(embed=ops.conv_planes(sd[prefix + "embed.weight"] * in_scale, sp_pre), embed_b=sd[prefix + "embed.bias"].contiguous(),
-                       blocks=blocks, fn_w=sd[prefix + "final_layer_norm.weight"].contiguous(),
-                       fn_b=sd[prefix + "final_layer_norm.bias"].contiguous(), layers=layers)
-            if not cond:
-                out.update(n_w=sd[prefix + "norm.weight"].contiguous(), n_b=sd[prefix + "norm.bias"].contiguous())
-            return out
-
         W["lin_pre"] = Planes.from_f32(sd["prenet.linear_pre.weight"], sp_pre)
         W["lin_pre_b"] = sd["prenet.linear_pre.bias"].contiguous()
         # SamplingBlock(up = down = 1) returns conv_res + skip1 + skip2 = 3 x (samper.py:75-100): folded into the embed conv
-        W["down"] = [backbone(f"prenet.downsample.{i}.1.", 2, None, 3.0) for i in range(len(p["sample_ratios"]))]
-        W["bb"] = backbone("prenet.vocos_backbone.", p["vocos_num_layers"], p["condition_dim"], 1.0)
+        W["down"] = [_backbone_weights(sd, f"prenet.downsample.{i}.1.", 2, None, 3.0, sp_pre) for i in range(len(p["sample_ratios"]))]
+        W["bb"] = _backbone_weights(sd, "prenet.vocos_backbone.", p["vocos_num_layers"], p["condition_dim"], 1.0, sp_pre)
         # all AdaLayerNorm scale / shift projections of the conditioned backbone as one [2 (L+1) dim, cond] matrix
         names = ["prenet.vocos_backbone.norm."] + [f"prenet.vocos_backbone.convnext.{i}.norm." for i in range(p["vocos_num_layers"])]
         W["cond_w"] = Planes.from_f32(torch.cat([torch.cat([sd[n + "scale.weight"], sd[n + "shift.weight"]], 0) for n in names], 0), True)
@@ -333,21 +377,24 @@ class BiCodec(_Face):
     def _conv(self, a: Planes, w: Planes, n, B, rows_in, ld, m, taps, **kw):
         ops.gemm(a, w, n, a_batch=B, a_rows_per_batch=rows_in, a_ld=ld, m_per_batch=m, taps=taps, **kw)
 
-    def _backbone(self, bw, x, B, T, dim, inter, cond=None, cond_stride=0, tag=""):
-        """VocosBackbone (vocos.py:273-335) on the fp32 trunk x [B*T, dim]; returns a new fp32 [B*T, dim]."""
-        M, sp = B * T, self.policy["prenet"]
-        cp = _pad_to(dim, 64)
-        pad = self._planes("bb_pad", (B, T + 6, cp), sp)
-        ops.rows_to_planes(x, B, T, dim, pad, cp, T + 6, 3)
-        y = self._buf("bb_y", (M, dim))
+    def _backbone(self, bw, x, B, T, dim, inter, cond=None, cond_stride=0, tag="", cin=None, split=None, scope=""):
+        """VocosBackbone (vocos.py:273-335) on the fp32 trunk x [B*T, cin] (cin defaults to dim); returns a new fp32 [B*T, dim].
+        `split` defaults to the prenet's precision; `scope` prefixes every scratch name."""
+        M = B * T
+        sp = self.policy["prenet"] if split is None else split
+        cin = dim if cin is None else cin
+        cp = _pad_to(cin, 64)
+        pad = self._planes(scope + "bb_pad", (B, T + 6, cp), sp)
+        ops.rows_to_planes(x, B, T, cin, pad, cp, T + 6, 3)
+        y = self._buf(scope + "bb_y", (M, dim))
         self._conv(pad, bw["embed"], dim, B, T + 6, cp, T, 7, bias=bw["embed_b"], out_f32=rowmap(y, dim, T, 0))
-        h = self._buf("bb_h" + tag, (M, dim))
+        h = self._buf(scope + "bb_h" + tag, (M, dim))
         if cond is None:
             ops.layernorm(y, bw["n_w"], bw["n_b"], B, T, dim, out_f32=h)
         else:
             ops.adalayernorm(y, cond[0], cond[0][dim:], cond_stride, B, T, dim, out_f32=h)
-        t1 = self._planes("bb_t1", (M, dim), sp)
-        hid = self._planes("bb_hid", (M, inter), sp)
+        t1 = self._planes(scope + "bb_t1", (M, dim), sp)
+        hid = self._planes(scope + "bb_hid", (M, inter), sp)
         hm = rowmap(h, dim, M, 0)
         for i, blk in enumerate(bw["blocks"]):
             if cond is None:
@@ -359,7 +406,7 @@ class BiCodec(_Face):
                      out_planes=hid, out_planes_map=(inter, M, 0))
             ops.gemm(hid, blk["w2"], dim, a_batch=1, a_rows_per_batch=M, a_ld=inter, m_per_batch=M, bias=blk["b2"],
                      gamma=blk["gamma"], residual=hm, out_f32=hm)
-        out = self._buf("bb_out" + tag, (M, dim))
+        out = self._buf(scope + "bb_out" + tag, (M, dim))
         ops.layernorm(h, bw["fn_w"], bw["fn_b"], B, T, dim, out_f32=out)
         return out
 
@@ -687,6 +734,71 @@ class BiCodec(_Face):
             taps.update(mel=mel.clone().reshape(B, T, -1), latent=lat32.clone().reshape(B, T, ECAPA_OUT), perceiver=xn.reshape(B, N, D),
                         z=zt.reshape(B, N, nl))
         return idx
+
+    # ------------------------------------------------------------------ semantic tokens
+    def _prepare_semantic(self):
+        if self._we is not None:
+            return self._we
+        if not self.semantic_tokens:
+            raise RuntimeError("this BiCodec was built without the semantic-token path: construct it with BiCodec(..., semantic_tokens=True)")
+        self._require_cuda()
+        e, q = self.cfg.get("encoder", ENCODER_PARAMS), self.cfg["quantizer"]
+        if any(w % 64 for w in (e["input_channels"], e["vocos_dim"], e["vocos_intermediate_dim"], e["out_channels"])):
+            raise ValueError("BiCodec encoder widths must be multiples of 64")
+        if q["input_dim"] != e["out_channels"]:
+            raise ValueError("quantizer input_dim must equal the encoder's out_channels")
+        keys = set(encoder_spec(self.cfg)) | {"quantizer.codebook.weight"}
+        sd ={k: v.detach().float() for k, v in self.state_dict().items() if k in keys}
+        # every encoder contraction is a 3-term split whatever `precision` says: the outputs are discrete
+        E = dict(enc=_backbone_weights(sd, "encoder.encoder.", e["vocos_num_layers"], None, 1.0, True),
+                 down=[_backbone_weights(sd, f"encoder.downsample.{i}.1.", 2, None, 3.0, True) for i in range(len(e["sample_ratios"]))],
+                 proj=Planes.from_f32(sd["encoder.project.weight"], True), proj_b=sd["encoder.project.bias"].contiguous())
+        v, g = sd["quantizer.in_project.weight_v"].double(), sd["quantizer.in_project.weight_g"].double()
+        E["w_in"] = (v * (g / v.reshape(v.shape[0], -1).norm(dim=1).reshape(g.shape)))[:, :, 0].float().contiguous()
+        E["b_in"] = sd["quantizer.in_project.bias"].contiguous()
+        E["cb_n"] = torch.nn.functional.normalize(sd["quantizer.codebook.weight"].double(), dim=1).contiguous()
+        self._we = E
+        return E
+
+    @torch.no_grad()
+    def get_semantic_tokens(self, batch, taps=None) -> torch.Tensor:
+        """bicodec.py:167-172: batch["feat"] [B, T, input_channels] (the channel-last wav2vec2 features; a bare tensor is also taken)
+        -> int64 [B, T], the layout detokenize takes.  taps (a dict) receives fp32 copies: "encoder" [B, T, out_channels] (the
+        Encoder's output, channel-last) and "z_e" [B, T, codebook_dim] (the in_project output, before normalisation)."""
+        E = self._prepare_semantic()
+        feat = batch["feat"] if isinstance(batch, dict) else batch
+        e, q = self.cfg.get("encoder", ENCODER_PARAMS), self.cfg["quantizer"]
+        if not isinstance(feat, torch.Tensor) or feat.ndim != 3 or feat.shape[2] != e["input_channels"]:
+            raise ValueError(f"feat must be [B, T, {e['input_channels']}]")
+        if feat.device.type != "cuda":
+            raise RuntimeError("unified_audio_b200.BiCodec runs on CUDA only (no CPU fallback): feat is on the CPU")
+        B, T, Cin = feat.shape
+        M, dim, inter, C = B * T, e["vocos_dim"], e["vocos_intermediate_dim"], e["out_channels"]
+        x = feat.float().contiguous().reshape(M, Cin)
+        # ---- Encoder (feat_encoder.py:79-90); scratch names under "enc_", apart from the prenet's
+        x = self._backbone(E["enc"], x, B, T, dim, inter, tag="_e", cin=Cin, split=True, scope="enc_")
+        for i, bw in enumerate(E["down"]):
+            x = self._backbone(bw, x, B, T, dim, inter, tag=f"_d{i}", split=True, scope="enc_")
+        xpl = self._planes("enc_x_p", (M, dim), True)
+        ops.split_f16(x, xpl)
+        z = self._buf("enc_z", (M, C))
+        ops.gemm(xpl, E["proj"], C, a_batch=1, a_rows_per_batch=M, a_ld=dim, m_per_batch=M, bias=E["proj_b"], out_f32=rowmap(z, C, M, 0))
+        # ---- FactorizedVectorQuantize.tokenize (factorized_vector_quantize.py:148-152,169-187)
+        idx = torch.empty(B, T, dtype=torch.int64, device=feat.device)
+        z_e = torch.empty(B, T, q["codebook_dim"], device=feat.device) if taps is not None else None
+        ops.fvq_tokenize(z, M, C, E["w_in"], E["b_in"], E["cb_n"], q["codebook_size"], q["codebook_dim"], idx, z_e)
+        if taps is not None:
+            taps.update(encoder=z.clone().reshape(B, T, C), z_e=z_e)
+        return idx
+
+    @torch.no_grad()
+    def tokenize(self, batch):
+        """bicodec.py:151-165: batch {"feat": [B, T, input_channels], "ref_wav": [B, L]} -> (semantic_tokens int64 [B, T],
+        global_tokens int32 [B, 1, token_num]), the reference's order.  Needs both token paths."""
+        missing = [f for f in ("semantic_tokens", "global_tokens") if not getattr(self, f)]
+        if missing:
+            raise RuntimeError(f"BiCodec.tokenize needs both token paths: construct it with {', '.join(f + '=True' for f in missing)}")
+        return self.get_semantic_tokens(batch), self.get_global_tokens(batch)
 
     def forward(self, *a, **k):
         raise RuntimeError("unified_audio_b200.BiCodec implements detokenize only (the decoder UniSE uses, model.py:193)")

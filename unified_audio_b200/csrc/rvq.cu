@@ -112,8 +112,120 @@ __global__ void rvq_decode_kernel(const int64_t* __restrict__ idx, const float* 
   }
 }
 
+// Factorised VQ tokenize (BiCodec's semantic quantiser, factorized_vector_quantize.py:148-152,169-187), all in fp64: the
+// codebook is 8-wide, so the whole scan is ~1 G fp64 FMA at the largest batches and needs no shortlist / re-rank.
+//   phase 1: a warp per row: z_e = W_in z + b_in (fp64 sums over D_in), e = z_e / max(|z_e|, 1e-12) -> shared memory;
+//   phase 2: the codebook streams through shared memory in tiles; warp w scans its slice of every tile with lane = row, so
+//            every lane of a warp reads the same code (broadcast); score 2 e.c - |c|^2 (-dist without the row constant |e|^2);
+//   then the FVQ_SLICES per-row winners are merged: highest score, lowest index on exact ties.
+constexpr int FVQ_ROWS = 32, FVQ_SLICES = 8, FVQ_TILE = 256;
+
+template <int CD>
+__global__ void __launch_bounds__(FVQ_ROWS * FVQ_SLICES)
+fvq_tokenize_kernel(const float* __restrict__ z, long long M, int D, const float* __restrict__ w_in, const float* __restrict__ b_in,
+                    const double* __restrict__ cb, int K, int cdim, int64_t* __restrict__ idx, float* __restrict__ z_e) {
+  __shared__ double e_s[FVQ_ROWS][CD];
+  __shared__ double c_s[FVQ_TILE][CD];
+  __shared__ double c2_s[FVQ_TILE];
+  __shared__ double best_s[FVQ_SLICES][FVQ_ROWS];
+  __shared__ int bi_s[FVQ_SLICES][FVQ_ROWS];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long row0 = (long long)blockIdx.x * FVQ_ROWS;
+  for (int r = warp; r < FVQ_ROWS; r += FVQ_SLICES) {
+    const long long m = row0 + r;
+    double acc[CD];
+#pragma unroll
+    for (int j = 0; j < CD; ++j) acc[j] = 0.0;
+    if (m < M) {
+      const float* zr = z + m * D;
+      for (int c = lane; c < D; c += 32) {
+        const double v = (double)zr[c];
+#pragma unroll
+        for (int j = 0; j < CD; ++j)
+          if (j < cdim) acc[j] = fma((double)w_in[(long long)j * D + c], v, acc[j]);
+      }
+    }
+    double n2 = 0.0;
+#pragma unroll
+    for (int j = 0; j < CD; ++j) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], o);
+      if (j < cdim && m < M) {
+        acc[j] += (double)b_in[j];
+        n2 = fma(acc[j], acc[j], n2);
+        if (z_e && lane == 0) z_e[m * cdim + j] = (float)acc[j];
+      }
+    }
+    const double inv = 1.0 / fmax(sqrt(n2), 1e-12);               // F.normalize
+    if (lane == 0) {
+#pragma unroll
+      for (int j = 0; j < CD; ++j) e_s[r][j] = (j < cdim && m < M) ? acc[j] * inv : 0.0;
+    }
+  }
+  __syncthreads();
+  double e[CD];
+#pragma unroll
+  for (int j = 0; j < CD; ++j) e[j] = e_s[lane][j];
+  double best = -INFINITY;
+  int bi = 0x7fffffff;
+  constexpr int PER = FVQ_TILE / FVQ_SLICES;
+  for (int k0 = 0; k0 < K; k0 += FVQ_TILE) {
+    const int nk = min(FVQ_TILE, K - k0);
+    for (int i = threadIdx.x; i < FVQ_TILE * CD; i += blockDim.x) {
+      const int k = i / CD, j = i % CD;
+      c_s[k][j] = (k < nk && j < cdim) ? cb[(long long)(k0 + k) * cdim + j] : 0.0;
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < nk; k += blockDim.x) {
+      double s = 0.0;
+#pragma unroll
+      for (int j = 0; j < CD; ++j) s = fma(c_s[k][j], c_s[k][j], s);
+      c2_s[k] = s;
+    }
+    __syncthreads();
+    const int kb = warp * PER, ke = min(kb + PER, nk);
+    for (int k = kb; k < ke; ++k) {                                  // ascending: strict > keeps the lowest index
+      double s = 0.0;
+#pragma unroll
+      for (int j = 0; j < CD; ++j) s = fma(e[j], c_s[k][j], s);
+      const double score = 2.0 * s - c2_s[k];
+      if (score > best) { best = score; bi = k0 + k; }
+    }
+    __syncthreads();
+  }
+  best_s[warp][lane] = best;
+  bi_s[warp][lane] = bi;
+  __syncthreads();
+  if (warp == 0) {
+    const long long m = row0 + lane;
+    double b = best_s[0][lane];
+    int id = bi_s[0][lane];
+    for (int w = 1; w < FVQ_SLICES; ++w) {
+      const double o = best_s[w][lane];
+      const int oi = bi_s[w][lane];
+      if (o > b || (o == b && oi < id)) { b = o; id = oi; }
+    }
+    if (m < M) idx[m] = id == 0x7fffffff ? 0 : (int64_t)id;        // an all-NaN row: index 0, as torch.max
+  }
+}
+
 }  // namespace qb
 using namespace qb;
+
+extern "C" int qb_fvq_tokenize(const float* z, int64_t M, int32_t D_in, const float* w_in, const float* b_in, const double* codebook_n,
+                               int32_t K, int32_t cdim, int64_t* idx, float* z_e, void* stream) {
+  QB_REQUIRE(z && w_in && b_in && codebook_n && idx && M >= 0 && D_in >= 1 && K >= 1, "fvq_tokenize: bad args");
+  QB_REQUIRE(cdim >= 1 && cdim <= 16, "fvq_tokenize: codebook_dim must be 1..16 (got %d)", cdim);
+  if (M == 0) return 0;
+  const unsigned grid = (unsigned)ceil_div(M, FVQ_ROWS);
+  if (cdim <= 8)
+    fvq_tokenize_kernel<8><<<grid, FVQ_ROWS * FVQ_SLICES, 0, (cudaStream_t)stream>>>(z, M, D_in, w_in, b_in, codebook_n, K, cdim, idx, z_e);
+  else
+    fvq_tokenize_kernel<16><<<grid, FVQ_ROWS * FVQ_SLICES, 0, (cudaStream_t)stream>>>(z, M, D_in, w_in, b_in, codebook_n, K, cdim, idx, z_e);
+  g_launches++;
+  QB_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
 
 extern "C" int64_t qb_rvq_workspace_bytes(int64_t M, int32_t D, int32_t K) {
   return M * D * 4 + 2 * M * D * 2 + M * (int64_t)K * 4 + 1024;

@@ -296,6 +296,12 @@ def rvq_decode(idx, codebooks, M, D, K, nq, out, out_ld, col_off):
     _lib.check(_lib.load().qb_rvq_decode(_p(idx), _p(codebooks), M, D, K, nq, _p(out), out_ld, col_off, _stream()))
 
 
+def fvq_tokenize(z, M, D_in, w_in, b_in, codebook_n, K, cdim, idx, z_e=None):
+    """z [M, D_in] fp32 -> idx [M] int64 (+ z_e [M, cdim] fp32); codebook_n is the fp64 normalised codebook [K, cdim]"""
+    assert codebook_n.dtype == torch.float64 and idx.dtype == torch.int64
+    _lib.check(_lib.load().qb_fvq_tokenize(_p(z), M, D_in, _p(w_in), _p(b_in), _p(codebook_n), K, cdim, _p(idx), _p(z_e), _stream()))
+
+
 def lm_qkv_prep(qkv, B, L, heads, pos0, cos, sin, q16, kc, vc, Lmax):
     _lib.check(_lib.load().qb_lm_qkv_prep(_p(qkv), B, L, heads, pos0, _p(cos), _p(sin), _p(q16), _p(kc), _p(vc), Lmax,
                                           _stream()))

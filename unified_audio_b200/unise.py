@@ -6,7 +6,8 @@ training / validation steps and checkpoint callbacks are out of scope, SURVEY 2)
     .extract_semantic_features(wavs [B, T] @ 16 kHz) -> [B, T/320, 768]        model.py:37-51
     .stft_logmel(x [B, T]) -> [B, ceil(T/320), 80]                               model.py:53-79
     .test_step((mode, enroll, src, tgt, fs, lengths, names), batch_idx)          model.py:170-286, modes 'se' / 'tse' / 'ss'
-and audio_tokenizer.py:30-125 for `BiCodecTokenizer.detokenize(global_tokens, semantic_tokens)`.
+and audio_tokenizer.py:30-125 for `BiCodecTokenizer.detokenize(global_tokens, semantic_tokens)` and, given the wav2vec2 front end,
+`BiCodecTokenizer.tokenize(wav) -> (global_tokens, semantic_tokens)`.
 
 Everything between the waveform in and the waveform out stays on the GPU: wrap-pad + 5 s segmenting (`qb_pad_wav`, no NumPy round
 trip), WavLM features (csrc/ssl.cu + the conv-GEMM / attention kernels), `LLM_SFT.generate` (csrc/llm.cu), `BiCodec.detokenize`.
@@ -31,15 +32,17 @@ SEG_LEN = 5 * 16000                                                            #
 
 
 class BiCodecTokenizer(nn.Module):
-    """audio_tokenizer.py:30-125, detokenize side and `get_ref_clip`.  `tokenize` (wav2vec2-large-xlsr-53 features + the BiCodec
-    encoder) is only called by the training / validation steps (model.py:96-99,139-142): out of scope, raises.
-    ref_segment_length = int(sample_rate * ref_segment_duration) // latent_hop_length * latent_hop_length (audio_tokenizer.py:60-64):
-    96000 for the published 16 kHz, 6 s, 320-sample configuration."""
+    """audio_tokenizer.py:30-125.  `tokenize` (UniSE tokenizes clean speech with it, model.py:96-102,134-140) needs the wav2vec2
+    front end, `feature_extractor` = SSLFrontEnd(WAV2VEC2_XLSR53) (extract_wav2vec2_features, audio_tokenizer.py:74-90), and a
+    BiCodec built with global_tokens=True and semantic_tokens=True; without them it raises NotImplementedError.  detokenize needs
+    neither.  ref_segment_length = int(sample_rate * ref_segment_duration) // latent_hop_length * latent_hop_length
+    (audio_tokenizer.py:60-64): 96000 for the published 16 kHz, 6 s, 320-sample configuration."""
 
-    def __init__(self, model, ref_segment_length: int = 96000):
+    def __init__(self, model, ref_segment_length: int = 96000, feature_extractor: Optional[nn.Module] = None):
         super().__init__()
         self.model = model
         self.ref_segment_length = int(ref_segment_length)
+        self.feature_extractor = feature_extractor
 
     @torch.no_grad()
     def get_ref_clip(self, wav: torch.Tensor) -> torch.Tensor:
@@ -54,9 +57,20 @@ class BiCodecTokenizer(nn.Module):
             return ops.pad_wav(wav, 0, n, wrap=True)
         return wav[:, :n].float().contiguous()
 
-    def tokenize(self, wav):
-        raise NotImplementedError("BiCodecTokenizer.tokenize is used by the training / validation steps only (model.py:96-99); "
-                                  "the inference path needs detokenize")
+    @torch.no_grad()
+    def tokenize(self, wav: torch.Tensor):
+        """audio_tokenizer.py:92-105: wav [B, L] @ 16 kHz -> (global_tokens int32 [B, 1, token_num], semantic_tokens int64 [B, T']),
+        the reference's order; everything stays on the device."""
+        missing = [] if self.feature_extractor is not None else ["a feature_extractor (SSLFrontEnd(WAV2VEC2_XLSR53))"]
+        missing += [f"BiCodec(..., {f}=True)" for f in ("global_tokens", "semantic_tokens") if not getattr(self.model, f, False)]
+        if missing:
+            raise NotImplementedError("BiCodecTokenizer.tokenize needs " + " and ".join(missing))
+        if wav.device.type != "cuda":
+            raise RuntimeError("unified_audio_b200.unise.BiCodecTokenizer runs on CUDA only (no CPU fallback)")
+        ref_wav = self.get_ref_clip(wav)
+        feat = self.feature_extractor(wav)
+        semantic_tokens, global_tokens = self.model.tokenize({"wav": wav, "ref_wav": ref_wav, "feat": feat})
+        return global_tokens, semantic_tokens
 
     @torch.no_grad()
     def detokenize(self, global_tokens: torch.Tensor, semantic_tokens: torch.Tensor) -> torch.Tensor:
