@@ -1,6 +1,7 @@
 """Multi-GPU plumbing of the hot path (SURVEY.md 8e): clips are independent, so ranks own contiguous batch
 shards with replicated weights and NO data-path collective; the single exchange step is one all-gather of the
-int64 token tensors.  Works with backend "nccl" (GPU) and "gloo" (CPU tests)."""
+int64 token tensors.  A validation epoch ends with one all-reduce of its running sums.  Works with backend
+"nccl" (GPU) and "gloo" (CPU tests)."""
 from __future__ import annotations
 
 from typing import Optional, Tuple
@@ -13,6 +14,15 @@ def shard_range(n_items: int, rank: int, world: int) -> Tuple[int, int]:
     base, rem = divmod(n_items, world)
     lo = rank * base + min(rank, rem)
     return lo, lo + base + (1 if rank < rem else 0)
+
+
+def all_reduce_sum(t: torch.Tensor, group=None) -> torch.Tensor:
+    """Sum `t` over the ranks of `group` in place with one `all_reduce` and return it; unchanged when torch.distributed is not
+    initialised.  `unise.Model.validation_epoch` sums its fp64 [Σ B·loss, Σ B·acc, Σ B] with it."""
+    import torch.distributed as dist
+    if dist.is_available() and dist.is_initialized():
+        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
+    return t
 
 
 def gather_tokens(tokens: torch.Tensor, n_total: int, group=None, buffers: Optional[dict] = None) -> torch.Tensor:

@@ -1,10 +1,12 @@
-"""UniSE inference surface (`Model.test_step`) on the device: the caller of the AR-LM hot path.
+"""UniSE inference and validation surface (`Model.test_step`, `Model.validation_step`) on the device: the callers of the AR-LM hot path.
 
 Mirrors QuarkAudio-UniSE/model/model.py:20-286 (a LightningModule in the reference; a plain nn.Module here - the Lightning task,
-training / validation steps and checkpoint callbacks are out of scope, SURVEY 2):
+the training step and checkpoint callbacks are out of scope, SURVEY 2):
     Model(config, tokenizer=BiCodecTokenizer(BiCodec), dnn=LLM_SFT, semantic_model=SSLFrontEnd(WAVLM_BASE_PLUS))
     .extract_semantic_features(wavs [B, T] @ 16 kHz) -> [B, T/320, 768]        model.py:37-51
     .stft_logmel(x [B, T]) -> [B, ceil(T/320), 80]                               model.py:53-79
+    .validation_step((mode, enroll, mix, speech, interf, fs, lengths, names))    model.py:134-160, modes 'se' / 'tse' / 'rtse'
+    .validation_epoch(batches) -> batch-size-weighted epoch means, across ranks   model.py:160 (log_dict on_epoch, sync_dist)
     .test_step((mode, enroll, src, tgt, fs, lengths, names), batch_idx)          model.py:170-286, modes 'se' / 'tse' / 'ss'
 and audio_tokenizer.py:30-125 for `BiCodecTokenizer.detokenize(global_tokens, semantic_tokens)` and, given the wav2vec2 front end,
 `BiCodecTokenizer.tokenize(wav) -> (global_tokens, semantic_tokens)`.
@@ -57,14 +59,18 @@ class BiCodecTokenizer(nn.Module):
             return ops.pad_wav(wav, 0, n, wrap=True)
         return wav[:, :n].float().contiguous()
 
-    @torch.no_grad()
-    def tokenize(self, wav: torch.Tensor):
-        """audio_tokenizer.py:92-105: wav [B, L] @ 16 kHz -> (global_tokens int32 [B, 1, token_num], semantic_tokens int64 [B, T']),
-        the reference's order; everything stays on the device."""
+    def require_tokenize(self) -> None:
+        """Raise the NotImplementedError `tokenize` raises when this tokenizer cannot tokenize; it names what is missing."""
         missing = [] if self.feature_extractor is not None else ["a feature_extractor (SSLFrontEnd(WAV2VEC2_XLSR53))"]
         missing += [f"BiCodec(..., {f}=True)" for f in ("global_tokens", "semantic_tokens") if not getattr(self.model, f, False)]
         if missing:
             raise NotImplementedError("BiCodecTokenizer.tokenize needs " + " and ".join(missing))
+
+    @torch.no_grad()
+    def tokenize(self, wav: torch.Tensor):
+        """audio_tokenizer.py:92-105: wav [B, L] @ 16 kHz -> (global_tokens int32 [B, 1, token_num], semantic_tokens int64 [B, T']),
+        the reference's order; everything stays on the device."""
+        self.require_tokenize()
         if wav.device.type != "cuda":
             raise RuntimeError("unified_audio_b200.unise.BiCodecTokenizer runs on CUDA only (no CPU fallback)")
         ref_wav = self.get_ref_clip(wav)
@@ -129,6 +135,77 @@ class Model(nn.Module):
     def forward(self, batch):
         """model.py:93-94: the reference's forward is empty; inference goes through test_step."""
         return None
+
+    # ------------------------------------------------------------------ validation (model.py:134-160)
+    @staticmethod
+    def _validation_inputs(batch):
+        """batch -> (mode, enroll, mix, the waveform the mode tokenizes: `interf` for 'rtse', `speech` otherwise, model.py:137-140).
+        Refuses what the reference would only fail on later, inside the tokenizer or the LM."""
+        mode, enroll, mix, speech, interf, fs, lengths, names = batch
+        if mode not in ("se", "tse", "rtse"):
+            raise ValueError(f"unknown mode {mode!r} (the reference's validation_step handles 'se', 'tse', 'rtse')")
+        name = "interf" if mode == "rtse" else "speech"
+        wav = interf if mode == "rtse" else speech
+        if wav is None:
+            raise ValueError(f"mode {mode!r} tokenizes `{name}`, which is None")
+        sizes = {"mix": mix.shape[0], name: wav.shape[0]}
+        if enroll is not None:
+            sizes["enroll"] = enroll.shape[0]
+        if len(set(sizes.values())) > 1:
+            raise ValueError(f"batch sizes differ: {sizes}")
+        return mode, enroll, mix, wav
+
+    @torch.no_grad()
+    def validation_step(self, batch, batch_idx=0):
+        """model.py:134-160: batch = (mode, enroll, mix, speech, interf, fs, lengths, names) on the device, mode 'se' / 'tse' / 'rtse'.
+        Tokenizes `speech` ('se', 'tse') or `interf` ('rtse') with `BiCodecTokenizer.tokenize`, extracts WavLM features of `mix` and,
+        when `enroll` is not None, of `enroll` (which then joins the LM prefix), and runs the teacher-forced `LLM_SFT.forward`.
+        Returns {"valid_loss", "valid_acc"}: 0-d fp32 device tensors, what the reference logs; no host synchronisation.
+
+        The reference's log-mels (`stft_logmel` of mix and enroll) are dead compute here: `LLM_SFT.forward` reads only the mix mel's
+        batch size and device (llm_sft.py:60) and whether the enrollment mel is None, so the step passes shape-only tensors
+        (`mel_like`), as `test_step` does.  `semantic_tokens` keep wav2vec2's unpadded length (80 000 samples -> 249 tokens) while the
+        WavLM features of `mix` are padded 160 / 160 (-> 250 frames); nothing assumes the two are equal."""
+        self.tokenizer.require_tokenize()
+        _, enroll, mix, wav = self._validation_inputs(batch)
+        if any(t is not None and t.device.type != "cuda" for t in (enroll, mix, wav)):
+            raise RuntimeError("unified_audio_b200.unise.Model runs on CUDA only (no CPU fallback)")
+        return self._validation_step(batch)
+
+    def _validation_step(self, batch):
+        """validation_step's control flow (model.py:135-160) over the three components; pinned against the reference's own
+        `validation_step` driven with stand-ins (oracle/make_golden_unise_validation.py -> tests/golden/unise_validation_glue.npz)."""
+        mode, enroll, mix, wav = self._validation_inputs(batch)
+        global_tokens, semantic_tokens = self.tokenizer.tokenize(wav)
+        mix_feats = self.extract_semantic_features(mix)
+        enroll_mel = enroll_feats = None
+        if enroll is not None:
+            enroll_mel, enroll_feats = self.mel_like(enroll), self.extract_semantic_features(enroll)
+        loss, acc = self.dnn(task_name=mode, enroll_mel=enroll_mel, enroll_feats=enroll_feats, mix_mel=self.mel_like(mix),
+                             mix_feats=mix_feats, global_ids=global_tokens.squeeze(1), semantic_ids=semantic_tokens)
+        return {"valid_loss": loss, "valid_acc": acc}
+
+    def validation_epoch(self, batches, group=None) -> dict:
+        """A validation epoch as the reference logs it (`log_dict(..., on_epoch=True, sync_dist=True)`, model.py:160).  Each batch's
+        tensors are moved to the LM's device and scored by `validation_step`.  Running sums of B·loss, B·acc and B (B = the batch's
+        clip count) stay on the device in fp64; when torch.distributed is initialised they are summed across the ranks of `group`
+        with one all_reduce (`parallel.all_reduce_sum`), and read on the host once, at the end.
+        Returns {"valid_loss": Σ B·loss / Σ B, "valid_acc": Σ B·acc / Σ B} as floats, over every batch of every rank."""
+        from .parallel import all_reduce_sum
+        dev = next(self.dnn.parameters()).device
+        sums = torch.zeros(3, dtype=torch.float64, device=dev)
+        n = 0
+        for i, batch in enumerate(batches):
+            batch = tuple(x.to(dev, non_blocking=True) if torch.is_tensor(x) else x for x in batch)
+            out = self.validation_step(batch, i)
+            b = batch[2].shape[0]
+            sums[:2] += b * torch.stack((out["valid_loss"], out["valid_acc"])).double()
+            n += b
+        sums[2] = n
+        loss, acc, total = all_reduce_sum(sums, group).tolist()
+        if total == 0:
+            raise ValueError("validation_epoch: no batch on any rank")
+        return {"valid_loss": loss / total, "valid_acc": acc / total}
 
     # ------------------------------------------------------------------ inference (model.py:170-286)
     def _segments(self, src: torch.Tensor) -> torch.Tensor:
