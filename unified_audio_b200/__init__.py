@@ -12,6 +12,9 @@ Public surface mirrors the reference (alibaba/unified-audio):
                       (HCodec-2.0/audio_tokenizer.py:47-61), Model.extract_semantic_features (U/model/model.py:38-51) and
                       BiCodecTokenizer.extract_wav2vec2_features (U/model/bicodec/audio_tokenizer.py:74-90) drive them
   HCodecTokenizer  <- QuarkAudio-HCodec/HCodec-2.0/audio_tokenizer.py:21-79 (pad_wav / tokenize / detokenize)
+  HCodecTokenizerH1  <- QuarkAudio-HCodec/HCodec-1.0/audio_tokenizer.py:18-66 (HuBERT-base features -> CodecH1)
+  HCodecTokenizerH15 <- QuarkAudio-HCodec/HCodec-1.5/audio_tokenizer.py:38-86 (wav2vec2-XLSR-53 features, WAV2VEC2_XLSR53_RAW ->
+                      CodecH15, length-packed codes)
   unise.Model      <- QuarkAudio-UniSE/model/model.py:20-286 (extract_semantic_features / test_step: 'se', 'tse', 'ss') with
                       unise.BiCodecTokenizer <- model/bicodec/audio_tokenizer.py:30-125 (get_ref_clip / tokenize / detokenize)
 Kernels live in csrc/ behind the C ABI of include/quark_b200.h (lib/libquark_b200.so).
@@ -26,4 +29,5 @@ from .llm import LLM_SFT  # noqa: E402,F401
 from .bicodec import BiCodec  # noqa: E402,F401
 from . import adaptive  # noqa: E402,F401
 from .ssl import HCodecTokenizer, HUBERT_BASE, SSLFrontEnd, WAV2VEC2_XLSR53, WAVLM_BASE_PLUS, pad_wav, wrap_segments  # noqa: E402,F401
+from .ssl import HCodecTokenizerH1, HCodecTokenizerH15, WAV2VEC2_XLSR53_RAW  # noqa: E402,F401
 from . import unise  # noqa: E402,F401

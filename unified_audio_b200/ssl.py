@@ -4,6 +4,11 @@
         Resample(48k -> 16k) -> pad 160/160 -> HuBERT-base (`AutoModel "bosonai/hubert_base"`, output_hidden_states) ->
         mean of the 13 hidden states -> sign(x) |x|^0.3                                       [B, T50, 768]
     HCodecTokenizer.pad_wav / tokenize      audio_tokenizer.py:63-75
+    HCodecTokenizerH1                       QuarkAudio-HCodec/HCodec-1.0/audio_tokenizer.py:18-66
+        pad_wav (640) -> pad 160/160 -> HuBERT-base at 16 kHz -> mean of the 13 hidden states -> sign(x) |x|^0.3 -> CodecH1.encode
+    HCodecTokenizerH15                      QuarkAudio-HCodec/HCodec-1.5/audio_tokenizer.py:38-86
+        pad_wav (prod(ratios) * 2) -> pad 160/160 -> wav2vec2-large-xlsr-53, no normalisation (WAV2VEC2_XLSR53_RAW) ->
+        (hidden_states[11] + hidden_states[14] + hidden_states[16]) / 3 -> sign(x) |x|^0.3 -> CodecH15.encode (length-packed codes)
     Model.extract_semantic_features         QuarkAudio-UniSE/model/model.py:38-51  (WavLM-base-plus, no compression)
     BiCodecTokenizer.extract_wav2vec2_features   QuarkAudio-UniSE/model/bicodec/audio_tokenizer.py:74-90
         Wav2Vec2FeatureExtractor(do_normalize=True) -> wav2vec2-large-xlsr-53 (no padding) ->
@@ -36,6 +41,8 @@ from torch import nn
 
 from . import ops
 from .codec import _Face, _Tree, _pad_to
+from .codec_h1 import CodecH1
+from .codec_h15 import CodecH15
 from .ops import ACT_GELU, Planes, rowmap
 
 HUBERT_BASE = dict(conv_dim=[512] * 7, conv_kernel=[10, 3, 3, 3, 3, 2, 2], conv_stride=[5, 2, 2, 2, 2, 2, 2], hidden=768,
@@ -45,6 +52,9 @@ WAVLM_BASE_PLUS = dict(HUBERT_BASE, num_buckets=320, max_distance=800, kind="wav
 # positional-conv output, k = the residual stream after layer k), do_normalize the feature extractor's per-utterance normalisation
 WAV2VEC2_XLSR53 = dict(HUBERT_BASE, hidden=1024, layers=24, heads=16, ffn=4096, kind="wav2vec2", hidden_state_ids=(11, 14, 16),
                        do_normalize=True)
+# the same model as H-Codec-1.5's tokenizer calls it (HCodec-1.5/audio_tokenizer.py:53-66): a bare `AutoModel`, no processor
+# normalisation; `HCodecTokenizerH15` adds the 160/160 pad and the front end is built with compress=True
+WAV2VEC2_XLSR53_RAW = dict(WAV2VEC2_XLSR53, do_normalize=False)
 
 
 def ssl_spec(c: dict) -> Dict[str, tuple]:
@@ -483,3 +493,107 @@ class HCodecTokenizer(nn.Module):
     @torch.no_grad()
     def detokenize(self, acoustic_codes, semantic_codes):
         return self.model.decode(acoustic_codes, semantic_codes)
+
+
+def _check_front_end(face: str, codec, fe: SSLFrontEnd, kind: str):
+    """the front-end settings a 16 kHz H-Codec tokenizer needs; each mismatch would give plausible codes with no error"""
+    c = fe.cfg
+    if c.get("kind", "hubert") != kind:                 # SSLFrontEnd runs a config without `kind` as HuBERT
+        raise ValueError(f"{face} needs a {kind} front end, got kind={c.get('kind')!r}")
+    if fe.in_rate != 16000:
+        raise ValueError(f"{face} takes 16 kHz audio: the front end must have in_rate=16000, got {fe.in_rate}")
+    if not fe.compress:
+        raise ValueError(f"{face} feeds sign(x)|x|^0.3 features to the codec: build the front end with compress=True")
+    if c["hidden"] != codec.c["sem_in"]:
+        raise ValueError(f"{face}: the front end's hidden width {c['hidden']} differs from the codec's semantic-encoder input "
+                         f"width {codec.c['sem_in']}")
+
+
+def _check_wav(face: str, wav):
+    if not isinstance(wav, torch.Tensor) or wav.ndim != 2:
+        raise ValueError(f"{face}: wav must be a [B, T] tensor, got {tuple(wav.shape) if isinstance(wav, torch.Tensor) else type(wav)}")
+    if wav.device.type != "cuda":
+        raise RuntimeError(f"unified_audio_b200.{face} runs on CUDA only (no CPU fallback)")
+
+
+class HCodecTokenizerH1(nn.Module):
+    """HCodecTokenizer of H-Codec-1.0 (HCodec-1.0/audio_tokenizer.py:18-66) on the device: pad_wav to a multiple of 640 ->
+    pad 160/160 + HuBERT-base, mean of the 13 hidden states, sign(x)|x|^0.3 (16 kHz in, no resampling) -> CodecH1.encode.
+
+    codec: CodecH1; feature_extractor: SSLFrontEnd(HUBERT_BASE, in_rate=16000, compress=True)."""
+
+    hop_length = 640                    # audio_tokenizer.py:31 (25 Hz); CodecH1's SEANet strides are fixed
+
+    def __init__(self, codec, feature_extractor: SSLFrontEnd):
+        super().__init__()
+        if not isinstance(codec, CodecH1) or isinstance(codec, CodecH15):
+            raise ValueError(f"HCodecTokenizerH1 needs a CodecH1, got {type(codec).__name__}")
+        _check_front_end("HCodecTokenizerH1", codec, feature_extractor, "hubert")
+        self.model, self.feature_extractor = codec, feature_extractor
+
+    def pad_wav(self, wav):
+        return pad_wav(wav, self.hop_length)
+
+    @torch.no_grad()
+    def extract_wav2vec2_features(self, wavs):
+        """audio_tokenizer.py:35-49 (HuBERT despite the name): wavs [B, T] -> [B, T/320, 768]"""
+        _check_wav("HCodecTokenizerH1", wavs)
+        return self.feature_extractor(wavs)
+
+    @torch.no_grad()
+    def tokenize(self, wav):
+        """audio_tokenizer.py:56-61: wav [B, T] @ 16 kHz -> (acoustic, semantic) int64 [B, nq, ceil(T / 640)]"""
+        _check_wav("HCodecTokenizerH1", wav)
+        wav = self.pad_wav(wav)
+        feats = self.feature_extractor(wav, channel_first=True)        # (b, d, t) written channel-first by the kernel
+        return self.model.encode(wav[:, None], feats)
+
+    @torch.no_grad()
+    def detokenize(self, acoustic_codes, semantic_codes):
+        """audio_tokenizer.py:63-66: -> wav [B, N * 640]"""
+        return self.model.decode(acoustic_codes, semantic_codes)
+
+
+class HCodecTokenizerH15(nn.Module):
+    """HCodecTokenizer of H-Codec-1.5 (HCodec-1.5/audio_tokenizer.py:38-86) on the device: pad_wav to a multiple of
+    prod(ratios) * 2 -> pad 160/160 + wav2vec2-large-xlsr-53 called bare (no processor normalisation), (hs[11] + hs[14] +
+    hs[16]) / 3, sign(x)|x|^0.3 -> the adaptive CodecH15.encode with the codec's own threshold (length-packed codes).
+
+    codec: CodecH15; feature_extractor: SSLFrontEnd(WAV2VEC2_XLSR53_RAW, in_rate=16000, compress=True)."""
+
+    def __init__(self, codec, feature_extractor: SSLFrontEnd):
+        super().__init__()
+        if not isinstance(codec, CodecH15):
+            raise ValueError(f"HCodecTokenizerH15 needs a CodecH15, got {type(codec).__name__}")
+        _check_front_end("HCodecTokenizerH15", codec, feature_extractor, "wav2vec2")
+        if feature_extractor.cfg.get("do_normalize"):
+            raise ValueError("HCodecTokenizerH15: the reference calls wav2vec2 without processor normalisation; build the front end "
+                             "from WAV2VEC2_XLSR53_RAW (do_normalize=False)")
+        self.model, self.feature_extractor = codec, feature_extractor
+        self.hop_length = math.prod(codec.c["ratios"]) * 2             # audio_tokenizer.py:71
+
+    def pad_wav(self, wav):
+        return pad_wav(wav, self.hop_length)
+
+    def _features(self, wavs, channel_first):
+        T = wavs.shape[-1]
+        return self.feature_extractor(ops.pad_wav(wavs, 160, T + 320), channel_first=channel_first)
+
+    @torch.no_grad()
+    def extract_wav2vec2_features(self, wavs):
+        """audio_tokenizer.py:52-66: wavs [B, T] -> pad 160/160 -> [B, T/320, 1024]"""
+        _check_wav("HCodecTokenizerH15", wavs)
+        return self._features(wavs, False)
+
+    @torch.no_grad()
+    def tokenize(self, wav):
+        """audio_tokenizer.py:76-81: wav [B, T] @ 16 kHz -> {'acoustic_codes', 'semantic_codes'} int64 [B, nq, G], token lengths
+        packed into the indices as CodecH15.encode returns them"""
+        _check_wav("HCodecTokenizerH15", wav)
+        wav = self.pad_wav(wav)
+        return self.model.encode(wav[:, None], self._features(wav, True))
+
+    @torch.no_grad()
+    def detokenize(self, acoustic_codes, semantic_codes, token_lengths=None):
+        """audio_tokenizer.py:83-86"""
+        return self.model.decode(acoustic_codes, semantic_codes, token_lengths)
