@@ -276,6 +276,14 @@ int qb_lm_decode_layer_tc(float* x, int64_t B, int32_t hidden, int32_t heads, in
                           const qb_half* wo, const qb_half* wgate, const qb_half* wup, const qb_half* wdown,
                           float* k_cache, float* v_cache, int32_t Lmax, const int32_t* pos, const float* rope_cos,
                           const float* rope_sin, float* q_buf, float* attn_buf, float* mlp_buf, void* stream);
+/* qb_lm_decode_layer_tc with one position per row: `pos` points at B device ints; row b's RoPE angle and K/V append use
+ * pos[b] and its attention reads keys 0..pos[b].  Serves llm_sft.py:155-191 when the rows' conditioning prefixes
+ * (llm_sft.py:108-122: task, enroll_sos, enrollment, mix_sos, mix) differ in length, i.e. target-speaker extraction over
+ * utterances whose enrollments differ in length. */
+int qb_lm_decode_layer_tc_rows(float* x, int64_t B, int32_t hidden, int32_t heads, int32_t inter, const qb_half* wqkv,
+                               const qb_half* wo, const qb_half* wgate, const qb_half* wup, const qb_half* wdown,
+                               float* k_cache, float* v_cache, int32_t Lmax, const int32_t* pos, const float* rope_cos,
+                               const float* rope_sin, float* q_buf, float* attn_buf, float* mlp_buf, void* stream);
 /* Keys whose K / V rows one lane of the cached-decode attention keeps in flight per trip: 8 (default; a single decode chain is
  * latency-bound) or 4 (several chains sharing the GPU are throughput-bound - LLM_SFT.generate's lanes select it).  Process-wide;
  * read at launch (and therefore fixed inside a captured graph).  Tokens do not depend on it only up to the fp32 summation order of
@@ -289,6 +297,11 @@ int qb_lm_set_att_unroll(int32_t keys_per_lane);
 int qb_lm_head_argmax_tc(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
                          int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride,
                          int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx, void* stream);
+/* qb_lm_head_argmax_tc with one position per row (`pos`: B device ints, each bumped once per step); the decode step of
+ * qb_lm_decode_layer_tc_rows (llm_sft.py:155-191, llm.py:286-287 over rows with prefixes of different lengths). */
+int qb_lm_head_argmax_tc_rows(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
+                              int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride,
+                              int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx, void* stream);
 
 /* Teacher-forced loss + accuracy (CustomLlamaModel.loss_function, QuarkAudio-UniSE/model/llm/llm.py:87-104): label-smoothed KL
  * (reduction batchmean) of log_softmax(logits [M, ld >= V]) against the smoothed one-hot targets [M] int64, and the arg-max
@@ -307,6 +320,13 @@ int qb_lm_head_sample_tc(const float* x, int64_t B, int32_t hidden, const qb_hal
                          int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride,
                          int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx, float* logits,
                          float temperature, int32_t top_k, float top_p, const uint32_t* seed, float* debug, void* stream);
+/* qb_lm_head_sample_tc with one position per row (`pos`: B device ints, each bumped once per step); the sampled decode step
+ * (llm_sft.py:155-161,184-190, llm.py:253-289) over rows with prefixes of different lengths.  The Philox counter is the same
+ * {step, row, call}: a row draws the same uniforms whatever the positions are. */
+int qb_lm_head_sample_tc_rows(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
+                              int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride,
+                              int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx, float* logits,
+                              float temperature, int32_t top_k, float top_p, const uint32_t* seed, float* debug, void* stream);
 
 /* ---------------------------------------------------------------- SSL feature front ends + tokenizer glue (SURVEY 8f.2 / 8f.3)
  * HuBERT-base / WavLM-base-plus (transformers modeling_hubert / modeling_wavlm) as the reference drives them from

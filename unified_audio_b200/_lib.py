@@ -101,6 +101,9 @@ SIGNATURES = {
                                         _vp, _vp, _vp, _vp]),
     "qb_lm_set_att_unroll": (C.c_int, [_i32]),
     "qb_lm_head_argmax_tc": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "qb_lm_decode_layer_tc_rows": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp,
+                                             _vp, _vp, _vp, _vp]),
+    "qb_lm_head_argmax_tc_rows": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "qb_ssl_conv0_workspace_bytes": (C.c_int64, [_i64, _i64, _i32]),
     "qb_ssl_conv0_gn_gelu": (C.c_int, [_vp, _i64, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "qb_ssl_conv0_bias": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
@@ -151,6 +154,8 @@ SIGNATURES = {
     "qb_lm_loss": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _f32, _vp, _vp, _vp]),
     "qb_lm_head_sample_tc": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _i32,
                                        _f32, _vp, _vp, _vp]),
+    "qb_lm_head_sample_tc_rows": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _f32,
+                                            _i32, _f32, _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -210,14 +210,15 @@ class LLM_SFT(_Face):
             cache.length = pos0 + L
             cache.pos.fill_(cache.length)
 
-    def _decode_layers(self, x: torch.Tensor, B: int, cache: StaticKVCache):
+    def _decode_layers(self, x: torch.Tensor, B: int, cache: StaticKVCache, row_pos: Optional[torch.Tensor] = None):
+        """row_pos: int32 [B] device positions, one per row (prefixes of different lengths); None = the cache's shared position"""
         W = self._prepare()
         ops.lm_set_att_unroll(self.att_unroll)
         H, heads, inter = self.hidden, self.heads, 4 * self.hidden
         qb, ab, mb = self._buf("dq", (B, H)), self._buf("da", (B, H)), self._buf("dm", (B, inter))
+        layer, pos = (ops.lm_decode_layer_tc, cache.pos) if row_pos is None else (ops.lm_decode_layer_tc_rows, row_pos)
         for i, Lw in enumerate(W["layers"]):
-            ops.lm_decode_layer_tc(x, B, H, heads, inter, Lw, cache.k[i], cache.v[i], cache.Lmax, cache.pos, W["cos"], W["sin"],
-                                   qb, ab, mb)
+            layer(x, B, H, heads, inter, Lw, cache.k[i], cache.v[i], cache.Lmax, pos, W["cos"], W["sin"], qb, ab, mb)
 
     @torch.no_grad()
     def llm_forward(self, inputs_embeds, attention_mask=None, past_key_values: Optional[StaticKVCache] = None,
@@ -271,7 +272,12 @@ class LLM_SFT(_Face):
                  out_f32=rowmap(out, self.hidden, B * T, 0))
         return out.reshape(B, T, self.hidden)
 
-    def _prefix(self, task_name, enroll_feats, mix_feats):
+    def _prefix(self, task_name, enroll_feats, mix_feats, enroll_lengths=None):
+        """[B, P, hidden]: task, (enroll_sos, adapter(enroll)), mix_sos, adapter(mix).  With `enroll_lengths` (host ints, one per row
+        of a right-padded enroll_feats) row b keeps only its first enroll_lengths[b] enrollment frames, so that its own prefix of
+        P_b = 3 + enroll_lengths[b] + T_mix positions has no padding inside it; zero rows fill positions P_b..P, P = the padded width."""
+        if enroll_lengths is not None:
+            return self._ragged_prefix(self._prefix(task_name, enroll_feats, mix_feats), enroll_lengths, enroll_feats.shape[1])
         B = mix_feats.shape[0]
         e = lambda w: w.detach().float()
         task = e(self.task_embedding.weight)[self.task_map[task_name]][None, None].expand(B, 1, -1)
@@ -281,6 +287,18 @@ class LLM_SFT(_Face):
             parts += [e(self.enroll_sos_embedding.weight)[0][None, None].expand(B, 1, -1), self._adapter(enroll_feats)]
         parts += [mix_sos, self._adapter(mix_feats)]
         return torch.cat(parts, 1)
+
+    @staticmethod
+    def _ragged_prefix(prefix, lengths, te_max):
+        """uniform prefix [B, P, H] = task, enroll_sos, enroll (te_max), mix_sos, mix -> row b moves its mix_sos + mix up to
+        right after its own lengths[b] enrollment frames; the positions after them gather a zero row"""
+        B, P, H = prefix.shape
+        idx = torch.full((B, P), P, dtype=torch.long)
+        for b, n in enumerate(lengths):
+            idx[b, :2 + n] = torch.arange(2 + n)
+            idx[b, 2 + n:P - (te_max - n)] = torch.arange(2 + te_max, P)
+        z = torch.cat([prefix, prefix.new_zeros(B, 1, H)], 1)
+        return torch.gather(z, 1, idx.to(prefix.device)[..., None].expand(B, P, H))
 
     # ------------------------------------------------------------------ teacher-forced forward (llm_sft.py:37-89)
     @torch.no_grad()
@@ -314,11 +332,19 @@ class LLM_SFT(_Face):
     @torch.no_grad()
     def generate(self, task_name, enroll_mel, enroll_feats, mix_mel, mix_feats, global_length: int = 32,
                  temperature: float = 0.8, top_k: int = 50, top_p: float = 0.95, do_sample: bool = True,
-                 use_cuda_graph: bool = True, seed: Optional[int] = None):
+                 use_cuda_graph: bool = True, seed: Optional[int] = None, enroll_lengths=None):
         """llm_sft.py:93-195 with the reference's signature and defaults.  do_sample=True draws every token on the device
         (top-k -> top-p -> temperature -> multinomial, csrc/llm.cu lm_sample_embed_kernel); `seed` (default: torch's
         global generator) makes the draw reproducible.  Greedy decoding ignores temperature / top_k / top_p exactly as the
-        reference's arg-max does (filters never remove the arg-max, llm.py:263-287)."""
+        reference's arg-max does (filters never remove the arg-max, llm.py:263-287).
+
+        `enroll_lengths` (ints [B], tensor or sequence): the valid frames of each row of a right-padded enroll_feats [B, Te_max, F],
+        for rows whose enrollments differ in length.  Row b then decodes exactly as if it were generated alone with
+        enroll_feats[b, :enroll_lengths[b]]: its prefix holds no padding, the padding sits after its own P_b positions, and the decode
+        kernels keep one position per row (starting at P_b).  A causal prefill never lets a real position see the padded tail, and
+        decode writes position P_b + s before it reads it, so the tail is never read.  None keeps the uniform path."""
+        if enroll_lengths is not None:
+            enroll_lengths = self._check_enroll_lengths(enroll_lengths, enroll_mel, enroll_feats, mix_feats.shape[0])
         sampling = None
         if do_sample:
             if not (0.0 < temperature <= 1.0):
@@ -333,13 +359,14 @@ class LLM_SFT(_Face):
         starts = list(range(0, Ball, self.chunk))         # decode kernels keep <= 32 sequences' rows in registers
         n_lanes = min(self.lanes, len(starts))
         outs = []
+        lens = lambda sl: None if enroll_lengths is None else enroll_lengths[sl]
         if n_lanes <= 1:
             for ci, b0 in enumerate(starts):
                 sl = slice(b0, min(b0 + self.chunk, Ball))
                 if sampling is not None:
                     sampling["call"] = ci
                 outs.append(self._generate_chunk(task_name, None if enroll_mel is None else enroll_feats[sl], mix_feats[sl],
-                                                 semantic_length, global_length, use_cuda_graph, sampling))
+                                                 semantic_length, global_length, use_cuda_graph, sampling, lens(sl)))
         else:
             # chunk ci runs on lane ci % n_lanes: the host enqueues one chunk after the other, the device overlaps the lanes
             n_pos = 2 + mix_feats.shape[1] + (0 if enroll_mel is None else 1 + enroll_feats.shape[1]) + global_length + 1 + semantic_length
@@ -356,13 +383,24 @@ class LLM_SFT(_Face):
                     stream.wait_event(ready)             # the inputs were produced on the caller's stream
                 with torch.cuda.stream(stream):
                     outs.append(view._generate_chunk(task_name, None if enroll_mel is None else enroll_feats[sl], mix_feats[sl],
-                                                     semantic_length, global_length, use_cuda_graph, sampling))
+                                                     semantic_length, global_length, use_cuda_graph, sampling, lens(sl)))
             for _, stream in views[:n_lanes]:
                 cur.wait_stream(stream)
             for gi, si in outs:                           # allocated on a lane's stream, consumed on the caller's
                 gi.record_stream(cur)
                 si.record_stream(cur)
         return torch.cat([o[0] for o in outs], 0), torch.cat([o[1] for o in outs], 0)
+
+    @staticmethod
+    def _check_enroll_lengths(enroll_lengths, enroll_mel, enroll_feats, B):
+        """-> host list of B ints in 1..Te_max (read once: the prefix layout is built on the host)"""
+        if enroll_mel is None or enroll_feats is None:
+            raise ValueError("enroll_lengths needs an enrollment (enroll_mel and enroll_feats)")
+        lens = [int(n) for n in (enroll_lengths.tolist() if torch.is_tensor(enroll_lengths) else enroll_lengths)]
+        te_max = enroll_feats.shape[1]
+        if len(lens) != B or any(n < 1 or n > te_max for n in lens):
+            raise ValueError(f"enroll_lengths must hold {B} lengths in 1..{te_max} (the padded enrollment), got {lens}")
+        return lens
 
     def _lanes(self, n: int, n_positions: int):
         """Lane = (shallow view of this module with its own workspace, decode state and captured graphs; its own stream).  The
@@ -382,11 +420,15 @@ class LLM_SFT(_Face):
             lanes.append((v, torch.cuda.Stream(device=self._dev())))
         return lanes
 
-    def _generate_chunk(self, task_name, enroll_feats, mix_feats, semantic_length, global_length, use_graph, sampling=None):
+    def _generate_chunk(self, task_name, enroll_feats, mix_feats, semantic_length, global_length, use_graph, sampling=None,
+                        enroll_lengths=None):
+        """enroll_lengths: host ints, one per row (ragged prefixes), or None.  P below is the padded prefix width: with ragged rows it
+        is the same for every chunk of a call, so the chunks share one decode state and its captured graphs."""
         W = self._prepare()
         dev = mix_feats.device
-        prefix = self._prefix(task_name, enroll_feats, mix_feats)
+        prefix = self._prefix(task_name, enroll_feats, mix_feats, enroll_lengths)
         B, P, H = prefix.shape
+        ragged = enroll_lengths is not None
         n_steps = global_length + 1 + semantic_length
         Lmax = -(-(P + n_steps) // 64) * 64
         self._ensure_rope(P + n_steps)
@@ -395,7 +437,7 @@ class LLM_SFT(_Face):
         samp_key = None if sampling is None else (sampling["temperature"], sampling["top_k"], sampling["top_p"])
         # Decode state (KV cache, counters, output ids) and the captured graphs are kept per shape: capturing and
         # instantiating ~560 kernel nodes costs the host 10-50 ms, as much as the whole generation takes on the device.
-        key = (B, P, n_steps, bool(use_graph), int(self.graph_steps), str(dev), samp_key)
+        key = (B, P, n_steps, bool(use_graph), int(self.graph_steps), str(dev), samp_key, ragged)
         st = self._gen_state.get(key)
         if st is None:
             self._gen_state.clear()                    # one shape at a time (the cache is ~0.9 GB at B=32)
@@ -406,7 +448,8 @@ class LLM_SFT(_Face):
                       pv=torch.zeros(max_cols // 16 + 1, 32, device=dev),
                       pi=torch.zeros(max_cols // 16 + 1, 32, dtype=torch.int32, device=dev), g1=None, gk=None, captured=False,
                       logits=torch.zeros(B, max_cols, device=dev) if sampling is not None else None,
-                      seed=torch.zeros(4, dtype=torch.int32, device=dev), dbg=torch.zeros(B, 4, device=dev))
+                      seed=torch.zeros(4, dtype=torch.int32, device=dev), dbg=torch.zeros(B, 4, device=dev),
+                      row_pos=torch.zeros(B, dtype=torch.int32, device=dev) if ragged else None)
             self._gen_state[key] = st
         cache, xs, rng, slot, out_ids, pv, pi = (st[k] for k in ("cache", "xs", "rng", "slot", "out_ids", "pv", "pi"))
         cache.length = 0
@@ -420,16 +463,27 @@ class LLM_SFT(_Face):
         rng.copy_(torch.tensor([self.global_offset, self.global_offset + self.global_size], dtype=torch.int32), non_blocking=True)
         x = prefix.reshape(B * P, H).contiguous().clone()
         self._prefill(x, B, P, cache)
+        row_pos = st["row_pos"]
+        start = None if row_pos is None else torch.tensor([3 + n + mix_feats.shape[1] for n in enroll_lengths], dtype=torch.int32)
+
+        def reset_pos():            # the first decode step of row b writes position P_b (P for every row without ragged prefixes)
+            if row_pos is None:
+                cache.pos.fill_(cache.length)
+            else:
+                row_pos.copy_(start, non_blocking=True)
+        if row_pos is not None:     # (_prefill has set the shared position)
+            reset_pos()
+        pos = cache.pos if row_pos is None else row_pos
+        sample = ops.lm_head_sample_tc if row_pos is None else ops.lm_head_sample_tc_rows
+        argmax = ops.lm_head_argmax_tc if row_pos is None else ops.lm_head_argmax_tc_rows
 
         def step():
-            self._decode_layers(xs, B, cache)
+            self._decode_layers(xs, B, cache, row_pos)
             if sampling is not None:
-                ops.lm_head_sample_tc(xs, B, H, W["head_p"], rng, max_cols, W["emb"], xs, out_ids, n_steps, cache.pos, slot, pv, pi,
-                                      st["logits"], sampling["temperature"], sampling["top_k"], sampling["top_p"], st["seed"],
-                                      st["dbg"])
+                sample(xs, B, H, W["head_p"], rng, max_cols, W["emb"], xs, out_ids, n_steps, pos, slot, pv, pi, st["logits"],
+                       sampling["temperature"], sampling["top_k"], sampling["top_p"], st["seed"], st["dbg"])
             else:
-                ops.lm_head_argmax_tc(xs, B, H, W["head_p"], rng, max_cols, W["emb"], xs, out_ids, n_steps, cache.pos, slot,
-                                      pv, pi)
+                argmax(xs, B, H, W["head_p"], rng, max_cols, W["emb"], xs, out_ids, n_steps, pos, slot, pv, pi)
 
         # All decode state is on the device, so a graph may hold any number of consecutive steps: one single-step graph
         # plus one of `graph_steps` steps (fewer replays per generation).
@@ -448,7 +502,7 @@ class LLM_SFT(_Face):
                     for _ in range(K):
                         step()
             st["captured"] = True
-            cache.pos.fill_(cache.length)
+            reset_pos()
             slot.zero_()
         g1, gk = (st["g1"], st["gk"]) if use_graph else (None, None)
 

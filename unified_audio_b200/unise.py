@@ -31,6 +31,10 @@ from .ssl import wrap_segments
 
 STFT_CONFIG = dict(hop_length=320, win_length=640, n_fft=640, n_mels=80)      # U/conf/config.yaml:124-128
 SEG_LEN = 5 * 16000                                                            # model.py:175
+# 5 s segments that go through WavLM / generate / detokenize together in Model.enhance_batch.  The faces keep their scratch buffers
+# per shape, and at shipped widths 128 segments per call ran out of an 80 GB H100 (in the BiCodec decoder's buffers); 32 is one LM
+# decode chunk.  Measured peak device memory: README (scripts/unise_enhance_bench.py).
+MAX_SEGMENTS = 32
 
 
 class BiCodecTokenizer(nn.Module):
@@ -212,13 +216,21 @@ class Model(nn.Module):
         return wrap_segments(src.float().contiguous(), SEG_LEN)          # np.pad(..., 'wrap') + reshape(-1, seg_len) on the device
 
     def _generate(self, task, enroll_feats, seg_src, do_sample, **gen_kw):
-        mix_mel = self.mel_like(seg_src)
-        mix_feats = self.extract_semantic_features(seg_src)
-        enroll_mel = None
         if enroll_feats is not None:                                    # torch.cat([enroll] * n_segments) (model.py:207-208)
             n = seg_src.size(0)
             enroll_feats = torch.cat([enroll_feats for _ in range(n)], 0)
+        return self._generate_rows(task, enroll_feats, None, seg_src, do_sample, **gen_kw)
+
+    def _generate_rows(self, task, enroll_feats, enroll_lengths, seg_src, do_sample, **gen_kw):
+        """WavLM features of the segments, then generate with one enrollment row per segment (right-padded to the longest when
+        `enroll_lengths` is given)"""
+        mix_mel = self.mel_like(seg_src)
+        mix_feats = self.extract_semantic_features(seg_src)
+        enroll_mel = None
+        if enroll_feats is not None:
             enroll_mel = mix_mel            # placeholder: only `is None` is tested for the enrollment mel (llm_sft.py:110-121)
+        if enroll_lengths is not None:
+            gen_kw = dict(gen_kw, enroll_lengths=enroll_lengths)
         gids, sids = self.dnn.generate(task_name=task, enroll_mel=enroll_mel, enroll_feats=enroll_feats, mix_mel=mix_mel,
                                        mix_feats=mix_feats, do_sample=do_sample, **gen_kw)
         return gids, sids
@@ -267,12 +279,125 @@ class Model(nn.Module):
             return est1, est2
         raise ValueError(f"unknown mode {mode!r} (the reference's test_step handles 'se', 'tse', 'ss')")
 
+    # ------------------------------------------------------------------ batched inference: many utterances per call
+    @torch.no_grad()
+    def enhance_batch(self, mode: str, enrolls, srcs, do_sample: bool = False, return_ids: bool = False,
+                      max_segments: int = MAX_SEGMENTS, **gen_kw):
+        """`enhance` over many utterances at once: srcs = list of [1, T_u] device tensors (any lengths), enrolls = list of [1, Te_u]
+        ('tse', any lengths) or None.  Returns a list with, for each utterance, what `enhance` returns for it alone.
+
+        Each utterance keeps its own wrap padding, its own 'se' peak normalisation and its own enrollment; their 5 s segments then
+        share the WavLM / generate / detokenize calls, at most `max_segments` segments per call.  In 'tse' each enrollment's WavLM
+        features are taken alone (WavLM's first GroupNorm spans time: padding would change them) and the LM prefixes differ in length
+        (generate's `enroll_lengths`).  Greedy tokens are those of `enhance` when the LM's decode attention keeps the same number of
+        keys in flight on both sides (LLM_SFT.att_unroll / lane_att_unroll; lanes only run when generate gets more than 32 rows).
+        With do_sample the draws differ from `enhance`'s: a row's uniforms depend on where it sits in the batch."""
+        srcs = list(srcs) if srcs is not None else []
+        if any(t is not None and t.device.type != "cuda" for t in srcs + list(enrolls or [])):
+            raise RuntimeError("unified_audio_b200.unise.Model runs on CUDA only (no CPU fallback)")
+        return self._enhance_batch(mode, enrolls, srcs, do_sample, return_ids, max_segments, **gen_kw)
+
+    @staticmethod
+    def _check_batch(mode, enrolls, srcs, max_segments):
+        if mode not in ("se", "tse", "ss"):
+            raise ValueError(f"unknown mode {mode!r} (the reference's test_step handles 'se', 'tse', 'ss')")
+        if not srcs:
+            raise ValueError("enhance_batch: no utterance")
+        if any(s.ndim != 2 or s.shape[0] != 1 or s.shape[1] < 1 for s in srcs):
+            raise ValueError(f"enhance_batch: every src must be [1, T], got {[tuple(s.shape) for s in srcs]}")
+        if mode == "tse" and enrolls is None:
+            raise ValueError("'tse' needs one enrollment per utterance")
+        if enrolls is not None:
+            enrolls = list(enrolls)
+            if len(enrolls) != len(srcs):
+                raise ValueError(f"{len(enrolls)} enrollments for {len(srcs)} utterances")
+            if mode == "tse" and any(e.ndim != 2 or e.shape[0] != 1 or e.shape[1] < 1 for e in enrolls):
+                raise ValueError(f"enhance_batch: every enrollment must be [1, Te], got {[tuple(e.shape) for e in enrolls]}")
+        if max_segments < 1:
+            raise ValueError(f"max_segments must be >= 1, got {max_segments}")
+        return enrolls
+
+    def _enhance_batch(self, mode, enrolls, srcs, do_sample=False, return_ids=False, max_segments=MAX_SEGMENTS, **gen_kw):
+        """_enhance's control flow per mode (model.py:174-286), applied per utterance, with the segments of all utterances batched;
+        pinned against the reference's `test_step` fixture and against `_enhance` (tests/test_unise_batch_host.py)."""
+        enrolls = self._check_batch(mode, enrolls, srcs, max_segments)
+        lens = [s.size(-1) for s in srcs]
+        segs = [self._segments(s) for s in srcs]
+        rows = [0]
+        for sg in segs:
+            rows.append(rows[-1] + sg.size(0))
+        cut = lambda x, u: x[rows[u]:rows[u + 1]]
+        trim = lambda est, u: cut(est, u).reshape(-1)[:lens[u]]
+        if mode == "se":                                                 # model.py:174-193, per utterance its own peak
+            seg = torch.cat([sg / s.abs().max(dim=-1, keepdim=True)[0] for sg, s in zip(segs, srcs)], 0)
+            est, gids, sids = self._run_segments("se", None, None, seg, do_sample, max_segments, **gen_kw)
+            return [(trim(est, u), cut(gids, u), cut(sids, u)) if return_ids else trim(est, u) for u in range(len(srcs))]
+        if mode == "tse":                                                # model.py:197-224
+            feats = [self.extract_semantic_features(e) for e in enrolls]          # each enrollment alone
+            te = [f.size(1) for f in feats]
+            pad = feats[0].new_zeros(1, max(te), feats[0].size(2))
+            per_row = [torch.cat([f, pad[:, :max(te) - f.size(1)]], 1) for f in feats]
+            ef = torch.cat([per_row[u] for u in range(len(srcs)) for _ in range(rows[u + 1] - rows[u])], 0)
+            el = [te[u] for u in range(len(srcs)) for _ in range(rows[u + 1] - rows[u])]
+            est, gids, sids = self._run_segments("tse", ef, el, torch.cat(segs, 0), do_sample, max_segments, **gen_kw)
+            return [(trim(est, u), cut(gids, u), cut(sids, u)) if return_ids else trim(est, u) for u in range(len(srcs))]
+        # 'ss', model.py:225-286: se on each utterance's first 5 s, then tse and rtse with that as the enrollment
+        first = torch.cat([s[:, :SEG_LEN] if n > SEG_LEN else sg[:1] for s, sg, n in zip(srcs, segs, lens)], 0)
+        enr = self._run_segments("se", None, None, first, do_sample, max_segments, **gen_kw)[0][:, :SEG_LEN]
+        enr = enr / (torch.amax(torch.abs(enr), dim=-1, keepdim=True) + 1e-5) * 0.99       # each utterance by its own peak
+        ef = self.extract_semantic_features(enr)
+        ef = torch.cat([ef[u:u + 1] for u in range(len(srcs)) for _ in range(rows[u + 1] - rows[u])], 0)
+        seg = torch.cat(segs, 0)
+        est1, _, _ = self._run_segments("tse", ef, None, seg, do_sample, max_segments, **gen_kw)
+        est2, _, _ = self._run_segments("rtse", ef, None, seg, do_sample, max_segments, **gen_kw)
+        return [(trim(est1, u), trim(est2, u)) for u in range(len(srcs))]
+
+    def _run_segments(self, task, enroll_feats, enroll_lengths, seg, do_sample, max_segments, **gen_kw):
+        """seg [S, SEG_LEN] (+ one enrollment row per segment) -> detokenized [S, SEG_LEN], global ids [S, 32], semantic ids [S, T],
+        at most max_segments segments per WavLM / generate / detokenize call"""
+        est, gids, sids = [], [], []
+        for s0 in range(0, seg.size(0), max_segments):
+            sl = slice(s0, s0 + max_segments)
+            g, s = self._generate_rows(task, None if enroll_feats is None else enroll_feats[sl],
+                                       None if enroll_lengths is None else enroll_lengths[sl], seg[sl], do_sample, **gen_kw)
+            est.append(self.tokenizer.detokenize(g.unsqueeze(1), s).squeeze(1))
+            gids.append(g)
+            sids.append(s)
+        if len(est) == 1:
+            return est[0], gids[0], sids[0]
+        return torch.cat(est, 0), torch.cat(gids, 0), torch.cat(sids, 0)
+
+    def test_epoch(self, batches, max_segments: int = MAX_SEGMENTS):
+        """test_step over many batches, with consecutive batches of the same mode enhanced together (`enhance_batch`, at most
+        max_segments 5 s segments per call).  Returns, and writes under `save_enhanced`, exactly what test_step returns and writes
+        for each batch, in order."""
+        batches = list(batches)
+        out, i = [], 0
+        while i < len(batches):
+            mode, j, n_seg = batches[i][0], i, 0
+            while j < len(batches) and batches[j][0] == mode and (j == i or n_seg + self._n_segments(batches[j][2]) <= max_segments):
+                n_seg += self._n_segments(batches[j][2])
+                j += 1
+            group = batches[i:j]
+            ests = self.enhance_batch(mode, [b[1] for b in group] if mode == "tse" else None, [b[2] for b in group],
+                                      do_sample=False, max_segments=max_segments)
+            out += [self._test_output(b, e) for b, e in zip(group, ests)]
+            i = j
+        return out
+
+    @staticmethod
+    def _n_segments(src):
+        return -(-src.size(-1) // SEG_LEN)
+
     def test_step(self, batch, batch_idx=0):
         """model.py:170-286: batch = (mode, enroll, src, tgt, fs, lengths, names); greedy decoding (do_sample = False, model.py:173).
         Returns the enhanced waveform(s) as NumPy (the reference's last step before its optional sf.write) and writes
         `<save_enhanced>/<name>.wav` (`_s1` / `_s2` for 'ss') when the config asks for it."""
         mode, enroll, src, tgt, fs, lengths, names = batch
-        out = self.enhance(mode, enroll, src, do_sample=False)
+        return self._test_output(batch, self.enhance(mode, enroll, src, do_sample=False))
+
+    def _test_output(self, batch, out):
+        mode, enroll, src, tgt, fs, lengths, names = batch
         outs = out if isinstance(out, tuple) else (out,)
         arrays = [o.cpu().numpy() for o in outs]
         save_dir = self.config.get("save_enhanced")
