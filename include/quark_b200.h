@@ -186,19 +186,11 @@ int qb_dwconv(const float* x, const float* w, const float* bias, int64_t B, int6
               float* out, void* stream);
 
 /* ---------------------------------------------------------------- sequence ops */
-/* Non-causal multi-head attention with RoPE applied to q,k on load
- * (encoder_modules/transformer.py:134-182).  qkv [B,T,3*H*D] fp32 (q|k|v), D = 64.  Output planes. */
-int qb_attention(const float* qkv, int64_t B, int64_t T, int32_t heads, const float* rope_cos,
-                 const float* rope_sin, qb_half* out_hi, qb_half* out_lo, void* stream);
-/* fp32 SIMT attention for head_dim 64 or 96 (H-Codec-1.0's decoder transformer: 768 / 8 heads). */
+/* Non-causal multi-head attention with RoPE applied to q,k on load (encoder_modules/transformer.py:134-182), fp32 SIMT:
+ * qkv [B,T,3*H*D] fp32 (q|k|v), head_dim D 64, 96 or 128.  Output planes.  The product runs head_dim 96 here (H-Codec-1.0's
+ * decoder transformer: 768 / 8 heads); 64 and 128 go to qb_attention_umma. */
 int qb_attention_hd(const float* qkv, int64_t B, int64_t T, int32_t heads, int32_t head_dim, const float* rope_cos,
                     const float* rope_sin, qb_half* out_hi, qb_half* out_lo, void* stream);
-/* Same attention on the tensor cores (mma.sync m16n8k16): q,k,v rounded to fp16 after RoPE, fp32
- * softmax / accumulation - the single-pass fp16 precision class.  workspace:
- * qb_attention_tc_workspace_bytes(B,T,heads). */
-int64_t qb_attention_tc_workspace_bytes(int64_t B, int64_t T, int32_t heads);
-int qb_attention_tc(const float* qkv, int64_t B, int64_t T, int32_t heads, const float* rope_cos,
-                    const float* rope_sin, qb_half* out_hi, qb_half* out_lo, void* workspace, void* stream);
 /* The same attention on the Hopper tensor cores (wgmma, accumulators in registers, TMA-fed operands; csrc/attention_umma.cu):
  * head_dim 64 or 128, any L; split = 0: single-pass fp16 operands, split = 1: fp16 hi + lo operands for both contractions (3 passes,
  * fp32-grade); causal = 1: query t attends keys <= t (the AR-LM's teacher-forced / prefill attention, U/model/llm/llm.py:195-216).

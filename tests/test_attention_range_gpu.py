@@ -316,41 +316,6 @@ def test_attention_relbias_range(lib, pattern):
         _report(f"attention_relbias {pattern} L={L}", None, got, ref, bound, S, mask, L)
 
 
-# ---------------------------------------------------------------------------------------------- mma.sync attention (QB_ATTENTION=legacy)
-@pytest.mark.parametrize("pattern", PLANTED)
-def test_attention_tc_range(lib, pattern):
-    """qkv_prep_kernel + flash_attn_kernel, single-pass fp16 operands, on the planted (fp16-exact) cases"""
-    from unified_audio_b200 import ops
-
-    def run(qkv, L, cos, sin):
-        ws = torch.zeros(ops.attention_tc_workspace_bytes(B, L, H), dtype=torch.uint8, device=DEV)
-        buf = _out_buf(B * L, H * 64)
-        ops.attention_tc(qkv, B, L, H, cos, sin, _planes(buf, B * L), ws)
-        return _collect("attention_tc", buf, B * L), False
-
-    _self_attention_cases(pattern, 64, "single", False, run, "attention_tc")
-
-
-@pytest.mark.parametrize("L", [37, 131])
-def test_attention_tc_dirty_workspace(lib, L):
-    """attention_tc's workspace holds nothing but the three operand planes its prep launch writes: 0xFF bytes or zeros, same bits"""
-    from unified_audio_b200 import ops
-    qt, k, v = _plant("ramp_noise", L, L, 64, 9 + L)
-    qkv = _pack(qt * 8.0, k, v)
-    cos, sin = ops.rope_tables(L, 64, DEV)
-    n = ops.attention_tc_workspace_bytes(B, L, H)
-    outs = []
-    for fill in (0xFF, 0):
-        ws = torch.full((n + 256,), fill, dtype=torch.uint8, device=DEV)
-        buf = _out_buf(B * L, H * 64)
-        ops.attention_tc(qkv, B, L, H, cos, sin, _planes(buf, B * L), ws[:n])
-        got = _collect("attention_tc", buf, B * L)
-        assert bool(torch.isfinite(got).all()), f"fill {fill:#x}: non-finite output"
-        assert bool((ws[n:] == fill).all()), "workspace written past qb_attention_tc_workspace_bytes"
-        outs.append(buf.clone())
-    assert torch.equal(outs[0], outs[1]), "the output depends on stale workspace bytes"
-
-
 # ---------------------------------------------------------------------------------------------- LM continuation prefill
 @pytest.mark.parametrize("pattern", PLANTED + ["causal", "wide"])
 @pytest.mark.parametrize("pos0", [0, 37, 64])

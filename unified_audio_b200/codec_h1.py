@@ -17,7 +17,6 @@ stream, from weights repacked here at first use.  `CodecH15` (codec_h15.py) buil
 from __future__ import annotations
 
 import math
-import os
 from typing import Dict
 
 import torch
@@ -271,11 +270,7 @@ class CodecH1(_CodecFace):
         ws = self._buf("lstm_ws", (max(ops.lstm_workspace_bytes(B, C), ops.lstm_tc_workspace_bytes(B, C)),), torch.uint8)
         lstm_u = ops.lstm_tc_units(C) if use_tc else 0
         cos, sin = self._cached(("rope", F, hd), lambda: ops.rope_tables(F, hd, self._dev()))
-        legacy = os.environ.get("QB_ATTENTION", "umma") == "legacy"
-        umma = (not legacy) and hd in (64, 128)          # wgmma attention (csrc/attention_umma.cu), both precision policies
-        tc_att = (not umma) and (not pa) and hd == 64
-        att_ws = (self._buf("att5_ws", (ops.attention_umma_workspace_bytes(B, F, heads, hd, pa),), torch.uint8) if umma else
-                  self._buf("att_ws", (ops.attention_tc_workspace_bytes(B, F, heads),), torch.uint8) if tc_att else None)
+        att_ws = self._buf("att5_ws", (ops.self_attention_workspace_bytes(B, F, heads, hd, pa),), torch.uint8)
         xm = rowmap(x, C, M, 0)
         for L in layers:
             ops.rmsnorm(x, L["in_w"], M, C, t_a)
@@ -285,12 +280,7 @@ class CodecH1(_CodecFace):
             else:
                 ops.lstm(xp, L["whh"], B, F, C, t_b, ws)
             self._linear(t_b, L["wqkv"], 3 * C, M, C, bias=L["bqkv"], out_f32=rowmap(qkv, 3 * C, M, 0))
-            if umma:
-                ops.attention_umma(qkv, B, F, heads, hd, cos, sin, t_a, att_ws, split=pa)
-            elif tc_att:   # legacy: single-pass fp16 policy, head_dim 64: mma.sync flash attention
-                ops.attention_tc(qkv, B, F, heads, cos, sin, t_a, att_ws)
-            else:        # split-precision policy or head_dim 96: fp32 SIMT attention
-                ops.attention_hd(qkv, B, F, heads, hd, cos, sin, t_a)
+            ops.self_attention(qkv, B, F, heads, hd, cos, sin, t_a, att_ws, pa)
             self._linear(t_a, L["wo"], C, M, C, residual=xm, out_f32=xm)
             ops.rmsnorm(x, L["post_w"], M, C, t_m)
             self._linear(t_m, L["w13"], 2 * I, M, C, act=ACT_SWIGLU, out_planes=hid, out_planes_map=(I, M, 0))

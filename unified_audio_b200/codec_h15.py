@@ -27,7 +27,6 @@ sizes the T + G sequences; decode reads the largest total length the same way (p
 from __future__ import annotations
 
 import math
-import os
 from typing import Dict
 
 import torch
@@ -153,20 +152,12 @@ class CodecH15(CodecH1):
         hid = self._planes("mm_hid", (M, FF), split)
         qkv = self._buf("mm_qkv", (M, 3 * C))
         cos, sin = self._cached(("rope_mimi", L, hd), lambda: self._rope_mimi(L, hd))
-        umma = hd in (64, 128) and os.environ.get("QB_ATTENTION", "umma") != "legacy"      # wgmma attention (csrc/attention_umma.cu)
-        tc_att = (not umma) and (not split) and hd == 64
-        att_ws = (self._buf("att5_ws", (ops.attention_umma_workspace_bytes(B, L, heads, hd, split),), torch.uint8) if umma else
-                  self._buf("att_ws", (ops.attention_tc_workspace_bytes(B, L, heads),), torch.uint8) if tc_att else None)
+        att_ws = self._buf("att5_ws", (ops.self_attention_workspace_bytes(B, L, heads, hd, split),), torch.uint8)
         xm = rowmap(x, C, M, 0)
         for i, Lw in enumerate(layers):
             ops.layernorm(x, Lw["n1w"], Lw["n1b"], 1, M, C, eps=1e-5, out=t_a)
             self._linear(t_a, Lw["wqkv"], 3 * C, M, C, out_f32=rowmap(qkv, 3 * C, M, 0))
-            if umma:
-                ops.attention_umma(qkv, B, L, heads, hd, cos, sin, t_b, att_ws)
-            elif tc_att:
-                ops.attention_tc(qkv, B, L, heads, cos, sin, t_b, att_ws)
-            else:
-                ops.attention_hd(qkv, B, L, heads, hd, cos, sin, t_b)
+            ops.self_attention(qkv, B, L, heads, hd, cos, sin, t_b, att_ws, split)
             self._linear(t_b, Lw["wo"], C, M, C, gamma=Lw["ls1"], residual=xm, out_f32=xm)
             ops.layernorm(x, Lw["n2w"], Lw["n2b"], 1, M, C, eps=1e-5, out=t_a)
             self._linear(t_a, Lw["w1"], FF, M, C, act=ACT_GELU, out_planes=hid, out_planes_map=(FF, M, 0))

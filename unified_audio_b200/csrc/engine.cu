@@ -508,7 +508,7 @@ static int run_transformer(qb_codec* c, const std::vector<TfLayerW>& layers, flo
   const bool pa = c->pol.lstm_attn;
   PlanesD t_a, t_b, t_m, hid;
   float *xp, *qkv;
-  void *lstm_ws, *att_ws = nullptr;
+  void *lstm_ws, *att_ws;
   QB_TRY(c->ws.planes(&t_a, "tf_a", (size_t)M * C, pa));
   QB_TRY(c->ws.planes(&t_b, "tf_b", (size_t)M * C, pa));
   QB_TRY(c->ws.planes(&t_m, "tf_m", (size_t)M * C, split_mlp));
@@ -516,12 +516,8 @@ static int run_transformer(qb_codec* c, const std::vector<TfLayerW>& layers, flo
   QB_TRY(c->ws.f32(&xp, "tf_xp", (size_t)M * 4 * C));
   QB_TRY(c->ws.f32(&qkv, "tf_qkv", (size_t)M * 3 * C));
   QB_TRY(c->ws.get(&lstm_ws, "lstm_ws", (size_t)qb_lstm_tc_workspace_bytes(B, C)));
-  // wgmma attention (attention_umma.cu) in both precision policies; QB_ATTENTION=legacy keeps the round-1 kernels (mma.sync flash
-  // attention for the single-pass policy, fp32 SIMT for the split one) for A/B runs
-  static const bool legacy = [] { const char* e = getenv("QB_ATTENTION"); return e && !strcmp(e, "legacy"); }();
-  const bool tc_att = legacy && !pa;
-  if (!legacy) QB_TRY(c->ws.get(&att_ws, "att5_ws", (size_t)qb_attention_umma_workspace_bytes(B, F, heads, hd, pa ? 1 : 0)));
-  else if (tc_att) QB_TRY(c->ws.get(&att_ws, "att_ws", (size_t)qb_attention_tc_workspace_bytes(B, F, heads)));
+  // wgmma attention (attention_umma.cu) in both precision policies
+  QB_TRY(c->ws.get(&att_ws, "att5_ws", (size_t)qb_attention_umma_workspace_bytes(B, F, heads, hd, pa ? 1 : 0)));
   const float *rc, *rs;
   QB_TRY(rope_tables(c, (int)F, hd, &rc, &rs));
   for (const TfLayerW& L : layers) {
@@ -529,9 +525,7 @@ static int run_transformer(qb_codec* c, const std::vector<TfLayerW>& layers, flo
     QB_TRY(lin(t_a, M, C, L.wih, 4 * C).bias(L.b_ih).out32(xp, 4 * C, M, 0).run(st));
     QB_TRY(qb_lstm_tc(xp, (const qb_half*)L.whh_perm, c->lstm_u, B, F, C, (qb_half*)t_b.hi, (qb_half*)t_b.lo, lstm_ws, st));
     QB_TRY(lin(t_b, M, C, L.wqkv, 3 * C).bias(L.bqkv).out32(qkv, 3 * C, M, 0).run(st));
-    if (!legacy) QB_TRY(qb_attention_umma(qkv, B, F, heads, hd, rc, rs, (qb_half*)t_a.hi, (qb_half*)t_a.lo, pa ? 1 : 0, 0, att_ws, st));
-    else if (tc_att) QB_TRY(qb_attention_tc(qkv, B, F, heads, rc, rs, (qb_half*)t_a.hi, (qb_half*)t_a.lo, att_ws, st));
-    else QB_TRY(qb_attention_hd(qkv, B, F, heads, hd, rc, rs, (qb_half*)t_a.hi, (qb_half*)t_a.lo, st));
+    QB_TRY(qb_attention_umma(qkv, B, F, heads, hd, rc, rs, (qb_half*)t_a.hi, (qb_half*)t_a.lo, pa ? 1 : 0, 0, att_ws, st));
     QB_TRY(lin(t_a, M, C, L.wo, C).residual(x, C, M, 0).out32(x, C, M, 0).run(st));
     QB_TRY(qb_rmsnorm(x, L.post_w, 1e-6f, M, C, nullptr, (qb_half*)t_m.hi, (qb_half*)t_m.lo, st));
     QB_TRY(lin(t_m, M, C, L.w13, 2 * I).act(QB_ACT_SWIGLU).outp(hid, I, M, 0).run(st));
@@ -1127,8 +1121,7 @@ static int lm_layers_prefill(qb_lm* m, float* x, int64_t B, int64_t L, qb_kv* kv
   QB_TRY(m->ws.f32(&qkv, "qkv", (size_t)M * 3 * H));
   QB_TRY(m->ws.f32(&q32, "q32", (size_t)M * H));
   // prefill from an empty cache: causal wgmma attention over the qkv rows (attention_umma.cu); a continuation reads the cache
-  static const bool legacy_att = [] { const char* e = getenv("QB_ATTENTION"); return e && !strcmp(e, "legacy"); }();
-  const bool umma = pos0 == 0 && !legacy_att;
+  const bool umma = pos0 == 0;
   void* att_ws = nullptr;
   if (umma) QB_TRY(m->ws.get(&att_ws, "att5_ws", (size_t)qb_attention_umma_workspace_bytes(B, L, heads, 64, 1)));
   for (int i = 0; i < m->cfg.layers; ++i) {

@@ -168,7 +168,7 @@ class LLM_SFT(_Face):
     # ------------------------------------------------------------------ transformer stack
     def _prefill(self, x: torch.Tensor, B: int, L: int, cache: StaticKVCache):
         """x [B*L, hidden] fp32, updated in place by the 12 layers; K/V written at cache.length..  cache None = a teacher-forced
-        forward that nobody will decode from: no KV cache is allocated or written (wgmma attention only)."""
+        forward that nobody will decode from: no KV cache is allocated or written."""
         W = self._prepare()
         H, heads, inter, M = self.hidden, self.heads, 4 * self.hidden, B * L
         pos0 = cache.length if cache is not None else 0
@@ -189,9 +189,7 @@ class LLM_SFT(_Face):
         # a prefill from an empty cache (every call of llm_forward / forward / generate) attends within its own L positions: the causal
         # wgmma attention (csrc/attention_umma.cu) reads the qkv GEMM's output directly; lm_qkv_prep still fills the fp32 KV cache for
         # the decode steps.  A continuation (pos0 > 0) keeps the cache-reading mma.sync kernel.
-        umma = pos0 == 0 and os.environ.get("QB_ATTENTION", "umma") != "legacy"
-        if cache is None and not umma:
-            raise RuntimeError("cache-less prefill needs the wgmma attention path")
+        umma = pos0 == 0
         att_ws = self._buf("att5_ws", (ops.attention_umma_workspace_bytes(B, L, heads, 64, True),), torch.uint8) if umma else None
         for i, Lw in enumerate(W["layers"]):
             ops.rmsnorm(x, Lw["in_w"], M, H, t1)
@@ -230,7 +228,7 @@ class LLM_SFT(_Face):
         W = self._prepare()
         B, L, H = inputs_embeds.shape
         cache = past_key_values
-        if cache is None and not use_cache and os.environ.get("QB_ATTENTION", "umma") != "legacy":
+        if cache is None and not use_cache:
             # teacher-forced forward (LLM_SFT.forward, llm_sft.py:93-135): nothing decodes from it, so no KV cache at all
             self._ensure_rope(L)
             x = inputs_embeds.float().reshape(B * L, H).contiguous().clone()

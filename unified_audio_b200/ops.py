@@ -230,20 +230,6 @@ def attention_hd(qkv, B, T, heads, head_dim, rope_cos, rope_sin, out: Planes):
                                            _stream()))
 
 
-def attention(qkv, B, T, heads, rope_cos, rope_sin, out: Planes):
-    _lib.check(_lib.load().qb_attention(_p(qkv), B, T, heads, _p(rope_cos), _p(rope_sin), _p(out.hi), _p(out.lo),
-                                        _stream()))
-
-
-def attention_tc_workspace_bytes(B, T, heads):
-    return int(_lib.load().qb_attention_tc_workspace_bytes(B, T, heads))
-
-
-def attention_tc(qkv, B, T, heads, rope_cos, rope_sin, out: Planes, workspace):
-    _lib.check(_lib.load().qb_attention_tc(_p(qkv), B, T, heads, _p(rope_cos), _p(rope_sin), _p(out.hi), _p(out.lo),
-                                           _p(workspace), _stream()))
-
-
 def attention_umma_workspace_bytes(B, L, heads, head_dim, split):
     return int(_lib.load().qb_attention_umma_workspace_bytes(B, L, heads, head_dim, int(bool(split))))
 
@@ -253,6 +239,30 @@ def attention_umma(qkv, B, L, heads, head_dim, rope_cos, rope_sin, out: Planes, 
     split = (out.lo is not None) if split is None else split
     _lib.check(_lib.load().qb_attention_umma(_p(qkv), B, L, heads, head_dim, _p(rope_cos), _p(rope_sin), _p(out.hi), _p(out.lo),
                                              int(bool(split)), int(bool(causal)), _p(workspace), _stream()))
+
+
+def self_attention_workspace_bytes(B, L, heads, head_dim, split):
+    """workspace of `self_attention`: the wgmma kernel's operand planes at head_dim 64 / 128, nothing for the SIMT kernel"""
+    return attention_umma_workspace_bytes(B, L, heads, head_dim, split) if head_dim in (64, 128) else 0
+
+
+def self_attention(qkv, B, L, heads, head_dim, rope_cos, rope_sin, out: Planes, workspace, split):
+    """Non-causal self-attention with RoPE: the wgmma kernel at head_dim 64 / 128 (split: fp16 hi + lo operands), the fp32 SIMT
+    kernel at any other head_dim.  The kernels are looked up in this module at each call, so a wrapper assigned to
+    `ops.attention_umma` / `ops.attention_hd` (bench.py counts attention FLOPs that way) sees every call."""
+    if head_dim in (64, 128):
+        attention_umma(qkv, B, L, heads, head_dim, rope_cos, rope_sin, out, workspace, split=split)
+    else:
+        attention_hd(qkv, B, L, heads, head_dim, rope_cos, rope_sin, out)
+
+
+# bench.py's H-Codec-1.5 FLOP counter wraps this name; it is the single-pass wgmma attention at head_dim 64, and no model calls it
+def attention_tc_workspace_bytes(B, T, heads):
+    return attention_umma_workspace_bytes(B, T, heads, 64, False)
+
+
+def attention_tc(qkv, B, T, heads, rope_cos, rope_sin, out: Planes, workspace):
+    attention_umma(qkv, B, T, heads, 64, rope_cos, rope_sin, out, workspace, split=False)
 
 
 def lstm_workspace_bytes(B, H):

@@ -33,7 +33,6 @@ XLSR-53 are loaded but never computed).  No PyTorch / CPU fallback.
 from __future__ import annotations
 
 import math
-import os
 from typing import Dict, Optional
 
 import torch
@@ -328,8 +327,7 @@ class SSLFrontEnd(_Face):
         t32 = self._buf("t32", (M, H))
         cos, sin = self._identity_rope(Tf, hd)
         wavlm = c.get("kind") == "wavlm"
-        umma = (not wavlm) and hd in (64, 128) and os.environ.get("QB_ATTENTION", "umma") != "legacy"
-        att_ws = self._buf("att5_ws", (ops.attention_umma_workspace_bytes(B, Tf, heads, hd, True),), torch.uint8) if umma else None
+        att_ws = None if wavlm else self._buf("att5_ws", (ops.self_attention_workspace_bytes(B, Tf, heads, hd, True),), torch.uint8)
         if wavlm:
             rel_table = self._cached(("rel", Tf), lambda: self._rel_table(Tf))
             gate = self._buf("gate", (B, heads, Tf))
@@ -339,10 +337,8 @@ class SSLFrontEnd(_Face):
             if wavlm:        # gated relative position bias from the layer INPUT (WavLMAttention.forward)
                 ops.wavlm_gate(xs, B, Tf, heads, hd, L["gru_w"], L["gru_b"], L["gru_c"], gate)
                 ops.attention_relbias(qkv, B, Tf, heads, hd, rel_table, gate, att)
-            elif umma:       # wgmma attention, split precision (csrc/attention_umma.cu)
-                ops.attention_umma(qkv, B, Tf, heads, hd, cos, sin, att, att_ws)
             else:
-                ops.attention_hd(qkv, B, Tf, heads, hd, cos, sin, att)
+                ops.self_attention(qkv, B, Tf, heads, hd, cos, sin, att, att_ws, True)
             ops.gemm(att, L["wo"], H, a_batch=1, a_rows_per_batch=M, a_ld=H, m_per_batch=M, bias=L["bo"],
                      residual=rowmap(xs, H, M, 0), out_f32=rowmap(t32, H, M, 0))
             ops.layernorm(t32, L["ln_w"], L["ln_b"], B, Tf, H, eps=c["eps"], out_f32=xs, out=xp)
@@ -409,16 +405,12 @@ class SSLFrontEnd(_Face):
         att = self._planes("att", (M, H))
         hid = self._planes("hid", (M, c["ffn"]))
         cos, sin = self._identity_rope(Tf, hd)
-        umma = hd in (64, 128) and os.environ.get("QB_ATTENTION", "umma") != "legacy"
-        att_ws = self._buf("att5_ws", (ops.attention_umma_workspace_bytes(B, Tf, heads, hd, True),), torch.uint8) if umma else None
+        att_ws = self._buf("att5_ws", (ops.self_attention_workspace_bytes(B, Tf, heads, hd, True),), torch.uint8)
         for li, L in enumerate(W["layers"]):                      # Wav2Vec2EncoderLayerStableLayerNorm; x <-> x2 ping-pong
             ops.layernorm(x, L["ln_w"], L["ln_b"], B, Tf, H, eps=c["eps"], out=xp)
             ops.gemm(xp, L["wqkv"], 3 * H, a_batch=1, a_rows_per_batch=M, a_ld=H, m_per_batch=M, bias=L["bqkv"],
                      out_f32=rowmap(qkv, 3 * H, M, 0))
-            if umma:
-                ops.attention_umma(qkv, B, Tf, heads, hd, cos, sin, att, att_ws)
-            else:
-                ops.attention_hd(qkv, B, Tf, heads, hd, cos, sin, att)
+            ops.self_attention(qkv, B, Tf, heads, hd, cos, sin, att, att_ws, True)
             ops.gemm(att, L["wo"], H, a_batch=1, a_rows_per_batch=M, a_ld=H, m_per_batch=M, bias=L["bo"],
                      residual=rowmap(x, H, M, 0), out_f32=rowmap(x2, H, M, 0))
             ops.layernorm(x2, L["fln_w"], L["fln_b"], B, Tf, H, eps=c["eps"], out=xp)
