@@ -210,7 +210,12 @@ __global__ void fsq_tokenize_kernel(const float* __restrict__ x, long long rows,
     for (int j = 0; j < 8; ++j)
       if (j < lv.n) acc[j] = fmaf(w_in[(long long)j * dim + c], v, acc[j]);
   }
-  float index = 0.f, basis = 1.f;
+  // The index is built in integers: sum_j (q_j + L_j / 2) * prod_{i<j} L_i, exact for any codebook up to 2^24 entries, and the
+  // index indices_to_level_indices() inverts.  The reference's float steps (codes_to_indices(): code = q / hw, then
+  // (code * hw + hw) * basis, truncated) give the same integer for every level up to 25, but only when each op is rounded on its
+  // own: contracted into FMAs, fl(-2/3) * 3 + 3 is 0.99999994 and truncation loses one (levels 6 and 7).  From level 26 on even
+  // the unfused terms stop being exact integers (fl(-7/13) * 13 + 13 = 5.9999995); the kernel still gives the exact index.
+  int index = 0, basis = 1;
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     if (j >= lv.n) break;
@@ -221,12 +226,10 @@ __global__ void fsq_tokenize_kernel(const float* __restrict__ x, long long rows,
     const float offset = (L % 2 == 0) ? 0.5f : 0.f;
     const float shift = atanhf(offset / half_l);
     const float q = rintf(tanhf(zj + shift) * half_l - offset);     // torch.round: half to even
-    const float hw = (float)(L / 2);
-    const float code = q / hw;                                      // quantize() -> codes_to_indices(), in the same float steps
-    index += (code * hw + hw) * basis;
-    basis *= (float)L;
+    index += ((int)q + L / 2) * basis;
+    basis *= L;
   }
-  if (lane == 0) idx[row] = (int32_t)index;
+  if (lane == 0) idx[row] = index;
 }
 
 }  // namespace qb
