@@ -22,16 +22,30 @@ def similarity_alignment(h: torch.Tensor, threshold: float, max_tokens_per_group
     if T <= 1:
         return torch.ones(B, 1, T), torch.ones(B, max(T - 1, 0)), torch.ones(B, dtype=torch.long)
     sim = F.cosine_similarity(h[:, :-1], h[:, 1:], dim=2)
+    seg, _, n_groups = segments_from_sim(sim, threshold, max_tokens_per_group)
+    G = int(n_groups.max())
+    align = torch.zeros(B, G, T)
+    align[torch.arange(B)[:, None].expand(B, T), seg, torch.arange(T)[None].expand(B, T)] = 1.0
+    return align, sim, n_groups
+
+
+def segments_from_sim(sim: torch.Tensor, threshold: float, max_tokens_per_group: int = 8):
+    """the grouping scan of similarity_alignment on given similarities sim [B,T-1] -> (frame -> token seg [B,T] int64,
+    frames per token lengths [B,T] int64 (0 past each clip's last token), n_groups [B] int64).  A frame opens a token when its
+    similarity to the previous frame is <= threshold or when the open token already holds max_tokens_per_group frames;
+    max_tokens_per_group <= 0 means no cap."""
+    B, T = sim.shape[0], sim.shape[1] + 1
     new_group = torch.cat([torch.ones(B, 1, dtype=torch.bool), sim <= threshold], 1)
     ar = torch.arange(T)[None]
     start = torch.cummax(ar * new_group.long(), dim=1).values               # index of the frame that opened the segment
-    split = ((ar - start) % max_tokens_per_group) == 0                      # similarity boundary or length cap
+    if max_tokens_per_group > 0:
+        split = ((ar - start) % max_tokens_per_group) == 0                  # similarity boundary or length cap
+    else:
+        split = new_group
     seg = torch.cumsum(split.long(), 1) - 1                                 # frame -> token
     n_groups = seg[:, -1] + 1
-    G = int(n_groups.max())
-    align = torch.zeros(B, G, T)
-    align[torch.arange(B)[:, None].expand(B, T), seg, ar.expand(B, T)] = 1.0
-    return align, sim, n_groups
+    lengths = torch.zeros(B, T, dtype=torch.long).scatter_add_(1, seg, torch.ones_like(seg))
+    return seg, lengths, n_groups
 
 
 def token_lengths(align: torch.Tensor) -> torch.Tensor:

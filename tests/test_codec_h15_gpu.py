@@ -175,3 +175,102 @@ def test_h15_bench_shape_vs_oracle(lib):
     e_wav = rel(rec, ref)
     print(f"[h15 bench shape] wav rel {e_wav:.2e}")
     assert rec.shape == ref.shape == (B, N * 640) and e_wav < TOL
+
+
+def _shallow_codec():
+    from oracle import hcodec15 as o15
+    from unified_audio_b200.codec_h15 import CodecH15
+    c = o15.h15_shallow()
+    sd = o15.make_state_dict(c, 11)
+    m = CodecH15(precision="mixed", _cfg={k: v for k, v in c.items() if k != "layer_scale"})
+    m.load_state_dict(sd, strict=True)
+    return c, sd, m.cuda()
+
+
+def _agg_taps(c):
+    last = c["agg"]["layers"] - 1
+    return [f"{a}.{k}" for a in ("sem_agg", "ac_agg") for k in ("interleaved", "layer0", f"layer{last}", "out")]
+
+
+def test_h15_one_frame_clips(lib):
+    """640 samples per clip (the shortest clip the tokenizer makes: it pads anything up to 640 samples to that) give one frame and
+    one token per clip: the frame -> token map handed to the aggregator kernels is int32 zeros, every tap matches the oracle, the
+    packed codes equal the oracle's and decode of them matches the oracle's decode.  The seed keeps every RVQ decision at least
+    5e-4 |token| from a tie."""
+    from oracle import hcodec15 as o15
+    from oracle.make_golden_h15 import synth
+    c, sd, m = _shallow_codec()
+    wav, feat = synth(c, 2, 1, 62)
+    assert wav.shape == (2, 1, 640)
+    otaps, gtaps = {}, {}
+    oa, osem = o15.codec_encode(sd, c, wav, feat, otaps)
+    out = m.encode(wav.cuda(), feat.cuda(), taps=gtaps)
+    torch.cuda.synchronize()
+    seg = gtaps["seg"]
+    assert seg.dtype == torch.int32 and tuple(seg.shape) == (2, 1) and not bool(seg.any())
+    assert gtaps["n_groups"].tolist() == [1, 1] and gtaps["token_lengths"].tolist() == [[1], [1]]
+    for k in ["enc.out", "sem.out"] + _agg_taps(c):
+        e = rel(gtaps[k], otaps[k])
+        print(f"  [h15 one frame] tap {k}: {e:.2e}")
+        assert e < TOL
+    assert torch.equal(out["acoustic_codes"].cpu(), oa) and torch.equal(out["semantic_codes"].cpu(), osem)
+    rec = m.decode(out["acoustic_codes"], out["semantic_codes"])
+    torch.cuda.synchronize()
+    ref = o15.codec_decode(sd, c, oa, osem)
+    e_wav = rel(rec, ref)
+    print(f"[h15 one frame] codes {oa[:, :, 0].tolist()}, wav rel {e_wav:.2e}")
+    assert rec.shape == ref.shape == (2, 640) and e_wav < TOL
+
+
+def _grouping_spread_inputs(c, N, seed):
+    """B = 3 clips of N frames whose features group very differently: clip 0 constant over time (its interior semantic frames are
+    identical and merge up to the cap), clip 1 random, clip 2 constant for the first half and random for the second"""
+    from oracle.make_golden_h15 import synth
+    wav, feat = synth(c, 3, N, seed)
+    g = torch.Generator().manual_seed(seed + 1)
+    T50 = 2 * N
+    col = torch.randn(c["sem_in"], 1, generator=g)
+    r = torch.randn(c["sem_in"], T50, generator=g)
+    feat[0] = (torch.sign(col) * col.abs() ** 0.3).expand(-1, T50)
+    feat[1] = torch.sign(r) * r.abs() ** 0.3
+    feat[2, :, : T50 // 2] = feat[0, :, : T50 // 2]
+    feat[2, :, T50 // 2:] = feat[1, :, T50 // 2:]
+    return wav, feat
+
+
+def test_h15_batch_with_padded_groups(lib):
+    """a batch whose clips have 3, 24 and about 14 tokens of 24 frames: the shorter clips carry padded groups (query rows that are
+    the bare embedding on the way in, zero tokens on the way out, length 0 packed as negative codes).  Grouping identical to the
+    oracle, every aggregator tap < 1e-3, the packed codes equal the oracle's (the seed keeps every RVQ decision of a live group at
+    least 1.8e-4 |token| from a tie, and every similarity 0.07 from the threshold) and decode of the oracle's codes < 1e-3."""
+    from oracle import adaptive as oad
+    from oracle import hcodec15 as o15
+    c, sd, m = _shallow_codec()
+    N = 24
+    wav, feat = _grouping_spread_inputs(c, N, 57)
+    otaps, gtaps = {}, {}
+    oa, osem = o15.codec_encode(sd, c, wav, feat, otaps)
+    out = m.encode(wav.cuda(), feat.cuda(), taps=gtaps)
+    torch.cuda.synchronize()
+    align, ng = otaps["align"], otaps["n_groups"]
+    G = align.shape[1]
+    print(f"[h15 padded groups] groups per clip {ng.tolist()} of {N} frames")
+    assert int(ng.max()) >= 3 * int(ng.min()) and int(ng.min()) < G
+    assert torch.equal(gtaps["n_groups"].cpu(), ng)
+    assert torch.equal(gtaps["seg"].cpu().long(), align.argmax(1)), "grouping differs from the oracle"
+    assert torch.equal(gtaps["token_lengths"].cpu(), oad.token_lengths(align))
+    for k in ["enc.out", "sem.out"] + _agg_taps(c):
+        e = rel(gtaps[k], otaps[k])
+        print(f"  [h15 padded groups] tap {k}: {e:.2e}")
+        assert e < TOL
+    pad = torch.arange(G)[None] >= ng[:, None]
+    for t in ("sem_agg.out", "ac_agg.out"):
+        assert not bool(gtaps[t].cpu().transpose(1, 2)[pad].any()), f"{t}: padded groups must be zero tokens"
+    assert bool((oa.transpose(1, 2)[pad] < 0).all())
+    assert torch.equal(out["acoustic_codes"].cpu(), oa) and torch.equal(out["semantic_codes"].cpu(), osem)
+    rec = m.decode(oa.cuda(), osem.cuda())
+    torch.cuda.synchronize()
+    ref = o15.codec_decode(sd, c, oa, osem)
+    e_wav = rel(rec, ref)
+    print(f"[h15 padded groups] wav rel {e_wav:.2e}")
+    assert rec.shape == ref.shape == (3, N * 640) and e_wav < TOL

@@ -382,6 +382,62 @@ def test_oracle_adaptive_alignment_matches_reference_fixture():
         assert torch.equal(oa.deaggregate(grouped, a)[:, :, : int(lens[0].sum())][0], oa.deaggregate_by_lengths(grouped, lens)[0])
 
 
+def _scan_groups(sim_row, threshold, cap):
+    """the grouping rule frame by frame: frame t opens a token when sim[t-1] <= threshold (compared in fp32, as a float32
+    tensor against a Python float is) or when the open token already holds `cap` frames (cap <= 0: no cap)"""
+    thr = float(np.float32(threshold))
+    seg, lens = [], []
+    for t in range(len(sim_row) + 1):
+        if t == 0 or float(sim_row[t - 1]) <= thr or (cap > 0 and lens[-1] == cap):
+            lens.append(0)
+        lens[-1] += 1
+        seg.append(len(lens) - 1)
+    return seg, lens
+
+
+def test_oracle_segments_from_sim_matches_frame_scan_and_reference_fixture():
+    """oracle.adaptive.segments_from_sim (the grouping half of similarity_alignment, taking similarities as input) against a
+    frame-by-frame scan, on the reference fixture (whose alignment matrices it must give as one-hots) and on the cases of
+    tests/test_adaptive_gpu.py plus no cap, cap 1 and similarities exactly at the threshold"""
+    from oracle import adaptive as oa
+
+    def check(sim, thr, cap):
+        seg, lengths, ng = oa.segments_from_sim(sim, thr, cap)
+        B, T = sim.shape[0], sim.shape[1] + 1
+        assert seg.shape == lengths.shape == (B, T) and ng.shape == (B,)
+        for b in range(B):
+            s, ln = _scan_groups(sim[b].tolist(), thr, cap)
+            assert seg[b].tolist() == s and int(ng[b]) == len(ln)
+            assert lengths[b].tolist() == ln + [0] * (T - len(ln))
+        return seg, ng
+
+    z = np.load(os.path.join(GOLD, "adaptive_alignment.npz"))
+    h = torch.from_numpy(z["h"])
+    for thr in (0.6, 0.85):
+        align, sim, n = oa.similarity_alignment(h, thr, 8)
+        seg, ng = check(sim, thr, 8)
+        assert torch.equal(ng, n)
+        ref = torch.from_numpy(z[f"align_{thr}"])
+        assert torch.equal(torch.nn.functional.one_hot(seg, ref.shape[1]).transpose(1, 2).to(ref.dtype), ref)
+        assert torch.equal(align, ref)
+    g = torch.Generator().manual_seed(3)
+    for B, T, D, thr, cap in ((3, 50, 64, 0.6, 8), (2, 200, 512, 0.3, 4), (1, 2, 16, 0.9, 8), (4, 33, 128, -2.0, 3), (2, 40, 32, 2.0, 8),
+                              (2, 60, 32, 0.5, 0), (2, 60, 32, 0.5, 1)):
+        base = torch.randn(B, T, D, generator=g)
+        h = base.clone()
+        for t in range(1, T):
+            h[:, t] = 0.7 * h[:, t - 1] + 0.7 * base[:, t]
+        align, sim, n = oa.similarity_alignment(h, thr, cap)
+        seg, ng = check(sim, thr, cap)
+        assert torch.equal(ng, n) and torch.equal(align.argmax(1), seg)
+    exact = torch.tensor([[1.0, 0.0, 1.0, 1.0, 0.0, 0.0, 1.0, 1.0, 1.0]])   # cosines of one-hot frames: exactly 0 or 1
+    for thr in (0.0, 1.0, 0.5, -2.0, 2.0):
+        for cap in (0, 1, 2, 3, 8):
+            check(exact, thr, cap)
+    assert oa.segments_from_sim(exact, 1.0, 0)[2].tolist() == [10]            # <= at the threshold: every frame opens a token
+    assert oa.segments_from_sim(exact, 0.0, 0)[2].tolist() == [4]
+
+
 def test_unise_face_host_logic():
     """unise.Model without a GPU: the checkpoint surface (state_dict holds the LM only, under `dnn.`, like model.py:81-91), the
     shape-only mel against the reference's formula (model.py:53-79 evaluated here with torch.stft on the CPU), the segment count of

@@ -27,9 +27,12 @@ def similarity_alignment(h: torch.Tensor, threshold: float, max_tokens_per_group
         raise RuntimeError("unified_audio_b200.adaptive runs on CUDA only (no CPU fallback)")
     B, T, D = h.shape
     h = h.float().contiguous()
-    if T <= 1:      # modeling_flexicodec_new.py:848-852
-        return (torch.ones(B, 1, T, device=h.device), torch.ones(B, max(T - 1, 0), device=h.device),
-                torch.ones(B, dtype=torch.long, device=h.device), torch.ones(B, 1, dtype=torch.long, device=h.device))
+    if T <= 1:      # modeling_flexicodec_new.py:848-852: one token holding the one frame
+        sim, ng = torch.ones(B, max(T - 1, 0), device=h.device), torch.ones(B, dtype=torch.long, device=h.device)
+        lens = torch.ones(B, 1, dtype=torch.long, device=h.device)
+        if not want_matrix:
+            return torch.zeros(B, T, dtype=torch.int32, device=h.device), sim, ng, lens
+        return torch.ones(B, 1, T, device=h.device), sim, ng, lens
     sim = torch.empty(B, T - 1, device=h.device)
     seg = torch.empty(B, T, dtype=torch.int32, device=h.device)
     lengths = torch.empty(B, T, dtype=torch.int32, device=h.device)

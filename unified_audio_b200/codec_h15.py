@@ -171,6 +171,12 @@ class CodecH15(CodecH1):
         t = self.c["agg"]
         D, G = t["dim"], plan["G"]
         L = T + G
+        # the kernel takes seg / lengths / offsets as row indices into the T + G sequence: a tensor of another dtype or shape
+        # would be read as out-of-range rows, so refuse it here
+        for key, shape in (("seg", (B, T)), ("lens32", (B, G)), ("offsets", (B, G)), ("ng32", (B,))):
+            v = plan[key]
+            if v.dtype != torch.int32 or tuple(v.shape) != shape:
+                raise ValueError(f"aggregation plan: {key} must be int32 {shape}, got {v.dtype} {tuple(v.shape)}")
         lib = _lib.load()
         x = self._buf(f"agg_x{L}", (B * L, D))
         qpos = self._buf(f"agg_qpos{G}", (B, G), torch.int32)
