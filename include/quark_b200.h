@@ -200,16 +200,11 @@ int64_t qb_attention_umma_workspace_bytes(int64_t B, int64_t L, int32_t heads, i
 int qb_attention_umma(const float* qkv, int64_t B, int64_t L, int32_t heads, int32_t head_dim, const float* rope_cos,
                       const float* rope_sin, qb_half* out_hi, qb_half* out_lo, int32_t split, int32_t causal, void* workspace,
                       void* stream);
-/* Single-layer LSTM recurrence (encoder_modules/transformer.py:115,133): xp [B,T,4H] fp32 already
- * holds x W_ih^T + b_ih + b_hh; w_hh planes [4H, H]; output h planes [B,T,H].
- * workspace: qb_lstm_workspace_bytes(B,H). */
-int64_t qb_lstm_workspace_bytes(int64_t B, int64_t H);
-int qb_lstm(const float* xp, const qb_half* whh_hi, const qb_half* whh_lo, int64_t B, int64_t T, int64_t H,
-            qb_half* out_hi, qb_half* out_lo, void* workspace, void* stream);
-
-/* Same recurrence on wgmma / TMA (the product path; lstm.cu's mma.sync version is kept as a
- * cross-check).  whh_perm: fp16 [H/U][4U][H] with row (4j+g) of slice c = gate g of hidden unit c*U+j,
- * U = qb_lstm_tc_units(H).  B <= 256 per call.  workspace: qb_lstm_tc_workspace_bytes(B,H). */
+/* Single-layer LSTM recurrence (encoder_modules/transformer.py:115,133) on wgmma / TMA: xp [B,T,4H] fp32 already
+ * holds x W_ih^T + b_ih + b_hh; output h planes [B,T,H] (out_lo may be NULL).  whh_perm: fp16 [H/U][4U][H] with
+ * row (4j+g) of slice c = gate g of hidden unit c*U+j, U = qb_lstm_tc_units(H) (0: width unsupported; H % 256 == 0
+ * is also required).  Any B: the rows run as independent recurrences in launches of at most 128 rows, one after
+ * the other, so a row's result does not depend on B.  workspace: qb_lstm_tc_workspace_bytes(B,H). */
 int32_t qb_lstm_tc_units(int64_t H);
 int64_t qb_lstm_tc_workspace_bytes(int64_t B, int64_t H);
 int qb_lstm_tc(const float* xp, const qb_half* whh_perm, int32_t units, int64_t B, int64_t T, int64_t H,

@@ -60,3 +60,39 @@ def test_h1_config1_roundtrip(lib, precision):
     e_wav = rel(rec, torch.from_numpy(z["wav_rec"]))
     print(f"[h1/{precision}] wav rel {e_wav:.2e}")
     assert rec.shape == (1, 16000) and e_wav < 1e-3
+
+
+def test_h1_batch_of_260_matches_batch_of_4(lib):
+    """A clip's codes do not depend on the batch it is encoded in: the shipped config at B = 260 (three LSTM launches of at most
+    128 rows per transformer layer) gives rows 0-3 the codes those four clips get at B = 4"""
+    from oracle import hcodec1
+    from unified_audio_b200.codec_h1 import CodecH1
+    m = CodecH1({}, {}, {})
+    m.load_state_dict(hcodec1.make_state_dict(hcodec1.H1, 5), strict=True)
+    m = m.cuda()
+    B, T = 260, 3200
+    g = torch.Generator().manual_seed(17)
+    x = 0.1 * torch.randn(B, 1, T, generator=g)
+    f = torch.randn(B, 768, T // 320, generator=g)
+    feat = torch.sign(f) * f.abs() ** 0.3
+    taps_b, taps_4 = {}, {}
+    codes_b = m.encode(x.cuda(), feat.cuda(), taps=taps_b)
+    codes_4 = m.encode(x[:4].cuda(), feat[:4].cuda(), taps=taps_4)
+    torch.cuda.synchronize()
+    diverged = [k for k in taps_4 if not torch.equal(taps_b[k][:4], taps_4[k])]
+    print(f"taps of rows 0-3 that differ between B = {B} and B = 4: {diverged or 'none'}")
+    for name, cb, c4 in zip(("acoustic", "semantic"), codes_b, codes_4):
+        assert torch.equal(cb[:4], c4), f"{name} codes of rows 0-3 differ between B = {B} and B = 4; taps that differ: {diverged}"
+
+
+def test_h1_small_decoder_width_rejected_at_prepare(lib):
+    """oracle.hcodec1.h1_small() has dec_dim 384, which the wgmma recurrence cannot run: encode fails while the weights are
+    packed, with a message naming the width, instead of inside a kernel"""
+    from oracle import hcodec1
+    from unified_audio_b200.codec_h1 import CodecH1
+    c = hcodec1.h1_small()
+    m = CodecH1(_cfg=c)
+    m.load_state_dict(hcodec1.make_state_dict(c, 1), strict=True)
+    m = m.cuda()
+    with pytest.raises(ValueError, match="LSTM width 384 unsupported by the wgmma recurrence"):
+        m.encode(torch.zeros(1, 1, 1280, device="cuda"), torch.zeros(1, c["sem_in"], 4, device="cuda"))

@@ -244,19 +244,19 @@ def test_attention_umma(lib, D, split, B, T, H):
 
 
 @pytest.mark.parametrize("B,T,H", [(2, 9, 256), (3, 20, 512), (5, 12, 1536), (70, 6, 512), (130, 5, 256)])
-def test_lstm(lib, B, T, H):
+def test_lstm_tc(lib, B, T, H):
     from unified_audio_b200 import ops
     k = 1.0 / math.sqrt(H)
     g = torch.Generator().manual_seed(41)
     whh = ((torch.rand(4 * H, H, generator=g) * 2 - 1) * k).to(DEV)
     xp = _mk((B, T, 4 * H), 42)
-    wp = ops.Planes.from_f32(whh, False)
+    U = ops.lstm_tc_units(H)
     out = ops.Planes.zeros((B, T, H), True, DEV)
-    ws = torch.zeros(ops.lstm_workspace_bytes(B, H), dtype=torch.uint8, device=DEV)
-    ops.lstm(xp, wp, B, T, H, out, ws)
+    ws = torch.zeros(ops.lstm_tc_workspace_bytes(B, H), dtype=torch.uint8, device=DEV)
+    ops.lstm_tc(xp, ops.lstm_tc_permute(whh, U), U, B, T, H, out, ws)
     torch.cuda.synchronize()
     # reference recurrence in fp64 with the same fp16-rounded operands (W_hh and h_{t-1})
-    W = wp.hi.double()
+    W = whh.half().double()
     h = torch.zeros(B, H, dtype=torch.float64, device=DEV)
     c = torch.zeros_like(h)
     outs = []
@@ -268,18 +268,9 @@ def test_lstm(lib, B, T, H):
         outs.append(h)
     ref = torch.stack(outs, 1)
     e = relerr(planes_ref(out), ref)
-    print(f"lstm B{B} T{T} H{H} relerr {e:.3e}")
-    # wgmma version (product path)
-    U = ops.lstm_tc_units(H)
-    out2 = ops.Planes.zeros((B, T, H), True, DEV)
-    ws2 = torch.zeros(ops.lstm_tc_workspace_bytes(B, H), dtype=torch.uint8, device=DEV)
-    ops.lstm_tc(xp, ops.lstm_tc_permute(whh, U), U, B, T, H, out2, ws2)
-    torch.cuda.synchronize()
-    e2 = relerr(planes_ref(out2), ref)
-    print(f"lstm_tc B{B} T{T} H{H} U{U} relerr {e2:.3e}")
-    assert e2 < 2e-3 and relerr(planes_ref(out2)[:, 0], ref[:, 0]) < 1e-5
-    assert e < 2e-3   # fp16 re-rounding of h can flip one ulp on a knife edge; exact-model error is ~1e-6
-    assert relerr(planes_ref(out)[:, 0], ref[:, 0]) < 1e-5
+    print(f"lstm_tc B{B} T{T} H{H} U{U} relerr {e:.3e}")
+    # fp16 re-rounding of h can flip one ulp on a knife edge; exact-model error is ~1e-6
+    assert e < 2e-3 and relerr(planes_ref(out)[:, 0], ref[:, 0]) < 1e-5
 
 
 def test_spectral(lib):

@@ -82,8 +82,6 @@ SIGNATURES = {
     "qb_attention_hd": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "qb_attention_umma_workspace_bytes": (C.c_int64, [_i64, _i64, _i32, _i32, _i32]),
     "qb_attention_umma": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp]),
-    "qb_lstm_workspace_bytes": (C.c_int64, [_i64, _i64]),
-    "qb_lstm": (C.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
     "qb_lstm_tc_units": (C.c_int32, [_i64]),
     "qb_lstm_tc_workspace_bytes": (C.c_int64, [_i64, _i64]),
     "qb_lstm_tc": (C.c_int, [_vp, _vp, _i32, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),

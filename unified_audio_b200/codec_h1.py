@@ -222,6 +222,9 @@ class CodecH1(_CodecFace):
         layers = []
         hdim = sd[f"{prefix}layers.0.self_attn.rnn.weight_hh_l0"].shape[1]
         lstm_u = ops.lstm_tc_units(hdim) if hdim % 256 == 0 else 0
+        if not lstm_u:
+            raise ValueError(f"{prefix}: LSTM width {hdim} unsupported by the wgmma recurrence "
+                             f"(needs H % 256 == 0, and H / U CTAs of U = 4, 8 or 12 units fitting on the SMs)")
         for i in range(n):
             p = f"{prefix}layers.{i}."
             a = p + "self_attn."
@@ -231,8 +234,7 @@ class CodecH1(_CodecFace):
                 in_w=sd[p + "input_layernorm.weight"].float().contiguous(), post_w=sd[p + "post_attention_layernorm.weight"].float().contiguous(),
                 wih=lw(sd[a + "rnn.weight_ih_l0"], "lstm_attn"),
                 b_ih=(sd[a + "rnn.bias_ih_l0"].float() + sd[a + "rnn.bias_hh_l0"].float()).contiguous(),
-                whh=Planes.from_f32(sd[a + "rnn.weight_hh_l0"].float().contiguous(), False),
-                whh_perm=(ops.lstm_tc_permute(sd[a + "rnn.weight_hh_l0"], lstm_u) if lstm_u else None),
+                whh_perm=ops.lstm_tc_permute(sd[a + "rnn.weight_hh_l0"], lstm_u), lstm_u=lstm_u,
                 wqkv=lw(torch.cat([sd[a + f"{n_}_proj.weight"].float() for n_ in "qkv"], 0), "lstm_attn"),
                 bqkv=torch.cat([sd[a + f"{n_}_proj.bias"].float() for n_ in "qkv"], 0).contiguous(),
                 wo=lw(sd[a + "o_proj.weight"], "lstm_attn"), w13=lw(w13.reshape(-1, w13.shape[-1]), "mlp"),
@@ -266,19 +268,14 @@ class CodecH1(_CodecFace):
         hid = self._planes("tf_hid", (M, I), pm)
         xp = self._buf("tf_xp", (M, 4 * C))
         qkv = self._buf("tf_qkv", (M, 3 * C))
-        use_tc = layers[0]["whh_perm"] is not None and B <= 256
-        ws = self._buf("lstm_ws", (max(ops.lstm_workspace_bytes(B, C), ops.lstm_tc_workspace_bytes(B, C)),), torch.uint8)
-        lstm_u = ops.lstm_tc_units(C) if use_tc else 0
+        ws = self._buf("lstm_ws", (ops.lstm_tc_workspace_bytes(B, C),), torch.uint8)
         cos, sin = self._cached(("rope", F, hd), lambda: ops.rope_tables(F, hd, self._dev()))
         att_ws = self._buf("att5_ws", (ops.self_attention_workspace_bytes(B, F, heads, hd, pa),), torch.uint8)
         xm = rowmap(x, C, M, 0)
         for L in layers:
             ops.rmsnorm(x, L["in_w"], M, C, t_a)
             self._linear(t_a, L["wih"], 4 * C, M, C, bias=L["b_ih"], out_f32=rowmap(xp, 4 * C, M, 0))
-            if use_tc:
-                ops.lstm_tc(xp, L["whh_perm"], lstm_u, B, F, C, t_b, ws)
-            else:
-                ops.lstm(xp, L["whh"], B, F, C, t_b, ws)
+            ops.lstm_tc(xp, L["whh_perm"], L["lstm_u"], B, F, C, t_b, ws)
             self._linear(t_b, L["wqkv"], 3 * C, M, C, bias=L["bqkv"], out_f32=rowmap(qkv, 3 * C, M, 0))
             ops.self_attention(qkv, B, F, heads, hd, cos, sin, t_a, att_ws, pa)
             self._linear(t_a, L["wo"], C, M, C, residual=xm, out_f32=xm)

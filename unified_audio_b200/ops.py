@@ -265,14 +265,6 @@ def attention_tc(qkv, B, T, heads, rope_cos, rope_sin, out: Planes, workspace):
     attention_umma(qkv, B, T, heads, 64, rope_cos, rope_sin, out, workspace, split=False)
 
 
-def lstm_workspace_bytes(B, H):
-    return int(_lib.load().qb_lstm_workspace_bytes(B, H))
-
-
-def lstm(xp, whh: Planes, B, T, H, out: Planes, workspace):
-    _lib.check(_lib.load().qb_lstm(_p(xp), _p(whh.hi), None, B, T, H, _p(out.hi), _p(out.lo), _p(workspace), _stream()))
-
-
 def lstm_tc_units(H):
     return int(_lib.load().qb_lstm_tc_units(H))
 
