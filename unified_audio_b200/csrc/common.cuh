@@ -163,5 +163,33 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, ui
       ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(x), "r"(y), "r"(z)
       : "memory");
 }
+// TMA store of one box from shared memory; elements outside the tensor map's bounds are not written.  Completion is tracked by
+// bulk groups: commit after the store, then wait (.read: until the shared-memory source may be overwritten).
+__device__ __forceinline__ void tma_store_3d(const void* tmap, const void* smem_src, int x, int y, int z) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(tmap), "r"(smem_u32(smem_src)), "r"(x), "r"(y), "r"(z)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// shared-memory accesses by 32-bit address (a generic pointer takes two registers)
+__device__ __forceinline__ void st_shared_f32x2(uint32_t addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y));
+}
+__device__ __forceinline__ float2 ld_shared_f32x2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v));
+}
+// barrier over `count` threads (a multiple of 32) under barrier id `id` (0 is __syncthreads')
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 }  // namespace qb

@@ -5,8 +5,13 @@
 // memory with the 128-byte TMA/wgmma swizzle; accumulators live in registers.  Warp roles (384 threads):
 //   warpgroup 0     TMA producer (one thread), shrunk to 40 registers by setmaxnreg
 //   warpgroups 1-2  wgmma m64nBNk16 on rows [0, 64) / [64, 128) of the tile, then the epilogue
-//                   (bias/act/gamma/residual -> global) straight from the accumulator registers;
-//                   the producer already fills the stages of the next tile meanwhile.  232 registers each.
+//                   (bias/act/gamma/residual) from the accumulator registers; the producer already fills the
+//                   stages of the next tile meanwhile.  232 registers each.
+// The two fast epilogue kinds never wait on global memory: the tile's bias / gamma are fetched while its main loop
+// runs and read from shared memory, the residual arrives by TMA into two 8 KB subtile buffers per warpgroup, and each
+// 64 x 128-byte output subtile leaves by TMA store, which drains while the next tile's main loop runs.  Shared memory:
+// 192 KB of stages + 32 KB of subtile buffers + the tile's bias / gamma.  On an H100 80GB HBM3 at 700 W this took the
+// ConvNeXt pwconv1 / pwconv2 GEMMs from 417 / 442 to 537 / 546 TFLOP/s (scripts/gemm_table.py).
 // Convolutions are expressed as `taps` shifted K-panels over a zero-padded channel-last buffer:
 // the A tensor map views the buffer as [batch][rows/stride][stride*C], so tap t of output row m is
 // the box at (x = (t % stride)*C + c, y = m + t / stride) - TMA-staged im2col without an im2col
@@ -46,10 +51,11 @@ static int current_device() {
 #endif
 
 // What the epilogue of a launch does, decided on the host so that the consumer branches once per tile:
-//   EPI_HI      (bias) (GELU) -> fp16 hi plane, one half2 store per accumulator pair (ConvNeXt pwconv1)
-//   EPI_F32     (bias) (* gamma) (+ residual) -> fp32, one float2 store per pair (pwconv2, o-proj, w2, residual convs)
+//   EPI_HI      (bias) (GELU) -> fp16 hi plane (ConvNeXt pwconv1)
+//   EPI_F32     (bias) (* gamma) (+ residual) -> fp32 (pwconv2, o-proj, w2, residual convs)
 //   EPI_GENERIC every other combination, element by element through epilogue_pair
-// The two fast kinds need an even N and even pitches / 8-byte aligned bases, so that every in-range pair is one aligned vector.
+// The two fast kinds stage each output subtile in shared memory and write it by TMA store, EPI_F32 reads its residual by TMA
+// load; they need 16-byte aligned bases and row pitches (classify_epilogue).
 enum EpiKind : int { EPI_GENERIC = 0, EPI_HI = 1, EPI_F32 = 2 };
 
 struct RowMapD {
@@ -174,52 +180,131 @@ constexpr int GEMM_THREADS = 3 * 128;           // warpgroup 0: TMA producer; wa
 // register split after setmaxnreg: 128 * 40 + 256 * 232 = 64512 of the SM's 65536 (the launch reserves 384 * 168)
 constexpr int GEMM_PRODUCER_REGS = 40, GEMM_CONSUMER_REGS = 232;
 
-// Fast epilogue kinds: accumulator pair (rows r, r + 8; columns n, n + 1 for n = c + 8j) -> one vector store each.
-// Same arithmetic, in the same order, as the vectorised branches of epilogue_pair.
+// Epilogue buffers of the fast kinds: per consumer warpgroup, EPI_BUFS subtiles of 64 rows x 128 bytes (32 fp32 or 64 fp16
+// columns) in the TMA 128-byte swizzle: row r at r * 128, its 16-byte chunk c at chunk position c ^ (r % 8).  The quad of
+// lanes holding one row of an 8-column group then writes 8 distinct chunk positions per 8 rows: no bank conflicts.
+constexpr int EPI_BUFS = 2;
+constexpr uint32_t EPI_SUB_BYTES = 64 * 128;
+
+// Per-column operands of a tile in shared memory, [bias | gamma] x BN floats: the 256 consumer threads fetch them at the start
+// of the tile, so that the latency hides behind its main loop, and store them once the main loop is done.
 template <int BN>
-__device__ __forceinline__ void epilogue_hi(const GemmParams& p, int b, int r, int c, const float (&acc)[BN / 2]) {
+__device__ __forceinline__ void load_tile_cols(const GemmParams& p, int n0, int ct, float (&v)[2 * BN / 256]) {
+#pragma unroll
+  for (int i = 0; i < 2 * BN / 256; ++i) {
+    const int k = ct + 256 * i, n = n0 + k % BN;
+    const float* src = k < BN ? p.bias : p.gamma;
+    v[i] = src && n < p.N ? __ldg(src + n) : 0.f;
+  }
+}
+
+// Fast epilogue kinds, on the 64 x BN half tile of one consumer warpgroup (rows row0 + [0, 64), columns n0 + [0, BN)):
+// accumulators -> swizzled subtile in shared memory -> one TMA store per subtile, issued by the warpgroup's first thread.
+// The stores drain while the next tile's main loop runs; the TMA map clips rows >= m_per_batch and columns >= N.
+// Same arithmetic, in the same order, as the vectorised branches of epilogue_pair.
+struct EpiCtx {
+  uint8_t* buf;        // this warpgroup's EPI_BUFS subtile buffers
+  uint64_t* rfull;     // one mbarrier per buffer: residual subtile landed
+  uint32_t cols;       // shared address of the tile's [bias | gamma]
+  int cw, b, row0, n0;
+};
+
+template <int BN>
+__device__ __forceinline__ void epilogue_hi(const GemmParams& p, const CUtensorMap* tmO, const EpiCtx& e, const float (&acc)[BN / 2]) {
+  constexpr int NSUB = BN / 64;
   const __half2 hmax = __float2half2_rn(65504.f), hmin = __float2half2_rn(-65504.f);
-  const bool gelu = p.act == QB_ACT_GELU;
-  __half* base = (__half*)p.ohi.ptr + ((long long)b * p.ohi.rpb + p.ohi.off + r) * p.ohi.ld;
-  const long long row8 = 8 * p.ohi.ld;
+  const bool gelu = p.act == QB_ACT_GELU, leader = (threadIdx.x & 127) == 0;
+  const int lane = threadIdx.x & 31;
+  // rows r and r + 8 (r % 8 = lane / 4) at 4-byte column offset 4 (lane % 4) of chunk jj, stored at chunk jj ^ (lane / 4)
+  const uint32_t th = smem_u32(e.buf) + (((threadIdx.x >> 5) & 3) * 16 + (lane >> 2)) * 128 + 4 * (lane & 3), sw = (lane >> 2) << 4;
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int n = c + 8 * j;
-    if (n >= p.N) break;
-    const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.f, 0.f);
+  for (int s = 0; s < NSUB; ++s) {
+    uint8_t* buf = e.buf + (s % EPI_BUFS) * EPI_SUB_BYTES;
+    if (s == 0) {                              // the previous tile's stores have read the buffers
+      if (leader) bulk_wait_read<0>();
+      named_bar_sync(2 + e.cw, 128);
+    } else if (s >= EPI_BUFS) {                // the store of subtile s - EPI_BUFS has read this buffer
+      if (leader) bulk_wait_read<EPI_BUFS - 1>();
+      named_bar_sync(2 + e.cw, 128);
+    }
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      if (r + 8 * h >= p.m_per_batch) continue;
-      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-      if (p.bias) { v0 += bb.x; v1 += bb.y; }
-      if (gelu) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
-      *reinterpret_cast<__half2*>(base + h * row8 + n) = __hmax2_nan(__hmin2_nan(__floats2half2_rn(v0, v1), hmax), hmin);
+    for (int jj = 0; jj < 8; ++jj) {
+      const int j = 8 * s + jj;
+      const float2 bb = p.bias ? ld_shared_f32x2(e.cols + 4 * (8 * j + 2 * (lane & 3))) : make_float2(0.f, 0.f);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (p.bias) { v0 += bb.x; v1 += bb.y; }
+        if (gelu) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
+        const __half2 o = __hmax2_nan(__hmin2_nan(__floats2half2_rn(v0, v1), hmax), hmin);
+        st_shared_b32(th + (s % EPI_BUFS) * EPI_SUB_BYTES + h * 1024 + ((16 * jj) ^ sw), *reinterpret_cast<const uint32_t*>(&o));
+      }
+    }
+    fence_proxy_async();
+    named_bar_sync(2 + e.cw, 128);
+    if (leader) {
+      tma_store_3d(tmO, buf, e.n0 + 64 * s, e.row0, e.b);
+      bulk_commit();
     }
   }
 }
 
+// The residual arrives by TMA into the subtile buffer the result is then written to: subtiles 0 .. EPI_BUFS - 1 were requested
+// during the main loop, subtile s + EPI_BUFS as soon as the store of subtile s has read its buffer.  Every element is read and
+// then written by the same thread, so the residual may be the output buffer itself.
 template <int BN>
-__device__ __forceinline__ void epilogue_f32(const GemmParams& p, int b, int r, int c, const float (&acc)[BN / 2]) {
-  float* base = (float*)p.o32.ptr + ((long long)b * p.o32.rpb + p.o32.off + r) * p.o32.ld;
-  const float* rbase = p.res.ptr ? (const float*)p.res.ptr + ((long long)b * p.res.rpb + p.res.off + r) * p.res.ld : nullptr;
-  const long long row8 = 8 * p.o32.ld, rrow8 = 8 * p.res.ld;
+__device__ __forceinline__ void epilogue_f32(const GemmParams& p, const CUtensorMap* tmO, const CUtensorMap* tmR, const EpiCtx& e,
+                                             const float (&acc)[BN / 2]) {
+  constexpr int NSUB = BN / 32;
+  static_assert(NSUB % (2 * EPI_BUFS) == 0, "each residual barrier completes an even number of phases per tile");
+  const bool res = p.res.ptr != nullptr, leader = (threadIdx.x & 127) == 0;
+  const int lane = threadIdx.x & 31;
+  // rows r and r + 8 (r % 8 = lane / 4) at byte 8 (lane % 2) of chunk 2 jj + (lane % 4) / 2, stored at that chunk ^ (lane / 4);
+  // 2 jj has no bit in common with (lane % 4) / 2, so the stored chunk is 2 jj ^ ((lane % 4) / 2 ^ lane / 4)
+  const uint32_t th = smem_u32(e.buf) + (((threadIdx.x >> 5) & 3) * 16 + (lane >> 2)) * 128 + 8 * (lane & 1),
+                 sw = (((lane >> 1) & 1) ^ (lane >> 2)) << 4;
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int n = c + 8 * j;
-    if (n >= p.N) break;
-    const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.f, 0.f);
-    const float2 g = p.gamma ? __ldg(reinterpret_cast<const float2*>(p.gamma + n)) : make_float2(1.f, 1.f);
+  for (int s = 0; s < NSUB; ++s) {
+    const int u = s % EPI_BUFS;
+    uint8_t* buf = e.buf + u * EPI_SUB_BYTES;
+    if (res) {
+      mbar_wait(&e.rfull[u], (s / EPI_BUFS) & 1);
+    } else if (s == 0) {                       // the previous tile's stores have read the buffers
+      if (leader) bulk_wait_read<0>();
+      named_bar_sync(2 + e.cw, 128);
+    } else if (s >= EPI_BUFS) {                // the store of subtile s - EPI_BUFS has read this buffer
+      if (leader) bulk_wait_read<EPI_BUFS - 1>();
+      named_bar_sync(2 + e.cw, 128);
+    }
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      if (r + 8 * h >= p.m_per_batch) continue;
-      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-      if (p.bias) { v0 += bb.x; v1 += bb.y; }
-      if (p.gamma) { v0 *= g.x; v1 *= g.y; }
-      if (rbase) {
-        const float2 rv = *reinterpret_cast<const float2*>(rbase + h * rrow8 + n);
-        v0 += rv.x; v1 += rv.y;
+    for (int jj = 0; jj < 4; ++jj) {
+      const int j = 4 * s + jj;
+      const uint32_t col = e.cols + 4 * (8 * j + 2 * (lane & 3));
+      const float2 bb = p.bias ? ld_shared_f32x2(col) : make_float2(0.f, 0.f);
+      const float2 g = p.gamma ? ld_shared_f32x2(col + 4 * BN) : make_float2(1.f, 1.f);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t el = th + u * EPI_SUB_BYTES + h * 1024 + ((32 * jj) ^ sw);
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (p.bias) { v0 += bb.x; v1 += bb.y; }
+        if (p.gamma) { v0 *= g.x; v1 *= g.y; }
+        if (res) {
+          const float2 rv = ld_shared_f32x2(el);
+          v0 += rv.x; v1 += rv.y;
+        }
+        st_shared_f32x2(el, v0, v1);
       }
-      *reinterpret_cast<float2*>(base + h * row8 + n) = make_float2(v0, v1);
+    }
+    fence_proxy_async();
+    named_bar_sync(2 + e.cw, 128);
+    if (leader) {
+      tma_store_3d(tmO, buf, e.n0 + 32 * s, e.row0, e.b);
+      bulk_commit();
+      if (res && s + EPI_BUFS < NSUB) {
+        bulk_wait_read<0>();
+        mbar_arrive_expect_tx(&e.rfull[u], EPI_SUB_BYTES);
+        tma_load_3d(buf, tmR, &e.rfull[u], e.n0 + 32 * (s + EPI_BUFS), e.row0, e.b);
+      }
     }
   }
 }
@@ -229,6 +314,7 @@ template <int NTERMS, int BN, int STAGES>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
+               const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes,
                const GemmParams p) {
   constexpr int BM = GEMM_BM, BK = GEMM_BK;
   constexpr int NPL = (NTERMS == 1) ? 1 : 2;
@@ -236,19 +322,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   constexpr uint32_t STAGE_BYTES = NPL * (A_BYTES + W_BYTES);
   constexpr int CONSUMER_WARPS = 8;
 
-  extern __shared__ uint8_t smem_raw[];
+  extern __shared__ __align__(128) uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
-  uint64_t* full = (uint64_t*)(smem + STAGES * STAGE_BYTES);
+  uint8_t* epi_smem = smem + STAGES * STAGE_BYTES;
+  float* tile_cols = (float*)(epi_smem + 2 * EPI_BUFS * EPI_SUB_BYTES);      // [bias | gamma] x BN
+  uint64_t* full = (uint64_t*)(tile_cols + 2 * BN);
   uint64_t* empty = full + STAGES;
+  uint64_t* rfull = empty + STAGES;        // [2][EPI_BUFS]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
+  const bool tma_epi = p.epi != EPI_GENERIC;
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], CONSUMER_WARPS); }
+    for (int s = 0; s < 2 * EPI_BUFS; ++s) mbar_init(&rfull[s], 1);
     fence_mbar_init();
   }
   if (threadIdx.x == 32) {
     prefetch_tmap(&tmA_hi); prefetch_tmap(&tmW_hi);
     if (NPL == 2) { prefetch_tmap(&tmA_lo); prefetch_tmap(&tmW_lo); }
+    if (tma_epi) { prefetch_tmap(&tmOut); if (p.res.ptr) prefetch_tmap(&tmRes); }
   }
   __syncthreads();
 
@@ -277,11 +369,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   } else {
     setmaxnreg_inc<GEMM_CONSUMER_REGS>();
     const int cw = wg - 1, wq = warp & 3;      // consumer warpgroup: rows [cw * 64, +64) of the tile
+    const bool leader = (threadIdx.x & 127) == 0, epi_res = p.epi == EPI_F32 && p.res.ptr;
+    const bool epi_cols = tma_epi && (p.bias || p.gamma);
     uint32_t stage = 0, phase = 0;
     float acc[BN / 2];
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const int n_tile = tile % p.num_n_tiles, m_tile = tile / p.num_n_tiles;
       const int b = m_tile / p.tiles_per_batch, m0 = (m_tile % p.tiles_per_batch) * BM, n0 = n_tile * BN;
+      float cols[2 * BN / 256];
+      if (epi_cols) load_tile_cols<BN>(p, n0, threadIdx.x - 128, cols);
       uint32_t prev_stage = 0;
       for (int kb = 0; kb < p.num_kb; ++kb) {
         mbar_wait(&full[stage], phase);
@@ -298,6 +394,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           }
         }
         wgmma_commit();
+        if (kb == 0 && epi_res && leader) {
+          // while the first MMAs run: the previous tile's stores have left the epilogue buffers, which may now take the
+          // first residual subtiles of this one
+          bulk_wait_read<0>();
+#pragma unroll
+          for (int u = 0; u < EPI_BUFS; ++u) {
+            uint64_t* bar = rfull + cw * EPI_BUFS + u;
+            mbar_arrive_expect_tx(bar, EPI_SUB_BYTES);
+            tma_load_3d(epi_smem + (cw * EPI_BUFS + u) * EPI_SUB_BYTES, &tmRes, bar, n0 + 32 * u, m0 + cw * 64, b);
+          }
+        }
         wgmma_wait<1>();                          // the MMAs of K-block kb - 1 are done: release their stage
         if (kb > 0 && lane == 0) mbar_arrive(&empty[prev_stage]);
         prev_stage = stage;
@@ -306,12 +413,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
       if (lane == 0) mbar_arrive(&empty[prev_stage]);
-      const int r = m0 + cw * 64 + wq * 16 + (lane >> 2), c = n0 + 2 * (lane & 3);
+      if (epi_cols) {
+        named_bar_sync(1, 256);                // both warpgroups are done with the previous tile's columns
+#pragma unroll
+        for (int i = 0; i < 2 * BN / 256; ++i) tile_cols[threadIdx.x - 128 + 256 * i] = cols[i];
+        named_bar_sync(1, 256);
+      }
+      const EpiCtx ec{epi_smem + cw * EPI_BUFS * EPI_SUB_BYTES, rfull + cw * EPI_BUFS, smem_u32(tile_cols), cw, b, m0 + cw * 64, n0};
       if (p.epi == EPI_HI) {
-        epilogue_hi<BN>(p, b, r, c, acc);
+        epilogue_hi<BN>(p, &tmOut, ec, acc);
       } else if (p.epi == EPI_F32) {
-        epilogue_f32<BN>(p, b, r, c, acc);
+        epilogue_f32<BN>(p, &tmOut, &tmRes, ec, acc);
       } else {
+        const int r = m0 + cw * 64 + wq * 16 + (lane >> 2), c = n0 + 2 * (lane & 3);
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
           epilogue_pair(p, b, r, c + 8 * j, acc[4 * j], acc[4 * j + 1]);
@@ -319,6 +433,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         }
       }
     }
+    if (tma_epi && leader) bulk_wait<0>();      // the shared-memory sources of the last stores stay valid until read
   }
 }
 
@@ -382,11 +497,11 @@ static EncodeTiledFn get_encode() {
 }
 
 static int make_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                    const cuuint32_t* box) {
+                    const cuuint32_t* box, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16) {
   EncodeTiledFn enc = get_encode();
   QB_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available (no CUDA driver?)");
   cuuint32_t es[3] = {1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(base), dims, strides_bytes, box, es,
+  CUresult r = enc(m, dtype, rank, const_cast<void*>(base), dims, strides_bytes, box, es,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   QB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed: %d (rank %d dims %llu %llu %llu)", (int)r, rank,
@@ -398,17 +513,35 @@ static RowMapD to_rm(const qb_rowmap& r) { return RowMapD{r.ptr, (long long)r.ld
 
 static bool aligned(const void* ptr, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(ptr) & (bytes - 1)) == 0; }
 
-// The conditions are those under which epilogue_pair takes its vectorised branch for every in-range pair (plus an 8-byte
-// aligned bias, loaded as float2), so each kind computes what epilogue_pair would.
+// A row map TMA can address as [batch][m_per_batch][N] based at row `off`: 16-byte aligned base and row pitch, columns
+// within the pitch, batches that do not overlap, and rows of whole 16-byte chunks (a TMA store writes the last chunk of a
+// row in full, so a partial one would overwrite the columns past N).
+static bool tma_rows(const RowMapD& r, long long esize, const GemmParams& p) {
+  return r.ld >= p.N && (r.ld * esize) % 16 == 0 && (p.N * esize) % 16 == 0 && aligned(r.ptr, 16) &&
+         (p.a_batch == 1 || r.rpb >= r.off + p.m_per_batch);
+}
+
+// The epilogues epilogue_pair computes with one vector store per pair, when the TMA requirements hold for every buffer the
+// kind reads or writes; each kind computes what epilogue_pair would.
 static int classify_epilogue(const GemmParams& p) {
-  if (p.N % 2 != 0 || p.act2 != QB_ACT_NONE || !aligned(p.bias, 8)) return EPI_GENERIC;
+  if (p.act2 != QB_ACT_NONE) return EPI_GENERIC;
   if (p.ohi.ptr && !p.olo.ptr && !p.o32.ptr && !p.res.ptr && !p.gamma && (p.act == QB_ACT_NONE || p.act == QB_ACT_GELU) &&
-      (p.ohi.ld & 1) == 0 && aligned(p.ohi.ptr, 4))
+      tma_rows(p.ohi, 2, p))
     return EPI_HI;
-  if (p.o32.ptr && !p.ohi.ptr && p.act == QB_ACT_NONE && (p.o32.ld & 1) == 0 && aligned(p.o32.ptr, 8) &&
-      (!p.res.ptr || ((p.res.ld & 1) == 0 && aligned(p.res.ptr, 8))) && aligned(p.gamma, 8))
+  if (p.o32.ptr && !p.ohi.ptr && p.act == QB_ACT_NONE && tma_rows(p.o32, 4, p) && (!p.res.ptr || tma_rows(p.res, 4, p)))
     return EPI_F32;
   return EPI_GENERIC;
+}
+
+// Output / residual map of the fast epilogue kinds: [batch][m_per_batch][N] from row `off`, one 64-row x 128-byte box per subtile.
+static int make_rows_map(CUtensorMap* m, const RowMapD& r, bool f32, const GemmParams& p) {
+  const cuuint64_t es = f32 ? 4 : 2, ld = (cuuint64_t)r.ld;
+  const cuuint64_t rows = p.a_batch > 1 ? (cuuint64_t)r.rpb : (cuuint64_t)p.m_per_batch;
+  cuuint64_t dims[3] = {(cuuint64_t)p.N, (cuuint64_t)p.m_per_batch, (cuuint64_t)p.a_batch};
+  cuuint64_t str[2] = {ld * es, rows * ld * es};
+  cuuint32_t box[3] = {(cuuint32_t)(128 / es), 64, 1};
+  return make_map(m, (const char*)r.ptr + r.off * ld * es, 3, dims, str, box,
+                  f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
 }
 
 static int fill_params(const qb_gemm_desc* d, GemmParams* p, int BN) {
@@ -465,9 +598,20 @@ static int launch_tc(const qb_gemm_desc* d, cudaStream_t st, int num_sms) {
   } else {
     mA_lo = mA_hi; mW_lo = mW_hi;
   }
+  CUtensorMap mOut = mA_hi, mRes = mA_hi;             // used by the fast epilogue kinds only
+  if (p.epi == EPI_HI) {
+    if (int e = make_rows_map(&mOut, p.ohi, false, p)) return e;
+  } else if (p.epi == EPI_F32) {
+    if (int e = make_rows_map(&mOut, p.o32, true, p)) return e;
+    if (p.res.ptr)
+      if (int e = make_rows_map(&mRes, p.res, true, p)) return e;
+  }
   constexpr int NPL = NTERMS == 1 ? 1 : 2;
-  constexpr size_t smem = (size_t)STAGES * NPL * (GEMM_BM * 64 * 2 + BN * 64 * 2) + 1024 + 256;
-  static_assert(smem <= 227 * 1024, "GEMM pipeline exceeds the 227 KB of shared memory a block may use");
+  // pipeline stages, epilogue subtile buffers, the tile's bias / gamma, mbarriers, and up to 896 bytes that align the
+  // (128-byte aligned) base to 1024
+  constexpr size_t smem = (size_t)STAGES * NPL * (GEMM_BM * 64 * 2 + BN * 64 * 2) + 2 * EPI_BUFS * EPI_SUB_BYTES + 2 * BN * 4 +
+                          (2 * STAGES + 2 * EPI_BUFS) * 8 + 1024 - 128;
+  static_assert(smem <= 227 * 1024, "GEMM pipeline and epilogue buffers exceed the 227 KB of shared memory a block may use");
   auto kern = gemm_tc_kernel<NTERMS, BN, STAGES>;
   static bool attr_set[QB_MAX_DEVICES] = {};          // the opt-in shared-memory limit is per-device state
   const int dev = current_device();
@@ -476,7 +620,7 @@ static int launch_tc(const qb_gemm_desc* d, cudaStream_t st, int num_sms) {
     attr_set[dev] = true;
   }
   int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-  kern<<<grid, GEMM_THREADS, smem, st>>>(mA_hi, mA_lo, mW_hi, mW_lo, p);
+  kern<<<grid, GEMM_THREADS, smem, st>>>(mA_hi, mA_lo, mW_hi, mW_lo, mOut, mRes, p);
   g_launches++;
   QB_CHECK_CUDA(cudaGetLastError());
   return 0;
@@ -501,7 +645,7 @@ extern "C" int qb_version(void) { return 100; }
 extern "C" int64_t qb_launch_count(void) { return (int64_t)g_launches.load(); }
 extern "C" void qb_launch_count_reset(void) { g_launches = 0; }
 
-// Three instantiations of one kernel, every stage 128 rows x 64 K, 192 KB of pipeline each:
+// Three instantiations of one kernel, every stage 128 rows x 64 K, 192 KB of pipeline each (plus 32 KB of epilogue buffers):
 //   single pass, n > 128:  128 x 256 tiles, 4 stages (48 KB)
 //   single pass, n <= 128: 128 x 128 tiles, 6 stages (32 KB) - a 256-wide tile would be at least half padding
 //   hi + lo split:         128 x 128 tiles, 3 stages (64 KB)
