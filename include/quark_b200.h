@@ -255,22 +255,15 @@ int qb_lm_flash_attn(const float* q32, const float* k_cache, const float* v_cach
  * Replaces: HF Llama decoder layer on one cached token - QuarkAudio-UniSE/model/llm/llm.py:195-228 driven by
  * llm_sft.py:155-191. */
 int qb_lm_pack_weight(const float* w, int64_t n, int64_t k, qb_half* out /* [n][2k] */, void* stream);
-/* One decoder layer for ONE new token per sequence (B <= 32): x [B,hidden] updated in place; K/V appended at *pos
- * (device int, not modified here).  wqkv = packed [q;k;v] rows [3*hidden, hidden]; scratch q_buf/attn_buf [B,hidden],
+/* One decoder layer for ONE new token per sequence (B <= 32): x [B,hidden] updated in place.  `pos` points at B device ints
+ * (not modified here): row b's RoPE angle and K/V append use pos[b] and its attention reads keys 0..pos[b], so rows whose
+ * conditioning prefixes (llm_sft.py:108-122) differ in length decode together.  wqkv = packed [q;k;v] rows [3*hidden, hidden]; scratch q_buf/attn_buf [B,hidden],
  * mlp_buf [B,inter].  The RMSNorm weights must be FOLDED into the following projection by the caller BEFORE packing
  * (wqkv' = wqkv diag(in_norm), wgate' / wup' likewise with post_norm): the kernels apply only the per-row 1/rms. */
 int qb_lm_decode_layer_tc(float* x, int64_t B, int32_t hidden, int32_t heads, int32_t inter, const qb_half* wqkv,
                           const qb_half* wo, const qb_half* wgate, const qb_half* wup, const qb_half* wdown,
                           float* k_cache, float* v_cache, int32_t Lmax, const int32_t* pos, const float* rope_cos,
                           const float* rope_sin, float* q_buf, float* attn_buf, float* mlp_buf, void* stream);
-/* qb_lm_decode_layer_tc with one position per row: `pos` points at B device ints; row b's RoPE angle and K/V append use
- * pos[b] and its attention reads keys 0..pos[b].  Serves llm_sft.py:155-191 when the rows' conditioning prefixes
- * (llm_sft.py:108-122: task, enroll_sos, enrollment, mix_sos, mix) differ in length, i.e. target-speaker extraction over
- * utterances whose enrollments differ in length. */
-int qb_lm_decode_layer_tc_rows(float* x, int64_t B, int32_t hidden, int32_t heads, int32_t inter, const qb_half* wqkv,
-                               const qb_half* wo, const qb_half* wgate, const qb_half* wup, const qb_half* wdown,
-                               float* k_cache, float* v_cache, int32_t Lmax, const int32_t* pos, const float* rope_cos,
-                               const float* rope_sin, float* q_buf, float* attn_buf, float* mlp_buf, void* stream);
 /* Keys whose K / V rows one lane of the cached-decode attention keeps in flight per trip: 8 (default; a single decode chain is
  * latency-bound) or 4 (several chains sharing the GPU are throughput-bound - LLM_SFT.generate's lanes select it).  Process-wide;
  * read at launch (and therefore fixed inside a captured graph).  Tokens do not depend on it only up to the fp32 summation order of
@@ -278,17 +271,13 @@ int qb_lm_decode_layer_tc_rows(float* x, int64_t B, int32_t hidden, int32_t head
 int qb_lm_set_att_unroll(int32_t keys_per_lane);
 /* Final RMSNorm + packed output head restricted to columns [range[0], range[1]) (device ints; llm_sft.py:148-153)
  * + greedy arg-max (llm.py:286-287, do_sample=False) -> out_ids[b*out_stride + slot[0]]; x_next[b] =
- * embedding[token]; then slot[0]++ and *pos++ (slot is int32[2], second word is scratch).  B <= 32.
+ * embedding[token]; then slot[0]++ and pos[b]++ for every row (pos: B device ints; slot is int32[2], second word is
+ * scratch).  B <= 32.
  * w_head must have final_norm folded in BEFORE packing (w_head' = w_head diag(final_norm)); max_cols and the range
  * width must be multiples of 16; part_val/part_idx: scratch [max_cols/16 * 32]. */
 int qb_lm_head_argmax_tc(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
                          int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride,
                          int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx, void* stream);
-/* qb_lm_head_argmax_tc with one position per row (`pos`: B device ints, each bumped once per step); the decode step of
- * qb_lm_decode_layer_tc_rows (llm_sft.py:155-191, llm.py:286-287 over rows with prefixes of different lengths). */
-int qb_lm_head_argmax_tc_rows(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
-                              int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride,
-                              int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx, void* stream);
 
 /* Teacher-forced loss + accuracy (CustomLlamaModel.loss_function, QuarkAudio-UniSE/model/llm/llm.py:87-104): label-smoothed KL
  * (reduction batchmean) of log_softmax(logits [M, ld >= V]) against the smoothed one-hot targets [M] int64, and the arg-max
@@ -307,13 +296,6 @@ int qb_lm_head_sample_tc(const float* x, int64_t B, int32_t hidden, const qb_hal
                          int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride,
                          int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx, float* logits,
                          float temperature, int32_t top_k, float top_p, const uint32_t* seed, float* debug, void* stream);
-/* qb_lm_head_sample_tc with one position per row (`pos`: B device ints, each bumped once per step); the sampled decode step
- * (llm_sft.py:155-161,184-190, llm.py:253-289) over rows with prefixes of different lengths.  The Philox counter is the same
- * {step, row, call}: a row draws the same uniforms whatever the positions are. */
-int qb_lm_head_sample_tc_rows(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
-                              int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride,
-                              int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx, float* logits,
-                              float temperature, int32_t top_k, float top_p, const uint32_t* seed, float* debug, void* stream);
 
 /* ---------------------------------------------------------------- SSL feature front ends + tokenizer glue (SURVEY 8f.2 / 8f.3)
  * HuBERT-base / WavLM-base-plus (transformers modeling_hubert / modeling_wavlm) as the reference drives them from
@@ -419,18 +401,18 @@ int qb_agg_gather(const float* x, const int32_t* qpos, const int32_t* n_groups, 
                   void* stream);
 
 /* ==========================================================================================================
- * Handle-level contract (SURVEY.md 8b): what a non-Python caller binds.  A handle owns its repacked weight arena,
- * workspace, KV cache and per-device context; every tensor argument is a caller-owned DEVICE pointer (row-major,
- * contiguous, 16-byte aligned); calls are stream-ordered and asynchronous, return 0 / negative, and never synchronise
- * the device after `*_load`.  A handle is bound to the device current at creation and is not thread-safe.
- * The op-level entry points above are what these are built from (csrc/engine.cu); the Python faces
- * (unified_audio_b200/codec.py, llm.py) call these for the product path.
+ * Handle-level contract (SURVEY.md 8b): what a non-Python caller binds for H-Codec-2.0 and its residual quantisers.  A
+ * handle owns its repacked weight arena, workspace and per-device context; every tensor argument is a caller-owned DEVICE
+ * pointer (row-major, contiguous, 16-byte aligned); calls are stream-ordered and asynchronous, return 0 / negative, and
+ * never synchronise the device after `*_load`.  A handle is bound to the device current at creation and is not
+ * thread-safe.  The op-level entry points above are what these are built from (csrc/engine.cu); `Codec`
+ * (unified_audio_b200/codec.py) calls these for the product path.  The UniSE AR-LM has no handle: `LLM_SFT`
+ * (unified_audio_b200/llm.py) composes the op-level LM entry points above, and its C surface is the decode step
+ * (qb_lm_decode_layer_tc + qb_lm_head_argmax_tc / qb_lm_head_sample_tc).
  * ========================================================================================================== */
 typedef struct qb_handle qb_handle;   /* per-device context */
 typedef struct qb_codec qb_codec;     /* H-Codec-2.0 model: weights + workspace */
 typedef struct qb_rvq qb_rvq;         /* one residual vector quantiser (codebooks + search constants) */
-typedef struct qb_lm qb_lm;           /* UniSE AR-LM: weights + workspace */
-typedef struct qb_kv qb_kv;           /* static fp32 KV cache + device-side decode state of one batch */
 
 /* A named fp32 tensor of the reference's state-dict (device pointer, contiguous). */
 typedef struct {
@@ -491,30 +473,6 @@ void qb_rvq_free(qb_rvq* q);
 int qb_rvq_encode_rows(qb_rvq* q, const float* x, int64_t M, int64_t* idx, float* quantized_or_null, void* stream);
 /* idx [M, nq] int64 -> out [M, D] fp32 (sum over layers, q = 0..nq-1 in order) */
 int qb_rvq_decode_rows(qb_rvq* q, const int64_t* idx, int64_t M, float* out, void* stream);
-
-/* UniSE AR-LM hyper-parameters (QuarkAudio-UniSE/conf/config.yaml:138-146; model/llm/llm.py:40-83). */
-typedef struct {
-  int32_t hidden, layers, heads, inter;       /* 512, 12, 8, 2048 (head_dim 64 required) */
-  int32_t vocab;                              /* 3 + global_size + semantic_size = 12291 */
-  int32_t max_positions;                      /* RoPE table rows allocated at load (grown by the caller via a reload) */
-} qb_lm_cfg;
-/* named weights: `layers.{i}.self_attn.{q,k,v,o}_proj.weight`, `layers.{i}.mlp.{gate,up,down}_proj.weight`,
- * `layers.{i}.{input,post_attention}_layernorm.weight`, `norm.weight`, `codec_embedding.weight`, `output_head.weight`. */
-int qb_lm_load(qb_handle* h, const qb_lm_cfg* cfg, const qb_tensor* named_weights, int32_t n, qb_lm** out);
-void qb_lm_free(qb_lm* m);
-int qb_kv_alloc(qb_lm* m, int64_t B, int32_t Lmax, qb_kv** out);
-void qb_kv_free(qb_kv* kv);
-int qb_kv_reset(qb_kv* kv, void* stream);
-/* CustomLlamaModel.llm_forward on a prefix (llm.py:150-228; llm_sft.py:130-135): embeds [B,P,hidden] appended to the
- * cache at its current length; last_hidden [B,P,hidden] = final-RMSNorm output (may be NULL). */
-int qb_lm_prefill(qb_lm* m, const float* embeds, int64_t B, int64_t P, qb_kv* kv, float* last_hidden, void* stream);
-/* n_steps cached greedy steps (llm_sft.py:137-193 with do_sample=False): starts from token `first_token`'s embedding,
- * each step restricts the head to columns [col_lo, col_hi) and feeds the arg-max back; out_ids [B, n_steps] int64 (raw
- * vocabulary ids).  B <= 32. */
-int qb_lm_decode_greedy(qb_lm* m, qb_kv* kv, int64_t B, int32_t first_token, int32_t n_steps, int32_t col_lo,
-                        int32_t col_hi, int64_t* out_ids, void* stream);
-/* Teacher-forced logits (llm_sft.py:81-86): embeds [B,L,hidden] -> logits [B,L,vocab] fp32 (fresh context, no cache kept). */
-int qb_lm_forward_logits(qb_lm* m, const float* embeds, int64_t B, int64_t L, float* logits, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,5 +1,5 @@
 """The handle-level C ABI (include/quark_b200.h "Handle-level contract", SURVEY.md 8b) driven through ctypes ONLY -
-qb_init / qb_codec_load / qb_codec_encode / qb_codec_decode / qb_rvq_* / qb_lm_* - against the golden fixtures generated from
+qb_init / qb_codec_load / qb_codec_encode / qb_codec_decode / qb_rvq_* - against the golden fixtures generated from
 the reference's own modules and against the oracle.  No Python orchestration of kernels on this path: torch only allocates
 the device buffers whose pointers are passed."""
 import ctypes as C
@@ -142,68 +142,4 @@ def test_codec_c_abi_roundtrip_against_reference_golden(lib, name):
     assert bool((idx.cpu()[safe] == oidx[safe]).all())
     assert torch.equal(out.cpu(), orvq.rvq_decode(idx.cpu(), cb_a)) and rel(quant, out) < 1e-6
     lib.qb_codec_free(codec)
-    lib.qb_handle_free(h)
-
-
-def test_lm_c_abi_against_oracle(lib):
-    """qb_lm_load / qb_kv_alloc / qb_lm_prefill / qb_lm_decode_greedy / qb_lm_forward_logits through ctypes only."""
-    from oracle import llama
-    from unified_audio_b200._lib import LmCfg
-    cfg = llama.LM_FULL
-    b = cfg["llm_base_config"]
-    sd = llama.make_lm_state_dict(cfg, 7, 2.0)
-    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    h, lm, kv = C.c_void_p(), C.c_void_p(), C.c_void_p()
-    _check(lib, lib.qb_init(0, C.byref(h)))
-    lc = LmCfg()
-    lc.hidden, lc.layers, lc.heads, lc.inter = b["hidden_size"], b["num_layers"], b["num_attention_heads"], 4 * b["hidden_size"]
-    lc.vocab, lc.max_positions = 3 + b["global_size"] + b["semantic_size"], 1024
-    arr, keep = _tensors(sd)
-    _check(lib, lib.qb_lm_load(h, C.byref(lc), arr, len(sd), C.byref(lm)))
-    del keep
-    B, P, T = 4, 40, 10
-    g = torch.Generator().manual_seed(31)
-    mix = torch.randn(B, P - 2, 768, generator=g)
-    prefix = llama._prefix(sd, cfg, "se", None, mix)                     # [B, P, 512] (host-side embedding glue)
-    ref_h, _ = llama.llm_forward(sd, cfg, prefix)
-    _check(lib, lib.qb_kv_alloc(lm, B, 128, C.byref(kv)))
-    # the prefix in two prefills on the same cache: the second continues it (lm_qkv_prep + lm_flash_attn at pos0 = 25)
-    P1 = 25
-    pre1, pre2 = prefix[:, :P1].cuda().contiguous(), prefix[:, P1:].cuda().contiguous()
-    hid1, hid2 = torch.empty(B, P1, 512, device="cuda"), torch.empty(B, P - P1, 512, device="cuda")
-    _check(lib, lib.qb_lm_prefill(lm, pre1.data_ptr(), B, P1, kv, hid1.data_ptr(), stream))
-    _check(lib, lib.qb_lm_prefill(lm, pre2.data_ptr(), B, P - P1, kv, hid2.data_ptr(), stream))
-    goff, soff = 3, 3 + b["global_size"]
-    gids = torch.empty(B, 33, dtype=torch.int64, device="cuda")
-    sids = torch.empty(B, T, dtype=torch.int64, device="cuda")
-    _check(lib, lib.qb_lm_decode_greedy(lm, kv, B, 0, 33, goff, goff + b["global_size"], gids.data_ptr(), stream))
-    _check(lib, lib.qb_lm_decode_greedy(lm, kv, B, 1, T, soff, soff + b["semantic_size"], sids.data_ptr(), stream))
-    torch.cuda.synchronize()
-    e_pre = max(rel(hid1, ref_h[:, :P1]), rel(hid2, ref_h[:, P1:]))
-    og, os_, margins = llama.sft_generate(sd, cfg, "se", None, mix, T, return_margins=True)
-    got = torch.cat([gids.cpu() - goff, sids.cpu() - soff], 1)
-    want = torch.cat([og, torch.zeros(B, 1, dtype=torch.long), os_], 1)
-    margins[:, 32] = 1.0
-    nbad = 0
-    for i in range(B):
-        d = (got[i] != want[i]).nonzero().flatten()
-        d = d[d != 32]
-        if len(d):
-            nbad += 1
-            assert float(margins[i, int(d[0])]) < 1e-4, "greedy token differs at a safe margin"
-    # teacher-forced logits
-    L = 24
-    x = torch.randn(B, L, 512, generator=g)
-    ref2, _ = llama.llm_forward(sd, cfg, x)
-    ref_logits = torch.nn.functional.linear(ref2, sd["output_head.weight"])
-    logits = torch.empty(B, L, lc.vocab, device="cuda")
-    xd = x.cuda().contiguous()
-    _check(lib, lib.qb_lm_forward_logits(lm, xd.data_ptr(), B, L, logits.data_ptr(), stream))
-    torch.cuda.synchronize()
-    e_log = rel(logits, ref_logits)
-    print(f"[c-abi lm] prefill rel {e_pre:.2e}; greedy: {B - nbad}/{B} sequences identical (others diverge at unsafe margins); logits rel {e_log:.2e}")
-    assert e_pre < TOL and e_log < TOL
-    assert lib.qb_lm_decode_greedy(lm, kv, B, 1, 500, soff, soff + 8192, sids.data_ptr(), stream) < 0     # cache too small: error code
-    lib.qb_kv_free(kv)
-    lib.qb_lm_free(lm)
     lib.qb_handle_free(h)

@@ -50,11 +50,17 @@ def _skinny_ref(x, w, norm):
     return val, SKINNY * S + 2.0 ** -24 * (3 * K // 16 + 16) * val.abs() + 1e-30
 
 
-def _attn_ref(q, K, V):
-    """fp64 softmax(q K^T) V for q [B, h, 64], K / V [B, h, n, 64], and the bound of an fp32 kernel: 1e-6 of the largest value,
-    plus the fp32 rounding of each 64-term score (2^-22 of sum |q_d k_d|) carried through the softmax weights onto V"""
+def _attn_ref(q, K, V, n=None):
+    """fp64 softmax(q K^T) V for q [B, h, 64], K / V [B, h, T, 64], and the bound of an fp32 kernel: 1e-6 of the largest value,
+    plus the fp32 rounding of each 64-term score (2^-22 of sum |q_d k_d|) carried through the softmax weights onto V.
+    n (int [B]): row b attends to its keys 0 .. n[b] - 1 only (the rest may hold anything); default all T"""
     q, K, V = q.double(), K.double(), V.double()
+    if n is not None:
+        keep = (torch.arange(K.shape[2], device=K.device)[None] < n.to(K.device)[:, None])[:, None, :, None]
+        K, V = K.masked_fill(~keep, 0.0), V.masked_fill(~keep, 0.0)
     sc = torch.einsum("bhd,bhtd->bht", q, K)
+    if n is not None:
+        sc = sc.masked_fill(~keep[..., 0], float("-inf"))
     ref = torch.einsum("bht,bhtd->bhd", torch.softmax(sc, -1), V)
     ds = 2.0 ** -22 * torch.einsum("bhd,bhtd->bht", q.abs(), K.abs()).amax(-1)
     bound = F32_TOL * ref.abs().max() + 2.0 * ds[..., None] * V.abs().amax(2) + 1e-30
@@ -110,46 +116,51 @@ def test_lm_pack_weight(lib):
 @pytest.mark.parametrize("B", [1, 5, 8, 9, 31, 32])
 def test_lm_decode_layer(lib, hidden, heads, inter, B):
     """One lm_decode_layer_tc (QKV + RoPE + cache append, decode attention, o_proj + residual, gate/up + SwiGLU, down + residual)
-    against an fp64 HF Llama decoder layer, stage by stage from the kernel's own inputs to that stage"""
+    against an fp64 HF Llama decoder layer, stage by stage from the kernel's own inputs to that stage; every row at one position,
+    then the rows at different positions (prefixes of different lengths), each row against its own position's reference"""
     from unified_audio_b200 import ops
     H = hidden
     f, Lw = _layer(H, inter, 10 * hidden + B)
     Lmax = 48
     cos, sin = ops.rope_tables(Lmax + 16, 64, DEV)                # the table is longer than the cache
-    for pos in (0, 37, Lmax - 1):
-        seed = 1000 * B + pos
+    cases = [[pos] * B for pos in (0, 37, Lmax - 1)] + [[(17 * b + Lmax - 1) % Lmax for b in range(B)]]
+    for pos in cases:
+        seed = 1000 * B + pos[0]
         x_all = torch.full((33, H), SENT, device=DEV)
         x_all[:B] = _rnd((B, H), seed, 1.5) + 0.2
         kc, vc = _rnd((B, heads, Lmax, 64), seed + 1), _rnd((B, heads, Lmax, 64), seed + 2)
-        kc[:, :, pos:] = float("nan")                            # row pos is the kernel's to write, rows above are never read
-        vc[:, :, pos:] = float("nan")
+        for b, p in enumerate(pos):                              # row p is the kernel's to write, rows above are never read
+            kc[b, :, p:] = float("nan")
+            vc[b, :, p:] = float("nan")
         kc0, vc0 = _bits(kc).clone(), _bits(vc).clone()
         q_all, a_all = torch.full((33, H), SENT, device=DEV), torch.full((33, H), SENT, device=DEV)
         m_all = torch.full((33, inter), SENT, device=DEV)
-        pos_t = torch.tensor([pos], dtype=torch.int32, device=DEV)
+        pos_t = torch.tensor(pos, dtype=torch.int32, device=DEV)
         x0 = x_all[:B].clone()
         ops.lm_decode_layer_tc(x_all[:B], B, H, heads, inter, Lw, kc, vc, Lmax, pos_t, cos, sin, q_all[:B], a_all[:B], m_all[:B])
         torch.cuda.synchronize()
-        tag = f"decode layer {H}/{heads}/{inter} B={B} pos={pos}"
+        tag = f"decode layer {H}/{heads}/{inter} B={B} pos={pos[0] if len(set(pos)) == 1 else 'per row'}"
         for nm, buf in (("x", x_all), ("q_buf", q_all), ("attn_buf", a_all), ("mlp_buf", m_all)):
             assert bool((buf[B:] == SENT).all()), f"{tag}: {nm} written past row B"
-        assert int(pos_t) == pos, "the layer must not move the position"
-        # QKV + RoPE at pos (q pre-scaled by 1/sqrt(64)), K/V appended at row pos
+        assert pos_t.tolist() == pos, "the layer must not move the positions"
+        # QKV + RoPE at each row's position (q pre-scaled by 1/sqrt(64)), K/V appended at that row of the cache
         val, bnd = _skinny_ref(x0, f["wqkv"], True)
         sh = lambda t: t.reshape(B, 3, heads, 64)
         val, bnd = sh(val), sh(bnd)
-        c, s = cos[pos].double(), sin[pos].double()
+        pl, bi = pos_t.long(), torch.arange(B, device=DEV)
+        c, s = cos[pl].double()[:, None], sin[pl].double()[:, None]
         q_ref, q_bnd = _rope_ref(val[:, 0], bnd[:, 0], c, s)
         k_ref, k_bnd = _rope_ref(val[:, 1], bnd[:, 1], c, s)
         _check(f"{tag} q_buf", q_all[:B].view(B, heads, 64), q_ref * 0.125, q_bnd * 0.125)
-        _check(f"{tag} k row", kc[:, :, pos], k_ref, k_bnd)
-        _check(f"{tag} v row", vc[:, :, pos], val[:, 2], bnd[:, 2])
-        rows = torch.ones(Lmax, dtype=torch.bool, device=DEV)
-        rows[pos] = False
-        assert torch.equal(_bits(kc)[:, :, rows], kc0[:, :, rows]) and torch.equal(_bits(vc)[:, :, rows], vc0[:, :, rows]), \
-            f"{tag}: a cache row other than pos changed"
-        # attention over rows 0..pos of the kernel's cache with the kernel's q
-        a_ref, a_bnd, _ = _attn_ref(q_all[:B].view(B, heads, 64), kc[:, :, :pos + 1], vc[:, :, :pos + 1])
+        _check(f"{tag} k row", kc[bi, :, pl], k_ref, k_bnd)
+        _check(f"{tag} v row", vc[bi, :, pl], val[:, 2], bnd[:, 2])
+        rows = torch.ones(B, Lmax, dtype=torch.bool, device=DEV)
+        rows[bi, pl] = False
+        other = lambda t: t.transpose(1, 2)[rows]
+        assert torch.equal(other(_bits(kc)), other(kc0)) and torch.equal(other(_bits(vc)), other(vc0)), \
+            f"{tag}: a cache row other than the row's position changed"
+        # attention of each row over its rows 0..pos[b] of the kernel's cache with the kernel's q
+        a_ref, a_bnd, _ = _attn_ref(q_all[:B].view(B, heads, 64), kc, vc, pos_t + 1)
         _check(f"{tag} attn_buf", a_all[:B].view(B, heads, 64), a_ref, a_bnd)
         a_ref = a_ref.reshape(B, H)
         # o_proj + residual (not observable on its own: its bound carries into the MLP and the final x)
@@ -188,7 +199,7 @@ def test_lm_decode_attention(lib, unroll, n):
             kc[:, :, n:] = float("nan")
             vc[:, :, n:] = float("nan")
             qb, ab, mb = torch.empty(B, H, device=DEV), torch.full((B, H), SENT, device=DEV), torch.empty(B, 64, device=DEV)
-            ops.lm_decode_layer_tc(x, B, H, heads, 64, Lw, kc, vc, Lmax, torch.tensor([pos], dtype=torch.int32, device=DEV),
+            ops.lm_decode_layer_tc(x, B, H, heads, 64, Lw, kc, vc, Lmax, torch.full((B,), pos, dtype=torch.int32, device=DEV),
                                    cos, sin, qb, ab, mb)
             torch.cuda.synchronize()
             ref, bound, sc = _attn_ref(qb.view(B, heads, 64), kc[:, :, :n], vc[:, :, :n])
@@ -275,7 +286,7 @@ def test_lm_head_argmax(lib, width):
     """Greedy head: the arg-max of the range over planted exact logits.  The row maximum just outside the range (lo - 1 and
     hi .. hi + 15, also past the end of the vocabulary) never wins; ties inside a CTA's two 8-column halves, across lanes and
     across CTAs resolve to the lowest id as torch.argmax does; x_next is emb[token] bit for bit; several back-to-back steps
-    advance pos and slot once each and fill out_ids column by column"""
+    advance every row's position and slot once each and fill out_ids column by column"""
     from unified_audio_b200 import ops
     gs = ss = width
     V = 3 + gs + ss
@@ -301,7 +312,8 @@ def test_lm_head_argmax(lib, width):
         steps = 4
         out_ids = torch.full((B, steps + 2), -7, dtype=torch.int64, device=DEV)
         x_next = torch.full((B + 1, HK), SENT, device=DEV)
-        pos = torch.tensor([5], dtype=torch.int32, device=DEV)
+        pos_all = torch.arange(B + 1, dtype=torch.int32, device=DEV) + 5       # one position per row, and a sentinel after them
+        pos = pos_all[:B]
         slot = torch.zeros(2, dtype=torch.int32, device=DEV)
         pv = torch.zeros(max_cols // 16 + 1, 32, device=DEV)
         pi = torch.zeros(max_cols // 16 + 1, 32, dtype=torch.int32, device=DEV)
@@ -318,7 +330,8 @@ def test_lm_head_argmax(lib, width):
         assert bool((out_ids[:, steps:] == -7).all()), "out_ids written past the steps taken"
         assert torch.equal(x_next[:B], emb[want]), "x_next must be emb[token]"
         assert bool((x_next[B] == SENT).all())
-        assert int(pos) == 5 + steps and slot.tolist() == [steps, 0], f"pos {int(pos)} slot {slot.tolist()}"
+        want_pos = torch.arange(B + 1, dtype=torch.int32) + 5 + torch.tensor([steps] * B + [0], dtype=torch.int32)
+        assert torch.equal(pos_all.cpu(), want_pos) and slot.tolist() == [steps, 0], f"pos {pos_all.tolist()} slot {slot.tolist()}"
 
 
 @pytest.mark.parametrize("B", [1, 9, 32])
@@ -337,7 +350,7 @@ def test_lm_head_logits(lib, B):
         seed = torch.tensor([1, 2, 0, 0], dtype=torch.int32, device=DEV)
         ops.lm_head_sample_tc(x, B, Hd, wp, torch.tensor([lo, hi], dtype=torch.int32, device=DEV), max_cols, emb,
                               torch.empty(B, Hd, device=DEV), torch.zeros(B, 1, dtype=torch.int64, device=DEV), 1,
-                              torch.zeros(1, dtype=torch.int32, device=DEV), torch.zeros(2, dtype=torch.int32, device=DEV),
+                              torch.zeros(B, dtype=torch.int32, device=DEV), torch.zeros(2, dtype=torch.int32, device=DEV),
                               torch.zeros(max_cols // 16 + 1, 32, device=DEV),
                               torch.zeros(max_cols // 16 + 1, 32, dtype=torch.int32, device=DEV), logits, 0.8, 50, 0.95, seed)
         torch.cuda.synchronize()
@@ -361,7 +374,7 @@ def _run_sampler(lo, width, V, logits_vals, temperature, top_k, top_p, seed=9876
     emb = _rnd((V + 16, HK), 5)
     x_next = torch.empty(B, HK, device=DEV)
     out_ids = torch.full((B, 16), -7, dtype=torch.int64, device=DEV)
-    pos = torch.tensor([11], dtype=torch.int32, device=DEV)
+    pos = torch.full((B,), 11, dtype=torch.int32, device=DEV)
     slot0_d = torch.tensor([slot0, 0], dtype=torch.int32, device=DEV)
     slot = slot0_d.clone()
     pv = torch.zeros(max_cols // 16 + 1, 32, device=DEV)

@@ -1,5 +1,5 @@
 """LLM_SFT.generate with ragged conditioning prefixes (`enroll_lengths`): rows whose enrollments differ in length decode in one call,
-with one position per row in the decode kernels (qb_lm_decode_layer_tc_rows / qb_lm_head_{argmax,sample}_tc_rows).  Reduced widths,
+with one position per row in the decode kernels (qb_lm_decode_layer_tc / qb_lm_head_{argmax,sample}_tc).  Reduced widths,
 as tests/test_lm_kernels_gpu.py.
 
 Every comparison holds the decode attention's keys in flight (att_unroll / lane_att_unroll) equal on both sides: 8 on a single chain

@@ -41,10 +41,6 @@ class CodecCfg(C.Structure):     # qb_codec_cfg
                                                                                              ("precision", C.c_int32)]
 
 
-class LmCfg(C.Structure):        # qb_lm_cfg
-    _fields_ = [(n, C.c_int32) for n in ("hidden", "layers", "heads", "inter", "vocab", "max_positions")]
-
-
 TAP_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64)
 PRECISION_CODES = {"mixed": 0, "accurate": 1, "fast": 2, "mixed_dec16": 3}
 
@@ -96,9 +92,6 @@ SIGNATURES = {
                                         _vp, _vp, _vp, _vp]),
     "qb_lm_set_att_unroll": (C.c_int, [_i32]),
     "qb_lm_head_argmax_tc": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
-    "qb_lm_decode_layer_tc_rows": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp,
-                                             _vp, _vp, _vp, _vp]),
-    "qb_lm_head_argmax_tc_rows": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "qb_ssl_conv0_workspace_bytes": (C.c_int64, [_i64, _i64, _i32]),
     "qb_ssl_conv0_gn_gelu": (C.c_int, [_vp, _i64, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "qb_ssl_conv0_bias": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
@@ -138,19 +131,9 @@ SIGNATURES = {
     "qb_rvq_free": (None, [_vp]),
     "qb_rvq_encode_rows": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp]),
     "qb_rvq_decode_rows": (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
-    "qb_lm_load": (C.c_int, [_vp, C.POINTER(LmCfg), C.POINTER(Tensor), _i32, C.POINTER(_vp)]),
-    "qb_lm_free": (None, [_vp]),
-    "qb_kv_alloc": (C.c_int, [_vp, _i64, _i32, C.POINTER(_vp)]),
-    "qb_kv_free": (None, [_vp]),
-    "qb_kv_reset": (C.c_int, [_vp, _vp]),
-    "qb_lm_prefill": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp]),
-    "qb_lm_decode_greedy": (C.c_int, [_vp, _vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
-    "qb_lm_forward_logits": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
     "qb_lm_loss": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _f32, _vp, _vp, _vp]),
     "qb_lm_head_sample_tc": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _i32,
                                        _f32, _vp, _vp, _vp]),
-    "qb_lm_head_sample_tc_rows": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _f32,
-                                            _i32, _f32, _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -3,8 +3,7 @@
 // qb_codec_*: H-Codec-2.0 `Codec.encode` / `Codec.decode` (QuarkAudio-HCodec/HCodec-2.0/vq/codec.py:75-99) as ONE C call each:
 // the handle owns the repacked weights (fp16 planes, conv taps, interleaved SwiGLU rows, LSTM unit-major slices, DFT matrices
 // built in fp64), the zero-padded channel-last workspace and the RoPE tables; the call enqueues ~340 kernels of this library on the
-// caller's stream.  qb_rvq_*: the two residual quantisers row-level.  qb_lm_*: the UniSE AR-LM prefill / greedy decode /
-// teacher-forced logits (QuarkAudio-UniSE/model/llm/llm.py:150-228, llm_sft.py:93-195).
+// caller's stream.  qb_rvq_*: the two residual quantisers row-level.
 // Host code only orchestrates: every arithmetic op is one of the op-level kernels behind the same header.
 #include <atomic>
 #include <cmath>
@@ -118,13 +117,6 @@ __global__ void add_vec_kernel(const float* __restrict__ a, const float* __restr
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) out[i] = a[i] + b[i];
 }
-// out[r, c] = w[r, c] * g[c]   (RMSNorm weight folded into the following projection)
-__global__ void scale_cols_kernel(const float* __restrict__ w, const float* __restrict__ g, long long rows, int cols,
-                                  float* __restrict__ out) {
-  const long long total = rows * cols;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
-    out[i] = w[i] * g[i % cols];
-}
 // RVQ search constants in fp64: consts[q*K + j] = -|e_qj|^2 / 2, then K values of -2; e2 per code for the host max
 __global__ void rvq_consts_kernel(const float* __restrict__ cb, int nq, int K, int D, float* __restrict__ consts, float* __restrict__ e2) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -141,11 +133,6 @@ __global__ void gather_rows_kernel(const float* __restrict__ table, const int64_
   const long long total = rows * cols;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
     out[i] = table[ids[i / cols] * cols + i % cols];
-}
-__global__ void fill_rows_kernel(const float* __restrict__ row, long long rows, int cols, float* __restrict__ out) {
-  const long long total = rows * cols;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
-    out[i] = row[i % cols];
 }
 // [B*N, nq] <-> [B, nq, N] int64 (the reference returns codes transposed, vq/codec.py:85-86)
 __global__ void codes_rows_to_bqn_kernel(const int64_t* __restrict__ rows, int B, int N, int nq, int64_t* __restrict__ out) {
@@ -946,263 +933,4 @@ extern "C" int qb_codec_decode(qb_codec* c, const int64_t* ac_codes, const int64
   g_launches++;
   QB_TRY(qb_rvq_decode(rows, c->q[1]->cb, B * N, Dq, c->cfg.codebook_size, nq, z, 2 * Dq, Dq, stream));
   return decode_z(c, z, B, N, wav, stream);
-}
-
-// ================================================================== UniSE AR-LM handles
-struct LmLayerW {
-  const float *in_w, *post_w;
-  PlanesD wqkv, wo, wgu, wd;                         // prefill / teacher-forced path: 3-term split planes
-  qb_half *wqkv_p, *wo_p, *wg_p, *wu_p, *wd_p;       // decode path: RMSNorm-folded, packed {hi[4], lo[4]} groups
-};
-struct qb_lm {
-  qb_handle* h;
-  qb_lm_cfg cfg;
-  Arena arena;
-  Workspace ws;
-  std::vector<LmLayerW> layers;
-  const float *norm, *emb, *rcos, *rsin;
-  PlanesD head;
-  qb_half* head_p;
-};
-struct qb_kv {
-  qb_lm* m;
-  Arena arena;
-  int64_t B;
-  int Lmax, length;
-  std::vector<float*> k, v;
-  int32_t *pos, *rng, *slot;
-  float *xs, *qb_, *ab, *mb, *pv;
-  int32_t* pi;
-  int max_cols;
-};
-
-namespace qb {
-__global__ void set_i32_kernel(int32_t* p, int32_t a, int32_t b, int n) {
-  if (threadIdx.x == 0) { p[0] = a; if (n > 1) p[1] = b; }
-}
-static int lm_pack(Arena& arena, const float* w, long long n, long long k, const float* fold /* [k] or NULL */, qb_half** out) {
-  QB_TRY(arena.alloc((void**)out, (size_t)n * k * 4, false));
-  const float* src = w;
-  float* tmp = nullptr;
-  if (fold) {
-    QB_CHECK_CUDA(cudaMalloc(&tmp, (size_t)n * k * 4));
-    scale_cols_kernel<<<grid_for(n * k), 256>>>(w, fold, n, (int)k, tmp);
-    src = tmp;
-  }
-  int e = qb_lm_pack_weight(src, n, k, *out, nullptr);
-  if (tmp) { cudaDeviceSynchronize(); cudaFree(tmp); }
-  return e;
-}
-}  // namespace qb
-
-extern "C" int qb_lm_load(qb_handle* h, const qb_lm_cfg* cfg, const qb_tensor* named, int32_t n, qb_lm** out) {
-  QB_REQUIRE(h && cfg && named && out && n > 0, "lm_load: bad args");
-  QB_REQUIRE(cfg->hidden == cfg->heads * 64 && cfg->hidden % 128 == 0 && cfg->inter % 16 == 0 && cfg->layers >= 1 && cfg->max_positions >= 1,
-             "lm_load: kernels assume head_dim 64 and hidden %% 128 == 0 (shipped config: 512 = 8 x 64)");
-  QB_CHECK_CUDA(cudaSetDevice(h->device));
-  WeightTable wt;
-  QB_TRY(wt.init(named, n));
-  qb_lm* m = new qb_lm();
-  struct Guard { qb_lm* m; ~Guard() { delete m; } } guard{m};
-  m->h = h; m->cfg = *cfg;
-  Loader L(wt, m->arena);
-  const int H = cfg->hidden, I = cfg->inter;
-  m->layers.resize(cfg->layers);
-  for (int i = 0; i < cfg->layers; ++i) {
-    const std::string p = "layers." + std::to_string(i) + ".";
-    LmLayerW& l = m->layers[i];
-    QB_TRY(L.f32(&l.in_w, p + "input_layernorm.weight"));
-    QB_TRY(L.f32(&l.post_w, p + "post_attention_layernorm.weight"));
-    const qb_tensor *wq, *wk, *wv, *wo, *wg, *wu, *wd;
-    QB_TRY(L.get(&wq, p + "self_attn.q_proj.weight", 2)); QB_TRY(L.get(&wk, p + "self_attn.k_proj.weight", 2));
-    QB_TRY(L.get(&wv, p + "self_attn.v_proj.weight", 2)); QB_TRY(L.get(&wo, p + "self_attn.o_proj.weight", 2));
-    QB_TRY(L.get(&wg, p + "mlp.gate_proj.weight", 2)); QB_TRY(L.get(&wu, p + "mlp.up_proj.weight", 2));
-    QB_TRY(L.get(&wd, p + "mlp.down_proj.weight", 2));
-    float* tmp;
-    QB_CHECK_CUDA(cudaMalloc(&tmp, (size_t)(3 * H * H > 2 * I * H ? 3 * H * H : 2 * I * H) * 4));
-    const qb_tensor* qkv3[3] = {wq, wk, wv};
-    for (int j = 0; j < 3; ++j) cudaMemcpy(tmp + (size_t)j * H * H, qkv3[j]->data, (size_t)H * H * 4, cudaMemcpyDeviceToDevice);
-    int e = L.planes_from(&l.wqkv, tmp, 3LL * H * H, true);
-    if (!e) e = lm_pack(m->arena, tmp, 3 * H, H, l.in_w, &l.wqkv_p);
-    if (!e) {
-      interleave_rows_kernel<<<grid_for((long long)I * H), 256>>>(wg->data, wu->data, I, H, tmp);
-      e = L.planes_from(&l.wgu, tmp, 2LL * I * H, true);
-    }
-    cudaDeviceSynchronize();
-    cudaFree(tmp);
-    QB_TRY(e);
-    QB_TRY(L.planes_from(&l.wo, wo->data, (long long)H * H, true));
-    QB_TRY(L.planes_from(&l.wd, wd->data, (long long)H * I, true));
-    QB_TRY(lm_pack(m->arena, wo->data, H, H, nullptr, &l.wo_p));
-    QB_TRY(lm_pack(m->arena, wg->data, I, H, l.post_w, &l.wg_p));
-    QB_TRY(lm_pack(m->arena, wu->data, I, H, l.post_w, &l.wu_p));
-    QB_TRY(lm_pack(m->arena, wd->data, H, I, nullptr, &l.wd_p));
-  }
-  QB_TRY(L.f32(&m->norm, "norm.weight"));
-  QB_TRY(L.f32(&m->emb, "codec_embedding.weight"));
-  const qb_tensor* wh;
-  QB_TRY(L.get(&wh, "output_head.weight", 2));
-  QB_REQUIRE(wh->shape[0] == cfg->vocab && wh->shape[1] == H, "lm_load: output_head.weight shape mismatch");
-  QB_TRY(L.planes_from(&m->head, wh->data, (long long)cfg->vocab * H, true));
-  QB_TRY(lm_pack(m->arena, wh->data, cfg->vocab, H, m->norm, &m->head_p));
-  {  // RoPE tables (HF LlamaRotaryEmbedding: theta 1e4, head_dim 64; llm.py:187)
-    const int R = cfg->max_positions;
-    std::vector<float> cs((size_t)R * 64), sn((size_t)R * 64);
-    for (int t = 0; t < R; ++t)
-      for (int i = 0; i < 32; ++i) {
-        const float inv = 1.0f / powf(10000.0f, (float)(2 * i) / 64.0f);
-        const float fr = (float)t * inv;
-        cs[(size_t)t * 64 + i] = cs[(size_t)t * 64 + i + 32] = cosf(fr);
-        sn[(size_t)t * 64 + i] = sn[(size_t)t * 64 + i + 32] = sinf(fr);
-      }
-    float *dc, *ds;
-    QB_TRY(m->arena.alloc((void**)&dc, cs.size() * 4, false));
-    QB_TRY(m->arena.alloc((void**)&ds, sn.size() * 4, false));
-    QB_CHECK_CUDA(cudaMemcpy(dc, cs.data(), cs.size() * 4, cudaMemcpyHostToDevice));
-    QB_CHECK_CUDA(cudaMemcpy(ds, sn.data(), sn.size() * 4, cudaMemcpyHostToDevice));
-    m->rcos = dc; m->rsin = ds;
-  }
-  QB_CHECK_CUDA(cudaDeviceSynchronize());
-  QB_CHECK_CUDA(cudaGetLastError());
-  guard.m = nullptr;
-  *out = m;
-  return 0;
-}
-extern "C" void qb_lm_free(qb_lm* m) { delete m; }
-
-extern "C" int qb_kv_alloc(qb_lm* m, int64_t B, int32_t Lmax, qb_kv** out) {
-  QB_REQUIRE(m && out && B >= 1 && Lmax >= 1, "kv_alloc: bad args");
-  QB_REQUIRE(Lmax <= m->cfg.max_positions, "kv_alloc: Lmax %d exceeds the RoPE table (%d rows; reload with a larger max_positions)", Lmax,
-             m->cfg.max_positions);
-  qb_kv* kv = new qb_kv();
-  struct Guard { qb_kv* k; ~Guard() { delete k; } } guard{kv};
-  kv->m = m; kv->B = B; kv->Lmax = Lmax; kv->length = 0;
-  const int H = m->cfg.hidden, heads = m->cfg.heads;
-  kv->k.resize(m->cfg.layers); kv->v.resize(m->cfg.layers);
-  for (int i = 0; i < m->cfg.layers; ++i) {
-    QB_TRY(kv->arena.alloc((void**)&kv->k[i], (size_t)B * heads * Lmax * 64 * 4, true));
-    QB_TRY(kv->arena.alloc((void**)&kv->v[i], (size_t)B * heads * Lmax * 64 * 4, true));
-  }
-  kv->max_cols = (int)pad_to(m->cfg.vocab, 16);
-  QB_TRY(kv->arena.alloc((void**)&kv->pos, 16, true));
-  QB_TRY(kv->arena.alloc((void**)&kv->rng, 16, true));
-  QB_TRY(kv->arena.alloc((void**)&kv->slot, 16, true));
-  QB_TRY(kv->arena.alloc((void**)&kv->xs, (size_t)B * H * 4, true));
-  QB_TRY(kv->arena.alloc((void**)&kv->qb_, (size_t)B * H * 4, true));
-  QB_TRY(kv->arena.alloc((void**)&kv->ab, (size_t)B * H * 4, true));
-  QB_TRY(kv->arena.alloc((void**)&kv->mb, (size_t)B * m->cfg.inter * 4, true));
-  QB_TRY(kv->arena.alloc((void**)&kv->pv, (size_t)(kv->max_cols / 16 + 1) * 32 * 4, true));
-  QB_TRY(kv->arena.alloc((void**)&kv->pi, (size_t)(kv->max_cols / 16 + 1) * 32 * 4, true));
-  guard.k = nullptr;
-  *out = kv;
-  return 0;
-}
-extern "C" void qb_kv_free(qb_kv* kv) { delete kv; }
-extern "C" int qb_kv_reset(qb_kv* kv, void* stream) {
-  QB_REQUIRE(kv != nullptr, "kv_reset: null cache");
-  kv->length = 0;
-  set_i32_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(kv->pos, 0, 0, 1);
-  QB_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-namespace qb {
-// llm.py:150-228 over x [B*L, H] (in place); K/V appended at kv->length
-static int lm_layers_prefill(qb_lm* m, float* x, int64_t B, int64_t L, qb_kv* kv, void* st) {
-  const int H = m->cfg.hidden, heads = m->cfg.heads, I = m->cfg.inter;
-  const int64_t M = B * L;
-  const int pos0 = kv->length;
-  QB_REQUIRE(pos0 + L <= kv->Lmax, "lm_prefill: KV cache too small (%d + %lld > %d)", pos0, (long long)L, kv->Lmax);
-  QB_REQUIRE(kv->B == B, "lm_prefill: cache built for batch %lld, got %lld", (long long)kv->B, (long long)B);
-  PlanesD t1, hid;
-  float *qkv, *q32;
-  QB_TRY(m->ws.planes(&t1, "t1", (size_t)M * H, true));
-  QB_TRY(m->ws.planes(&hid, "hid", (size_t)M * I, true));
-  QB_TRY(m->ws.f32(&qkv, "qkv", (size_t)M * 3 * H));
-  QB_TRY(m->ws.f32(&q32, "q32", (size_t)M * H));
-  // prefill from an empty cache: causal wgmma attention over the qkv rows (attention_umma.cu); a continuation reads the cache
-  const bool umma = pos0 == 0;
-  void* att_ws = nullptr;
-  if (umma) QB_TRY(m->ws.get(&att_ws, "att5_ws", (size_t)qb_attention_umma_workspace_bytes(B, L, heads, 64, 1)));
-  for (int i = 0; i < m->cfg.layers; ++i) {
-    const LmLayerW& w = m->layers[i];
-    QB_TRY(qb_rmsnorm(x, w.in_w, 1e-6f, M, H, nullptr, (qb_half*)t1.hi, (qb_half*)t1.lo, st));
-    QB_TRY(lin(t1, M, H, w.wqkv, 3 * H).out32(qkv, 3 * H, M, 0).run(st));
-    QB_TRY(qb_lm_qkv_prep(qkv, B, L, heads, pos0, m->rcos, m->rsin, q32, kv->k[i], kv->v[i], kv->Lmax, st));
-    if (umma) QB_TRY(qb_attention_umma(qkv, B, L, heads, 64, m->rcos, m->rsin, (qb_half*)t1.hi, (qb_half*)t1.lo, 1, 1, att_ws, st));
-    else QB_TRY(qb_lm_flash_attn(q32, kv->k[i], kv->v[i], B, L, heads, pos0, kv->Lmax, (qb_half*)t1.hi, (qb_half*)t1.lo, st));
-    QB_TRY(lin(t1, M, H, w.wo, H).residual(x, H, M, 0).out32(x, H, M, 0).run(st));
-    QB_TRY(qb_rmsnorm(x, w.post_w, 1e-6f, M, H, nullptr, (qb_half*)t1.hi, (qb_half*)t1.lo, st));
-    QB_TRY(lin(t1, M, H, w.wgu, 2 * I).act(QB_ACT_SWIGLU).outp(hid, I, M, 0).run(st));
-    QB_TRY(lin(hid, M, I, w.wd, H).residual(x, H, M, 0).out32(x, H, M, 0).run(st));
-  }
-  kv->length = pos0 + (int)L;
-  set_i32_kernel<<<1, 32, 0, (cudaStream_t)st>>>(kv->pos, kv->length, 0, 1);
-  g_launches++;
-  QB_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-}  // namespace qb
-
-extern "C" int qb_lm_prefill(qb_lm* m, const float* embeds, int64_t B, int64_t P, qb_kv* kv, float* last_hidden, void* stream) {
-  QB_REQUIRE(m && embeds && kv && B >= 1 && P >= 1 && kv->m == m, "lm_prefill: bad args");
-  const int H = m->cfg.hidden;
-  float* x;
-  QB_TRY(m->ws.f32(&x, "x", (size_t)B * P * H));
-  QB_CHECK_CUDA(cudaMemcpyAsync(x, embeds, (size_t)B * P * H * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  QB_TRY(lm_layers_prefill(m, x, B, P, kv, stream));
-  if (last_hidden) QB_TRY(qb_rmsnorm(x, m->norm, 1e-6f, B * P, H, last_hidden, nullptr, nullptr, stream));
-  return 0;
-}
-
-extern "C" int qb_lm_decode_greedy(qb_lm* m, qb_kv* kv, int64_t B, int32_t first_token, int32_t n_steps, int32_t col_lo,
-                                   int32_t col_hi, int64_t* out_ids, void* stream) {
-  QB_REQUIRE(m && kv && out_ids && kv->m == m && B >= 1 && B <= 32 && kv->B == B, "lm_decode_greedy: bad args (1 <= B <= 32, cache of the same batch)");
-  QB_REQUIRE(first_token >= 0 && first_token < m->cfg.vocab && col_lo >= 0 && col_hi <= m->cfg.vocab && col_hi > col_lo &&
-                 (col_hi - col_lo) % 16 == 0, "lm_decode_greedy: bad token / column range (width must be a multiple of 16)");
-  QB_REQUIRE(kv->length > 0 && kv->length + n_steps <= kv->Lmax, "lm_decode_greedy: needs a prefilled cache with room for %d more positions", n_steps);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int H = m->cfg.hidden, heads = m->cfg.heads, I = m->cfg.inter;
-  fill_rows_kernel<<<grid_for((long long)B * H), 256, 0, st>>>(m->emb + (size_t)first_token * H, B, H, kv->xs);
-  set_i32_kernel<<<1, 32, 0, st>>>(kv->rng, col_lo, col_hi, 2);
-  set_i32_kernel<<<1, 32, 0, st>>>(kv->slot, 0, 0, 2);
-  g_launches += 3;
-  const int max_cols = col_hi - col_lo;
-  for (int s = 0; s < n_steps; ++s) {
-    for (int i = 0; i < m->cfg.layers; ++i) {
-      const LmLayerW& w = m->layers[i];
-      QB_TRY(qb_lm_decode_layer_tc(kv->xs, B, H, heads, I, w.wqkv_p, w.wo_p, w.wg_p, w.wu_p, w.wd_p, kv->k[i], kv->v[i], kv->Lmax, kv->pos,
-                                   m->rcos, m->rsin, kv->qb_, kv->ab, kv->mb, stream));
-    }
-    QB_TRY(qb_lm_head_argmax_tc(kv->xs, B, H, m->head_p, kv->rng, max_cols, m->emb, kv->xs, out_ids, n_steps, kv->pos, kv->slot, kv->pv,
-                                kv->pi, stream));
-  }
-  kv->length += n_steps;
-  return 0;
-}
-
-extern "C" int qb_lm_forward_logits(qb_lm* m, const float* embeds, int64_t B, int64_t L, float* logits, void* stream) {
-  QB_REQUIRE(m && embeds && logits && B >= 1 && L >= 1, "lm_forward_logits: bad args");
-  QB_REQUIRE(L <= m->cfg.max_positions, "lm_forward_logits: L exceeds the RoPE table");
-  const int H = m->cfg.hidden, heads = m->cfg.heads, V = m->cfg.vocab;
-  const int Lmax = (int)pad_to(L, 64);
-  // scratch context (no cache kept): K/V of every layer from the workspace
-  qb_kv kv;
-  kv.m = m; kv.B = B; kv.Lmax = Lmax; kv.length = 0;
-  kv.k.resize(m->cfg.layers); kv.v.resize(m->cfg.layers);
-  for (int i = 0; i < m->cfg.layers; ++i) {
-    QB_TRY(m->ws.f32(&kv.k[i], "fk" + std::to_string(i), (size_t)B * heads * Lmax * 64));
-    QB_TRY(m->ws.f32(&kv.v[i], "fv" + std::to_string(i), (size_t)B * heads * Lmax * 64));
-  }
-  QB_TRY(m->ws.get((void**)&kv.pos, "fpos", 16));
-  float *x, *hs;
-  PlanesD hp;
-  QB_TRY(m->ws.f32(&x, "x", (size_t)B * L * H));
-  QB_CHECK_CUDA(cudaMemcpyAsync(x, embeds, (size_t)B * L * H * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  QB_TRY(lm_layers_prefill(m, x, B, L, &kv, stream));
-  QB_TRY(m->ws.f32(&hs, "hs", (size_t)B * L * H));
-  QB_TRY(m->ws.planes(&hp, "hp", (size_t)B * L * H, true));
-  QB_TRY(qb_rmsnorm(x, m->norm, 1e-6f, B * L, H, nullptr, (qb_half*)hp.hi, (qb_half*)hp.lo, stream));
-  (void)hs;
-  return lin(hp, B * L, H, m->head, V).out32(logits, V, B * L, 0).run(stream);
 }

@@ -253,17 +253,14 @@ lm_flash_attn_kernel(const float* __restrict__ q32, const float* __restrict__ kc
 }
 
 // ------------------------------------------------------------------------------------------ decode step
-// Positions of the decode step: row b reads pos[b * pos_stride].  Stride 0 is one position shared by every row; stride 1
-// gives each row its own (rows whose prefixes differ in length).  The last block of a step bumps every position once.
-__device__ __forceinline__ void bump_positions(int* pos, int pos_stride, int B) {
-  const int n = pos_stride ? B : 1;
-  for (int i = 0; i < n; ++i) pos[i * pos_stride] += 1;
-}
+// Positions of the decode step: row b reads pos[b] (rows whose prefixes differ in length sit at different positions).  The head's
+// block of row b bumps pos[b] after its dependency wait: every kernel of the step that reads positions has finished by then, and
+// the next step reads them after its own wait.
 
 // greedy token from the head partials, next input embedding, position / slot bump
 __global__ void lm_argmax_embed_kernel(const float* __restrict__ part_val, const int* __restrict__ part_idx, int n_part,
                                        int B, const float* __restrict__ emb, int Hd, float* __restrict__ x_next,
-                                       int64_t* __restrict__ out_ids, int out_stride, int* __restrict__ pos, int pos_stride,
+                                       int64_t* __restrict__ out_ids, int out_stride, int* __restrict__ pos,
                                        int* __restrict__ slot, const int* __restrict__ range, int vocab) {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");          // no-ops unless launched as a programmatic dependent
@@ -294,6 +291,7 @@ __global__ void lm_argmax_embed_kernel(const float* __restrict__ part_val, const
     if ((unsigned)bi >= (unsigned)vocab) bi = range_lo;
     si[0] = bi;
     out_ids[(size_t)b * out_stride + *slot] = (int64_t)bi;
+    pos[b] += 1;
   }
   __syncthreads();
   const int tok = si[0];
@@ -303,7 +301,7 @@ __global__ void lm_argmax_embed_kernel(const float* __restrict__ part_val, const
   if (threadIdx.x == 0) {
     __threadfence();
     const int done = atomicAdd(slot + 1, 1);          // slot[1] = arrival counter
-    if (done == B - 1) { slot[1] = 0; *slot += 1; bump_positions(pos, pos_stride, B); }
+    if (done == B - 1) { slot[1] = 0; *slot += 1; }
   }
 }
 
@@ -408,7 +406,7 @@ __global__ void __launch_bounds__(256)
 lm_sample_embed_kernel(const float* __restrict__ logits, int ld, const int* __restrict__ range, int B, float inv_temp,
                        int top_k, float top_p, const unsigned* __restrict__ seed /* {seed_lo, seed_hi, call, 0} */,
                        const float* __restrict__ emb, int Hd, float* __restrict__ x_next, int64_t* __restrict__ out_ids,
-                       int out_stride, int* __restrict__ pos, int pos_stride, int* __restrict__ slot, float* __restrict__ dbg) {
+                       int out_stride, int* __restrict__ pos, int* __restrict__ slot, float* __restrict__ dbg) {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
   extern __shared__ uint32_t ls_smem[];
@@ -547,13 +545,13 @@ lm_sample_embed_kernel(const float* __restrict__ logits, int ld, const int* __re
     __syncthreads();
   }
   const int tok = sh_tok;
-  if (tid == 0) out_ids[(size_t)b * out_stride + *slot] = (int64_t)tok;
+  if (tid == 0) { out_ids[(size_t)b * out_stride + *slot] = (int64_t)tok; pos[b] += 1; }
   for (int k = tid; k < Hd; k += 256) x_next[(size_t)b * Hd + k] = emb[(size_t)tok * Hd + k];
   __syncthreads();
   if (tid == 0) {
     __threadfence();
     const int done = atomicAdd(slot + 1, 1);
-    if (done == B - 1) { slot[1] = 0; *slot += 1; bump_positions(pos, pos_stride, B); }
+    if (done == B - 1) { slot[1] = 0; *slot += 1; }
   }
 }
 
@@ -580,8 +578,7 @@ struct SkParams {
   float* out;            // RESID: x [B,N] updated in place; GATEUP: [B,N]; QKV: q [B,H*64]
   int N;
   int H, Lmax;
-  const int* pos;        // QKV: row b's position is pos[b * pos_stride] (see bump_positions)
-  int pos_stride;
+  const int* pos;        // QKV: row b's position is pos[b]
   const float* rcos;
   const float* rsin;
   float* kc;
@@ -767,7 +764,7 @@ lm_skinny_kernel(const SkParams p) {
   } else if (MODE == SK_GATEUP) {
     p.out[(size_t)b * p.N + row0 + c] = silu_f(v0) * v1;
   } else {  // SK_QKV
-    const int pos = p.pos[b * p.pos_stride], dd = dd0 + c;
+    const int pos = p.pos[b], dd = dd0 + c;
     if (sec < 2) {
       const float c1 = p.rcos[pos * 64 + dd], s1 = p.rsin[pos * 64 + dd];
       const float c2 = p.rcos[pos * 64 + dd + 32], s2 = p.rsin[pos * 64 + dd + 32];
@@ -794,13 +791,13 @@ lm_skinny_kernel(const SkParams p) {
 template <int LM_ATT_U>
 __global__ void __launch_bounds__(256)
 lm_decode_attn2_kernel(const float* __restrict__ q, const float* __restrict__ kc, const float* __restrict__ vc, int H,
-                       int Lmax, const int* __restrict__ posp, int pos_stride, float* __restrict__ out) {
+                       int Lmax, const int* __restrict__ posp, float* __restrict__ out) {
   __shared__ __align__(16) float sacc[16][64];
   __shared__ float sm[16], sl[16];
   pdl_wait();
   const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int c = lane & 15, hw = warp * 2 + (lane >> 4);
-  const int n = posp[b * pos_stride] + 1;        // keys 0..pos of this row (its K / V at pos were appended by lm_skinny<QKV>)
+  const int n = posp[b] + 1;                     // keys 0..pos of this row (its K / V at pos were appended by lm_skinny<QKV>)
   const float4 qv = *reinterpret_cast<const float4*>(q + (size_t)b * H * 64 + h * 64 + 4 * c);
   const float4* kb = reinterpret_cast<const float4*>(kc + ((size_t)b * H + h) * Lmax * 64) + c;
   const float4* vb = reinterpret_cast<const float4*>(vc + ((size_t)b * H + h) * Lmax * 64) + c;
@@ -931,16 +928,15 @@ extern "C" int qb_lm_set_att_unroll(int32_t keys_per_lane) {
   return 0;
 }
 
-// pos_stride: 0 = one position shared by the batch (*pos), 1 = one per row (pos[0..B))
-static int lm_decode_layer(float* x, int64_t B, int32_t hidden, int32_t heads, int32_t inter, const qb_half* wqkv,
-                           const qb_half* wo, const qb_half* wgate, const qb_half* wup, const qb_half* wdown, float* k_cache,
-                           float* v_cache, int32_t Lmax, const int32_t* pos, int pos_stride, const float* rope_cos,
-                           const float* rope_sin, float* q_buf, float* attn_buf, float* mlp_buf, void* stream) {
+extern "C" int qb_lm_decode_layer_tc(float* x, int64_t B, int32_t hidden, int32_t heads, int32_t inter, const qb_half* wqkv,
+                                     const qb_half* wo, const qb_half* wgate, const qb_half* wup, const qb_half* wdown,
+                                     float* k_cache, float* v_cache, int32_t Lmax, const int32_t* pos, const float* rope_cos,
+                                     const float* rope_sin, float* q_buf, float* attn_buf, float* mlp_buf, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   QB_REQUIRE(B >= 1 && B <= 32, "lm_decode_layer_tc: batch must be 1..32 (got %lld)", (long long)B);
   QB_REQUIRE(hidden == heads * 64 && hidden % 16 == 0 && inter % 16 == 0, "lm_decode_layer_tc: unsupported dims");
   SkParams p = {};
-  p.B = (int)B; p.eps = 1e-6f; p.H = heads; p.Lmax = Lmax; p.pos = pos; p.pos_stride = pos_stride;
+  p.B = (int)B; p.eps = 1e-6f; p.H = heads; p.Lmax = Lmax; p.pos = pos;
   p.rcos = rope_cos; p.rsin = rope_sin;
   p.kc = k_cache; p.vc = v_cache;
   // RMSNorm + QKV + RoPE + cache append
@@ -950,8 +946,7 @@ static int lm_decode_layer(float* x, int64_t B, int32_t hidden, int32_t heads, i
   // (latency-bound), 4 when several chains share the GPU (throughput-bound)
   auto att = g_lm_att_unroll == 4 ? lm_decode_attn2_kernel<4> : lm_decode_attn2_kernel<8>;
   QB_CHECK_CUDA(launch_pdl(att, dim3((unsigned)heads, (unsigned)B), dim3(256), 0, st, (const float*)q_buf,
-                           (const float*)k_cache, (const float*)v_cache, (int)heads, (int)Lmax, (const int*)pos, pos_stride,
-                           attn_buf));
+                           (const float*)k_cache, (const float*)v_cache, (int)heads, (int)Lmax, (const int*)pos, attn_buf));
   // o_proj + residual
   p.x = attn_buf; p.K = hidden; p.W = (const uint4*)wo; p.out = x; p.N = hidden;
   if (int e = launch_skinny<SK_RESID>(p, hidden / 8, st)) return e;
@@ -964,25 +959,10 @@ static int lm_decode_layer(float* x, int64_t B, int32_t hidden, int32_t heads, i
   return 0;
 }
 
-extern "C" int qb_lm_decode_layer_tc(float* x, int64_t B, int32_t hidden, int32_t heads, int32_t inter, const qb_half* wqkv,
-                                     const qb_half* wo, const qb_half* wgate, const qb_half* wup, const qb_half* wdown,
-                                     float* k_cache, float* v_cache, int32_t Lmax, const int32_t* pos, const float* rope_cos,
-                                     const float* rope_sin, float* q_buf, float* attn_buf, float* mlp_buf, void* stream) {
-  return lm_decode_layer(x, B, hidden, heads, inter, wqkv, wo, wgate, wup, wdown, k_cache, v_cache, Lmax, pos, 0, rope_cos, rope_sin,
-                         q_buf, attn_buf, mlp_buf, stream);
-}
-
-extern "C" int qb_lm_decode_layer_tc_rows(float* x, int64_t B, int32_t hidden, int32_t heads, int32_t inter, const qb_half* wqkv,
-                                          const qb_half* wo, const qb_half* wgate, const qb_half* wup, const qb_half* wdown,
-                                          float* k_cache, float* v_cache, int32_t Lmax, const int32_t* pos, const float* rope_cos,
-                                          const float* rope_sin, float* q_buf, float* attn_buf, float* mlp_buf, void* stream) {
-  return lm_decode_layer(x, B, hidden, heads, inter, wqkv, wo, wgate, wup, wdown, k_cache, v_cache, Lmax, pos, 1, rope_cos, rope_sin,
-                         q_buf, attn_buf, mlp_buf, stream);
-}
-
-static int lm_head_argmax(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range, int32_t max_cols,
-                          const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride, int32_t* pos, int pos_stride,
-                          int32_t* slot, float* part_val, int32_t* part_idx, void* stream) {
+extern "C" int qb_lm_head_argmax_tc(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
+                                    int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids,
+                                    int32_t out_stride, int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx,
+                                    void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   QB_REQUIRE(B >= 1 && B <= 32 && max_cols % 16 == 0, "lm_head_argmax_tc: bad args (max_cols must be a multiple of 16)");
   SkParams p = {};
@@ -991,32 +971,17 @@ static int lm_head_argmax(const float* x, int64_t B, int32_t hidden, const qb_ha
   if (int e = launch_skinny<SK_HEAD>(p, max_cols / 16, st)) return e;
   QB_CHECK_CUDA(launch_pdl(lm_argmax_embed_kernel, dim3((unsigned)B), dim3(128), 0, st, (const float*)part_val,
                            (const int*)part_idx, (int)(max_cols / 16), (int)B, embedding, (int)hidden, x_next, out_ids,
-                           (int)out_stride, (int*)pos, pos_stride, (int*)slot, (const int*)range, 0x7ffffffe));
+                           (int)out_stride, (int*)pos, (int*)slot, (const int*)range, 0x7ffffffe));
   return 0;
-}
-
-extern "C" int qb_lm_head_argmax_tc(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
-                                    int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids,
-                                    int32_t out_stride, int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx,
-                                    void* stream) {
-  return lm_head_argmax(x, B, hidden, w_head, range, max_cols, embedding, x_next, out_ids, out_stride, pos, 0, slot, part_val,
-                        part_idx, stream);
-}
-
-extern "C" int qb_lm_head_argmax_tc_rows(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
-                                         int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids,
-                                         int32_t out_stride, int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx,
-                                         void* stream) {
-  return lm_head_argmax(x, B, hidden, w_head, range, max_cols, embedding, x_next, out_ids, out_stride, pos, 1, slot, part_val,
-                        part_idx, stream);
 }
 
 // Sampled decoding step: as qb_lm_head_argmax_tc, but the head writes the full range logits [B][max_cols] and the token is
 // drawn by lm_sample_embed_kernel (top-k -> top-p -> temperature -> multinomial, llm.py:253-289).
-static int lm_head_sample(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range, int32_t max_cols,
-                          const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride, int32_t* pos, int pos_stride,
-                          int32_t* slot, float* part_val, int32_t* part_idx, float* logits, float temperature, int32_t top_k,
-                          float top_p, const uint32_t* seed, float* debug, void* stream) {
+extern "C" int qb_lm_head_sample_tc(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
+                                    int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids,
+                                    int32_t out_stride, int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx,
+                                    float* logits, float temperature, int32_t top_k, float top_p, const uint32_t* seed,
+                                    float* debug, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   QB_REQUIRE(B >= 1 && B <= 32 && max_cols % 16 == 0, "lm_head_sample_tc: bad args (max_cols must be a multiple of 16)");
   QB_REQUIRE(logits && seed, "lm_head_sample_tc: logits / seed buffers required");
@@ -1031,26 +996,8 @@ static int lm_head_sample(const float* x, int64_t B, int32_t hidden, const qb_ha
   QB_REQUIRE(smem <= 160 * 1024, "lm_head_sample_tc: range too wide (%d columns)", max_cols);
   QB_CHECK_CUDA(launch_pdl(lm_sample_embed_kernel, dim3((unsigned)B), dim3(256), smem, st, (const float*)logits, (int)max_cols,
                            (const int*)range, (int)B, 1.0f / temperature, (int)top_k, top_p, (const unsigned*)seed, embedding,
-                           (int)hidden, x_next, out_ids, (int)out_stride, (int*)pos, pos_stride, (int*)slot, debug));
+                           (int)hidden, x_next, out_ids, (int)out_stride, (int*)pos, (int*)slot, debug));
   return 0;
-}
-
-extern "C" int qb_lm_head_sample_tc(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
-                                    int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids,
-                                    int32_t out_stride, int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx,
-                                    float* logits, float temperature, int32_t top_k, float top_p, const uint32_t* seed,
-                                    float* debug, void* stream) {
-  return lm_head_sample(x, B, hidden, w_head, range, max_cols, embedding, x_next, out_ids, out_stride, pos, 0, slot, part_val,
-                        part_idx, logits, temperature, top_k, top_p, seed, debug, stream);
-}
-
-extern "C" int qb_lm_head_sample_tc_rows(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
-                                         int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids,
-                                         int32_t out_stride, int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx,
-                                         float* logits, float temperature, int32_t top_k, float top_p, const uint32_t* seed,
-                                         float* debug, void* stream) {
-  return lm_head_sample(x, B, hidden, w_head, range, max_cols, embedding, x_next, out_ids, out_stride, pos, 1, slot, part_val,
-                        part_idx, logits, temperature, top_k, top_p, seed, debug, stream);
 }
 
 extern "C" int qb_lm_loss(const float* logits, int64_t ld, int64_t M, int32_t V, const int64_t* targets, float label_smoothing,

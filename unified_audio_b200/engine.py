@@ -1,6 +1,6 @@
 """ctypes front end of the handle-level C ABI (include/quark_b200.h "Handle-level contract"; csrc/engine.cu):
-per-device context, H-Codec-2.0 codec handle, residual-VQ handle, UniSE LM handle + KV cache.  The Python faces
-(codec.py, llm.py) are thin callers of these for the product path."""
+per-device context, H-Codec-2.0 codec handle, residual-VQ handle.  `Codec` (codec.py) is a thin caller of these for the
+product path; the UniSE LM (llm.py) composes the op-level entry points instead."""
 from __future__ import annotations
 
 import ctypes as C
@@ -9,7 +9,7 @@ from typing import Dict, Optional
 import torch
 
 from . import _lib
-from ._lib import CodecCfg, LmCfg, PRECISION_CODES, TAP_FN, Tensor
+from ._lib import CodecCfg, PRECISION_CODES, TAP_FN, Tensor
 
 _CONTEXTS: Dict[int, "Context"] = {}
 
@@ -173,67 +173,3 @@ class RvqEngine:
         out = torch.empty(idx.shape[0], self.D, device=idx.device)
         _lib.check(self.lib.qb_rvq_decode_rows(self.h, idx.data_ptr(), idx.shape[0], out.data_ptr(), _stream()))
         return out
-
-
-class LmEngine:
-    """qb_lm + qb_kv: UniSE AR-LM prefill / greedy decode / teacher-forced logits."""
-
-    def __init__(self, device, hidden, layers, heads, inter, vocab, max_positions, state_dict):
-        self.lib = _lib.load()
-        cfg = LmCfg()
-        cfg.hidden, cfg.layers, cfg.heads, cfg.inter, cfg.vocab, cfg.max_positions = hidden, layers, heads, inter, vocab, max_positions
-        self.cfg = cfg
-        arr, keep = _tensor_array(state_dict)
-        h = C.c_void_p()
-        _lib.check(self.lib.qb_lm_load(Context.get(device).h, C.byref(cfg), arr, len(state_dict), C.byref(h)))
-        del keep
-        self.h = h
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                self.lib.qb_lm_free(self.h)
-                self.h = None
-        except Exception:
-            pass
-
-    def kv_alloc(self, B: int, Lmax: int):
-        return KvCache(self, B, Lmax)
-
-    def prefill(self, embeds: torch.Tensor, kv: "KvCache", want_hidden=True):
-        B, P, H = embeds.shape
-        embeds = embeds.float().contiguous()
-        out = torch.empty(B, P, H, device=embeds.device) if want_hidden else None
-        _lib.check(self.lib.qb_lm_prefill(self.h, embeds.data_ptr(), B, P, kv.h, out.data_ptr() if out is not None else None, _stream()))
-        return out
-
-    def decode_greedy(self, kv: "KvCache", B, first_token, n_steps, col_lo, col_hi):
-        out = torch.empty(B, n_steps, dtype=torch.int64, device="cuda")
-        _lib.check(self.lib.qb_lm_decode_greedy(self.h, kv.h, B, first_token, n_steps, col_lo, col_hi, out.data_ptr(), _stream()))
-        return out
-
-    def forward_logits(self, embeds: torch.Tensor):
-        B, L, H = embeds.shape
-        embeds = embeds.float().contiguous()
-        logits = torch.empty(B, L, self.cfg.vocab, device=embeds.device)
-        _lib.check(self.lib.qb_lm_forward_logits(self.h, embeds.data_ptr(), B, L, logits.data_ptr(), _stream()))
-        return logits
-
-
-class KvCache:
-    def __init__(self, lm: LmEngine, B: int, Lmax: int):
-        self.lm, self.lib = lm, lm.lib
-        h = C.c_void_p()
-        _lib.check(self.lib.qb_kv_alloc(lm.h, B, Lmax, C.byref(h)))
-        self.h = h
-
-    def reset(self):
-        _lib.check(self.lib.qb_kv_reset(self.h, _stream()))
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                self.lib.qb_kv_free(self.h)
-                self.h = None
-        except Exception:
-            pass

@@ -57,7 +57,7 @@ class StaticKVCache:
         self.k = [torch.zeros(B, heads, Lmax, 64, dtype=torch.float32, device=device) for _ in range(layers)]
         self.v = [torch.zeros(B, heads, Lmax, 64, dtype=torch.float32, device=device) for _ in range(layers)]
         self.B, self.heads, self.layers, self.Lmax, self.length = B, heads, layers, Lmax, 0
-        self.pos = torch.zeros(1, dtype=torch.int32, device=device)     # device copy used by the decode kernels
+        self.pos = torch.zeros(B, dtype=torch.int32, device=device)     # row b's position, read (and bumped) by the decode kernels
 
     def get_seq_length(self):
         return self.length
@@ -208,15 +208,13 @@ class LLM_SFT(_Face):
             cache.length = pos0 + L
             cache.pos.fill_(cache.length)
 
-    def _decode_layers(self, x: torch.Tensor, B: int, cache: StaticKVCache, row_pos: Optional[torch.Tensor] = None):
-        """row_pos: int32 [B] device positions, one per row (prefixes of different lengths); None = the cache's shared position"""
+    def _decode_layers(self, x: torch.Tensor, B: int, cache: StaticKVCache):
         W = self._prepare()
         ops.lm_set_att_unroll(self.att_unroll)
         H, heads, inter = self.hidden, self.heads, 4 * self.hidden
         qb, ab, mb = self._buf("dq", (B, H)), self._buf("da", (B, H)), self._buf("dm", (B, inter))
-        layer, pos = (ops.lm_decode_layer_tc, cache.pos) if row_pos is None else (ops.lm_decode_layer_tc_rows, row_pos)
         for i, Lw in enumerate(W["layers"]):
-            layer(x, B, H, heads, inter, Lw, cache.k[i], cache.v[i], cache.Lmax, pos, W["cos"], W["sin"], qb, ab, mb)
+            ops.lm_decode_layer_tc(x, B, H, heads, inter, Lw, cache.k[i], cache.v[i], cache.Lmax, cache.pos, W["cos"], W["sin"], qb, ab, mb)
 
     @torch.no_grad()
     def llm_forward(self, inputs_embeds, attention_mask=None, past_key_values: Optional[StaticKVCache] = None,
@@ -426,7 +424,6 @@ class LLM_SFT(_Face):
         dev = mix_feats.device
         prefix = self._prefix(task_name, enroll_feats, mix_feats, enroll_lengths)
         B, P, H = prefix.shape
-        ragged = enroll_lengths is not None
         n_steps = global_length + 1 + semantic_length
         Lmax = -(-(P + n_steps) // 64) * 64
         self._ensure_rope(P + n_steps)
@@ -435,7 +432,7 @@ class LLM_SFT(_Face):
         samp_key = None if sampling is None else (sampling["temperature"], sampling["top_k"], sampling["top_p"])
         # Decode state (KV cache, counters, output ids) and the captured graphs are kept per shape: capturing and
         # instantiating ~560 kernel nodes costs the host 10-50 ms, as much as the whole generation takes on the device.
-        key = (B, P, n_steps, bool(use_graph), int(self.graph_steps), str(dev), samp_key, ragged)
+        key = (B, P, n_steps, bool(use_graph), int(self.graph_steps), str(dev), samp_key)
         st = self._gen_state.get(key)
         if st is None:
             self._gen_state.clear()                    # one shape at a time (the cache is ~0.9 GB at B=32)
@@ -446,8 +443,7 @@ class LLM_SFT(_Face):
                       pv=torch.zeros(max_cols // 16 + 1, 32, device=dev),
                       pi=torch.zeros(max_cols // 16 + 1, 32, dtype=torch.int32, device=dev), g1=None, gk=None, captured=False,
                       logits=torch.zeros(B, max_cols, device=dev) if sampling is not None else None,
-                      seed=torch.zeros(4, dtype=torch.int32, device=dev), dbg=torch.zeros(B, 4, device=dev),
-                      row_pos=torch.zeros(B, dtype=torch.int32, device=dev) if ragged else None)
+                      seed=torch.zeros(4, dtype=torch.int32, device=dev), dbg=torch.zeros(B, 4, device=dev))
             self._gen_state[key] = st
         cache, xs, rng, slot, out_ids, pv, pi = (st[k] for k in ("cache", "xs", "rng", "slot", "out_ids", "pv", "pi"))
         cache.length = 0
@@ -461,27 +457,21 @@ class LLM_SFT(_Face):
         rng.copy_(torch.tensor([self.global_offset, self.global_offset + self.global_size], dtype=torch.int32), non_blocking=True)
         x = prefix.reshape(B * P, H).contiguous().clone()
         self._prefill(x, B, P, cache)
-        row_pos = st["row_pos"]
-        start = None if row_pos is None else torch.tensor([3 + n + mix_feats.shape[1] for n in enroll_lengths], dtype=torch.int32)
+        # the first decode step of row b writes position P_b (P for every row without ragged prefixes)
+        starts = torch.tensor([P] * B if enroll_lengths is None else [3 + n + mix_feats.shape[1] for n in enroll_lengths],
+                              dtype=torch.int32)
 
-        def reset_pos():            # the first decode step of row b writes position P_b (P for every row without ragged prefixes)
-            if row_pos is None:
-                cache.pos.fill_(cache.length)
-            else:
-                row_pos.copy_(start, non_blocking=True)
-        if row_pos is not None:     # (_prefill has set the shared position)
-            reset_pos()
-        pos = cache.pos if row_pos is None else row_pos
-        sample = ops.lm_head_sample_tc if row_pos is None else ops.lm_head_sample_tc_rows
-        argmax = ops.lm_head_argmax_tc if row_pos is None else ops.lm_head_argmax_tc_rows
+        def reset_pos():
+            cache.pos.copy_(starts, non_blocking=True)
+        reset_pos()
 
         def step():
-            self._decode_layers(xs, B, cache, row_pos)
+            self._decode_layers(xs, B, cache)
             if sampling is not None:
-                sample(xs, B, H, W["head_p"], rng, max_cols, W["emb"], xs, out_ids, n_steps, pos, slot, pv, pi, st["logits"],
-                       sampling["temperature"], sampling["top_k"], sampling["top_p"], st["seed"], st["dbg"])
+                ops.lm_head_sample_tc(xs, B, H, W["head_p"], rng, max_cols, W["emb"], xs, out_ids, n_steps, cache.pos, slot, pv, pi,
+                                      st["logits"], sampling["temperature"], sampling["top_k"], sampling["top_p"], st["seed"], st["dbg"])
             else:
-                argmax(xs, B, H, W["head_p"], rng, max_cols, W["emb"], xs, out_ids, n_steps, pos, slot, pv, pi)
+                ops.lm_head_argmax_tc(xs, B, H, W["head_p"], rng, max_cols, W["emb"], xs, out_ids, n_steps, cache.pos, slot, pv, pi)
 
         # All decode state is on the device, so a graph may hold any number of consecutive steps: one single-step graph
         # plus one of `graph_steps` steps (fewer replays per generation).

@@ -327,51 +327,31 @@ def lm_set_att_unroll(keys_per_lane: int):
     _lib.check(_lib.load().qb_lm_set_att_unroll(int(keys_per_lane)))
 
 
+def _check_pos(pos, B):
+    """the decode step reads (and the head bumps) one position per row: pos[b]"""
+    if pos.dtype != torch.int32 or pos.numel() < B or not pos.is_contiguous():
+        raise ValueError(f"per-row positions must be a contiguous int32 tensor of >= {B} elements, got {pos.dtype} {tuple(pos.shape)}")
+
+
 def lm_decode_layer_tc(x, B, hidden, heads, inter, L, kc, vc, Lmax, pos, cos, sin, q_buf, attn_buf, mlp_buf):
+    _check_pos(pos, B)
     _lib.check(_lib.load().qb_lm_decode_layer_tc(_p(x), B, hidden, heads, inter, _p(L["wqkv_p"]), _p(L["wo_p"]), _p(L["wg_p"]),
                                                  _p(L["wu_p"]), _p(L["wd_p"]), _p(kc), _p(vc), Lmax, _p(pos), _p(cos), _p(sin),
                                                  _p(q_buf), _p(attn_buf), _p(mlp_buf), _stream()))
 
 
-def lm_decode_layer_tc_rows(x, B, hidden, heads, inter, L, kc, vc, Lmax, pos, cos, sin, q_buf, attn_buf, mlp_buf):
-    """lm_decode_layer_tc with pos = int32 [B]: one position per row"""
-    _check_row_pos(pos, B)
-    _lib.check(_lib.load().qb_lm_decode_layer_tc_rows(_p(x), B, hidden, heads, inter, _p(L["wqkv_p"]), _p(L["wo_p"]), _p(L["wg_p"]),
-                                                      _p(L["wu_p"]), _p(L["wd_p"]), _p(kc), _p(vc), Lmax, _p(pos), _p(cos), _p(sin),
-                                                      _p(q_buf), _p(attn_buf), _p(mlp_buf), _stream()))
-
-
 def lm_head_argmax_tc(x, B, hidden, w_head_p, rng, max_cols, emb, x_next, out_ids, out_stride, pos, slot, pv, pi):
+    _check_pos(pos, B)
     _lib.check(_lib.load().qb_lm_head_argmax_tc(_p(x), B, hidden, _p(w_head_p), _p(rng), max_cols, _p(emb), _p(x_next),
                                                 _p(out_ids), out_stride, _p(pos), _p(slot), _p(pv), _p(pi), _stream()))
 
 
-def lm_head_argmax_tc_rows(x, B, hidden, w_head_p, rng, max_cols, emb, x_next, out_ids, out_stride, pos, slot, pv, pi):
-    """lm_head_argmax_tc with pos = int32 [B]: every row's position is bumped"""
-    _check_row_pos(pos, B)
-    _lib.check(_lib.load().qb_lm_head_argmax_tc_rows(_p(x), B, hidden, _p(w_head_p), _p(rng), max_cols, _p(emb), _p(x_next),
-                                                     _p(out_ids), out_stride, _p(pos), _p(slot), _p(pv), _p(pi), _stream()))
-
-
 def lm_head_sample_tc(x, B, hidden, w_head_p, rng, max_cols, emb, x_next, out_ids, out_stride, pos, slot, pv, pi, logits,
                       temperature, top_k, top_p, seed, debug=None):
+    _check_pos(pos, B)
     _lib.check(_lib.load().qb_lm_head_sample_tc(_p(x), B, hidden, _p(w_head_p), _p(rng), max_cols, _p(emb), _p(x_next),
                                                 _p(out_ids), out_stride, _p(pos), _p(slot), _p(pv), _p(pi), _p(logits),
                                                 float(temperature), int(top_k), float(top_p), _p(seed), _p(debug), _stream()))
-
-
-def lm_head_sample_tc_rows(x, B, hidden, w_head_p, rng, max_cols, emb, x_next, out_ids, out_stride, pos, slot, pv, pi, logits,
-                           temperature, top_k, top_p, seed, debug=None):
-    """lm_head_sample_tc with pos = int32 [B]: every row's position is bumped"""
-    _check_row_pos(pos, B)
-    _lib.check(_lib.load().qb_lm_head_sample_tc_rows(_p(x), B, hidden, _p(w_head_p), _p(rng), max_cols, _p(emb), _p(x_next),
-                                                     _p(out_ids), out_stride, _p(pos), _p(slot), _p(pv), _p(pi), _p(logits),
-                                                     float(temperature), int(top_k), float(top_p), _p(seed), _p(debug), _stream()))
-
-
-def _check_row_pos(pos, B):
-    if pos.dtype != torch.int32 or pos.numel() < B or not pos.is_contiguous():
-        raise ValueError(f"per-row positions must be a contiguous int32 tensor of >= {B} elements, got {pos.dtype} {tuple(pos.shape)}")
 
 
 def ssl_conv0_gn_gelu(x, w, gn_w, gn_b, eps, k, stride, out: Planes, ld, rows_per_batch, row_off, y_scratch, workspace):
