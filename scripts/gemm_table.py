@@ -58,9 +58,10 @@ def planes(shape, split, g, scale=1.0):
 
 
 def case(name, *, m, n, k, split, taps=1, stride=1, batch=1, m_per_batch=None, a_rpb=None, bias=False, gamma=False,
-         residual=False, act=0, act2=0, out="f32", out_ld=None):
+         residual=False, inplace=False, act=0, act2=0, out="f32", out_ld=None, planes_pad=0):
     """One ops.gemm call built the way engine.cu builds it.  Returns (callable, issued FLOP, (M, N, K) for torch.matmul,
-    the kernel variant qb_gemm picks)."""
+    the kernel variant qb_gemm picks).  inplace: the residual is the fp32 output itself; planes_pad: the planes are written
+    at row offset planes_pad of (m_per_batch + 2 planes_pad)-row batches, the zero-padded input of the next conv."""
     from unified_audio_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(1)
     mpb = m_per_batch or m // batch
@@ -78,17 +79,19 @@ def case(name, *, m, n, k, split, taps=1, stride=1, batch=1, m_per_batch=None, a
     if act == ops.ACT_SNAKE or act2 == ops.ACT_SNAKE:
         kw["act_param" if act == ops.ACT_SNAKE else "act2_param"] = torch.rand(n, generator=g, device="cuda") + 0.5
     keep = []
-    if residual:
+    if out in ("f32", "f32+planes"):
+        o = torch.randn(batch * mpb, ld, generator=g, device="cuda")
+        keep.append(o)
+        kw["out_f32"] = ops.rowmap(o, ld, mpb, 0)
+    if residual and inplace:
+        kw["residual"] = kw["out_f32"]
+    elif residual:
         r = torch.randn(batch * mpb, ld, generator=g, device="cuda")
         keep.append(r)
         kw["residual"] = ops.rowmap(r, ld, mpb, 0)
-    if out in ("f32", "f32+planes"):
-        o = torch.empty(batch * mpb, ld, device="cuda")
-        keep.append(o)
-        kw["out_f32"] = ops.rowmap(o, ld, mpb, 0)
     if out in ("planes", "f32+planes"):
-        kw["out_planes"] = ops.Planes.zeros((batch * mpb, ld), split, "cuda")
-        kw["out_planes_map"] = (ld, mpb, 0)
+        kw["out_planes"] = ops.Planes.zeros((batch * (mpb + 2 * planes_pad), ld), split, "cuda")
+        kw["out_planes_map"] = (ld, mpb + 2 * planes_pad, planes_pad)
     fn = lambda: ops.gemm(a, w, n, **kw)     # noqa: E731
     fn._keep = keep
     flop = 2.0 * batch * mpb * n * taps * k * (3 if split else 1)
@@ -107,12 +110,29 @@ def shapes():
         ("tf.w13_swiglu", 4, dict(m=M, n=2 * IT, k=C, split=True, act=ops.ACT_SWIGLU, out="planes")),
         ("tf.w2", 4, dict(m=M, n=C, k=IT, split=True, residual=True)),
         ("resnet.conv_k3", 8, dict(m=M, n=C, k=C, split=True, taps=3, batch=64, bias=True, residual=True)),
-        ("sem.conv_k3_elu", 8, dict(m=M, n=C, k=C, split=True, taps=3, batch=64, act=ops.ACT_ELU, out="planes")),
-        ("sem.conv_1x1_res", 8, dict(m=M, n=C, k=C, split=True, batch=64, residual=True, act2=ops.ACT_ELU, out="f32+planes")),
+    ] + sem_shapes() + [
         ("enc.out_conv_strided", 1, dict(m=64 * 125, n=1024, k=C, split=True, taps=9, stride=4, batch=64, bias=True)),
         ("dec.head", 1, dict(m=M, n=1922, k=C, split=True, bias=True, out_ld=1984)),
         ("stft.stage1_n128", 1, dict(m=M * 30, n=128, k=64, split=True)),
     ]
+
+
+def sem_shapes():
+    """encode_sem (engine.cu) at the bench shape: 768 -> 1536 channels, blocks at 500, 250 and 250 frames per clip with
+    strides 2, 1, 2.  Every conv but the last writes fp16 hi + lo planes for the next one."""
+    from unified_audio_b200 import ops
+    B, Cs, ELU = 64, 1536, ops.ACT_ELU
+    sem = dict(split=True, batch=64, n=Cs, k=Cs)
+    planes = dict(out="f32+planes", planes_pad=1)
+    rows = [("sem.s_conv_k3@500", 1, dict(sem, m=B * 500, k=768, taps=3, act2=ELU, **planes))]
+    for t, blocks in ((500, 1), (250, 2)):
+        rows += [(f"sem.conv_k3_elu@{t}", 2 * blocks, dict(sem, m=B * t, taps=3, act=ELU, out="planes")),
+                 (f"sem.conv_1x1_res_elu@{t}", blocks, dict(sem, m=B * t, residual=True, inplace=True, act2=ELU, **planes)),
+                 (f"sem.conv_1x1_res@{t}", blocks, dict(sem, m=B * t, residual=True, inplace=True, **planes))]
+    for i, (t, s, act2) in enumerate(((500, 2, ELU), (250, 1, ELU), (250, 2, 0))):
+        rows.append((f"sem.block{i}_conv_s{s}@{t}", 1, dict(sem, m=B * (t // s), taps=3, stride=s, bias=True, act2=act2, **planes)))
+    rows.append(("sem.conv2@125", 1, dict(sem, m=B * 125, n=512, taps=3)))
+    return rows
 
 
 def matmul_rate(mnk):
@@ -128,7 +148,7 @@ def part_table():
     for name, calls, kw in shapes():
         fn, flop, mnk, kern = case(name, **kw)
         ms = timed(fn)
-        rows.append(dict(name=name, calls_per_step=calls, mnk=list(mnk), split=kw["split"], kernel=kern, ms=ms,
+        rows.append(dict(name=name, calls_per_step=calls, mnk=list(mnk), split=kw["split"], kernel=kern, m_per_batch=mnk[0] // kw.get("batch", 1), ms=ms,
                          tflops_issued=flop / ms / 1e9, ms_per_step=ms * calls, cublas_fp16=matmul_rate(mnk)))
         del fn
         torch.cuda.empty_cache()
@@ -212,6 +232,8 @@ def main():
     doc = {}
     for part in args.parts.split(","):
         doc[part] = dict(card=card, table=part_table, ksweep=part_ksweep, smsweep=part_smsweep, profile=part_profile)[part]()
+        if part == "table":
+            doc["table_ms_per_step"] = sum(r["ms_per_step"] for r in doc[part])
     os.makedirs(args.out, exist_ok=True)
     path = os.path.join(args.out, args.tag + ".json")
     with open(path, "w") as f:

@@ -187,6 +187,9 @@ __device__ __forceinline__ float2 ld_shared_f32x2(uint32_t addr) {
 __device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v));
 }
+__device__ __forceinline__ void st_shared_b16(uint32_t addr, __half v) {
+  asm volatile("st.shared.b16 [%0], %1;" ::"r"(addr), "h"(__half_as_ushort(v)));
+}
 // barrier over `count` threads (a multiple of 32) under barrier id `id` (0 is __syncthreads')
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");

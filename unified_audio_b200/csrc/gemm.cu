@@ -51,9 +51,11 @@ static int current_device() {
 #endif
 
 // What the epilogue of a launch does, decided on the host so that the consumer branches once per tile:
-//   EPI_HI      (bias) (GELU) -> fp16 hi plane (ConvNeXt pwconv1)
-//   EPI_F32     (bias) (* gamma) (+ residual) -> fp32 (pwconv2, o-proj, w2, residual convs)
-//   EPI_GENERIC every other combination, element by element through epilogue_pair
+//   EPI_HI      (bias) (GELU | ELU | SwiGLU) -> fp16 hi plane (+ lo plane)   (ConvNeXt pwconv1, transformer w13, semantic k3 convs)
+//   EPI_F32     (bias) (* gamma) (+ residual) -> fp32, and optionally (ELU) -> hi (+ lo) planes through their own row map
+//               (pwconv2, o-proj, w2, residual convs, the semantic encoder's fp32 + planes convs)
+//   EPI_GENERIC every other combination (Snake, tanh, ReLU, gamma or residual into planes, unaligned buffers), element by element
+//               through epilogue_pair
 // The two fast kinds stage each output subtile in shared memory and write it by TMA store, EPI_F32 reads its residual by TMA
 // load; they need 16-byte aligned bases and row pitches (classify_epilogue).
 enum EpiKind : int { EPI_GENERIC = 0, EPI_HI = 1, EPI_F32 = 2 };
@@ -201,7 +203,7 @@ __device__ __forceinline__ void load_tile_cols(const GemmParams& p, int n0, int 
 // Fast epilogue kinds, on the 64 x BN half tile of one consumer warpgroup (rows row0 + [0, 64), columns n0 + [0, BN)):
 // accumulators -> swizzled subtile in shared memory -> one TMA store per subtile, issued by the warpgroup's first thread.
 // The stores drain while the next tile's main loop runs; the TMA map clips rows >= m_per_batch and columns >= N.
-// Same arithmetic, in the same order, as the vectorised branches of epilogue_pair.
+// Same arithmetic, in the same order, as epilogue_pair / epi_finish_scalar.
 struct EpiCtx {
   uint8_t* buf;        // this warpgroup's EPI_BUFS subtile buffers
   uint64_t* rfull;     // one mbarrier per buffer: residual subtile landed
@@ -209,18 +211,27 @@ struct EpiCtx {
   int cw, b, row0, n0;
 };
 
-template <int BN>
-__device__ __forceinline__ void epilogue_hi(const GemmParams& p, const CUtensorMap* tmO, const EpiCtx& e, const float (&acc)[BN / 2]) {
-  constexpr int NSUB = BN / 64;
+// 64-column fp16 subtiles, 128-byte rows.  Without a lo plane the subtiles alternate between the two buffers; with one, each
+// subtile puts hi in the first buffer and lo in the second.  SwiGLU reduces each interleaved (gate, up) accumulator pair to one
+// output column, 4 j + lane % 4 for the pair at columns 8 j + 2 (lane % 4): a 64 x BN half tile gives BN / 2 output columns.
+// A hi plane alone with no activation or GELU is rounded as epilogue_pair's half2 branch rounds it; every other case through
+// split_f16, as epi_finish_scalar.
+template <int BN, bool SWIGLU>
+__device__ __forceinline__ void epilogue_hi(const GemmParams& p, const CUtensorMap* tmHi, const CUtensorMap* tmLo, const EpiCtx& e,
+                                                const float (&acc)[BN / 2]) {
+  constexpr int NSUB = SWIGLU ? BN / 128 : BN / 64, JS = SWIGLU ? 16 : 8;      // subtiles; 8-column accumulator groups per subtile
   const __half2 hmax = __float2half2_rn(65504.f), hmin = __float2half2_rn(-65504.f);
-  const bool gelu = p.act == QB_ACT_GELU, leader = (threadIdx.x & 127) == 0;
+  const int act = p.act;
+  const bool lo = BN == 128 && p.olo.ptr != nullptr, leader = (threadIdx.x & 127) == 0;
+  const bool rn_sat = BN == 256 || (!lo && (act == QB_ACT_NONE || act == QB_ACT_GELU));
   const int lane = threadIdx.x & 31;
-  // rows r and r + 8 (r % 8 = lane / 4) at 4-byte column offset 4 (lane % 4) of chunk jj, stored at chunk jj ^ (lane / 4)
-  const uint32_t th = smem_u32(e.buf) + (((threadIdx.x >> 5) & 3) * 16 + (lane >> 2)) * 128 + 4 * (lane & 3), sw = (lane >> 2) << 4;
+  // rows r and r + 8 (r % 8 = lane / 4) at byte (SWIGLU ? 2 : 4) (lane % 4) of a 16-byte chunk c, stored at chunk c ^ (lane / 4)
+  const uint32_t th = smem_u32(e.buf) + (((threadIdx.x >> 5) & 3) * 16 + (lane >> 2)) * 128 + (SWIGLU ? 2 : 4) * (lane & 3),
+                 sw = (lane >> 2) << 4;
 #pragma unroll
   for (int s = 0; s < NSUB; ++s) {
-    uint8_t* buf = e.buf + (s % EPI_BUFS) * EPI_SUB_BYTES;
-    if (s == 0) {                              // the previous tile's stores have read the buffers
+    const uint32_t bh = (lo ? 0 : s % EPI_BUFS) * EPI_SUB_BYTES, bl = EPI_SUB_BYTES;
+    if (s == 0 || lo) {                        // the previous stores have read the buffers
       if (leader) bulk_wait_read<0>();
       named_bar_sync(2 + e.cw, 128);
     } else if (s >= EPI_BUFS) {                // the store of subtile s - EPI_BUFS has read this buffer
@@ -228,48 +239,76 @@ __device__ __forceinline__ void epilogue_hi(const GemmParams& p, const CUtensorM
       named_bar_sync(2 + e.cw, 128);
     }
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
-      const int j = 8 * s + jj;
+    for (int jj = 0; jj < JS; ++jj) {
+      const int j = JS * s + jj;
       const float2 bb = p.bias ? ld_shared_f32x2(e.cols + 4 * (8 * j + 2 * (lane & 3))) : make_float2(0.f, 0.f);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
         if (p.bias) { v0 += bb.x; v1 += bb.y; }
-        if (gelu) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
-        const __half2 o = __hmax2_nan(__hmin2_nan(__floats2half2_rn(v0, v1), hmax), hmin);
-        st_shared_b32(th + (s % EPI_BUFS) * EPI_SUB_BYTES + h * 1024 + ((16 * jj) ^ sw), *reinterpret_cast<const uint32_t*>(&o));
+        if (SWIGLU) {                          // output column 4 jj + lane % 4: chunk jj / 2, byte 8 (jj % 2) + 2 (lane % 4)
+          const uint32_t el = th + h * 1024 + ((16 * (jj >> 1)) ^ sw) + 8 * (jj & 1);
+          __half hv, lv;
+          split_f16(silu_f(v0) * v1, hv, lv);
+          st_shared_b16(el + bh, hv);
+          if (lo) st_shared_b16(el + bl, lv);
+        } else {
+          const uint32_t el = th + h * 1024 + ((16 * jj) ^ sw);
+          if (act == QB_ACT_GELU) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
+          else if (BN == 128 && act == QB_ACT_ELU) { v0 = elu_f(v0); v1 = elu_f(v1); }
+          if (rn_sat) {
+            const __half2 o = __hmax2_nan(__hmin2_nan(__floats2half2_rn(v0, v1), hmax), hmin);
+            st_shared_b32(el + bh, *reinterpret_cast<const uint32_t*>(&o));
+          } else {
+            __half2 hv, lv;
+            split_f16(v0, hv.x, lv.x);
+            split_f16(v1, hv.y, lv.y);
+            st_shared_b32(el + bh, *reinterpret_cast<const uint32_t*>(&hv));
+            if (lo) st_shared_b32(el + bl, *reinterpret_cast<const uint32_t*>(&lv));
+          }
+        }
       }
     }
     fence_proxy_async();
     named_bar_sync(2 + e.cw, 128);
     if (leader) {
-      tma_store_3d(tmO, buf, e.n0 + 64 * s, e.row0, e.b);
+      const int x = (SWIGLU ? e.n0 / 2 : e.n0) + 64 * s;
+      tma_store_3d(tmHi, e.buf + bh, x, e.row0, e.b);
+      if (lo) tma_store_3d(tmLo, e.buf + bl, x, e.row0, e.b);
       bulk_commit();
     }
   }
 }
 
-// The residual arrives by TMA into the subtile buffer the result is then written to: subtiles 0 .. EPI_BUFS - 1 were requested
-// during the main loop, subtile s + EPI_BUFS as soon as the store of subtile s has read its buffer.  Every element is read and
-// then written by the same thread, so the residual may be the output buffer itself.
+// 32-column fp32 subtiles.  The residual arrives by TMA into the subtile buffer the result is then written to.  Every element is
+// read and then written by the same thread, so the residual may be the output buffer itself.
+// Without planes the subtiles alternate between the two buffers: subtiles 0 .. EPI_BUFS - 1 of the residual were requested
+// during the main loop, subtile s + EPI_BUFS as soon as the store of subtile s has read its buffer.
+// With planes, (act2) -> split_f16 of the fp32 result: the first buffer holds each subtile's residual and result, the second its
+// hi and lo planes as two 64-row x 64-byte boxes in the 64-byte swizzle (row r at r * 64, chunk c at c ^ (r / 2 % 4)); the
+// residual of subtile s + 1 is requested once the stores of subtile s have read both.
 template <int BN>
-__device__ __forceinline__ void epilogue_f32(const GemmParams& p, const CUtensorMap* tmO, const CUtensorMap* tmR, const EpiCtx& e,
-                                             const float (&acc)[BN / 2]) {
+__device__ __forceinline__ void epilogue_f32(const GemmParams& p, const CUtensorMap* tmO, const CUtensorMap* tmR, const CUtensorMap* tmHi,
+                                             const CUtensorMap* tmLo, const EpiCtx& e, const float (&acc)[BN / 2]) {
   constexpr int NSUB = BN / 32;
+  constexpr uint32_t LO_OFF = EPI_SUB_BYTES / 2;
   static_assert(NSUB % (2 * EPI_BUFS) == 0, "each residual barrier completes an even number of phases per tile");
-  const bool res = p.res.ptr != nullptr, leader = (threadIdx.x & 127) == 0;
-  const int lane = threadIdx.x & 31;
+  const bool res = p.res.ptr != nullptr, planes = BN == 128 && p.ohi.ptr != nullptr, lo = p.olo.ptr != nullptr;
+  const bool elu = p.act2 == QB_ACT_ELU;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const int lane = threadIdx.x & 31, row = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
   // rows r and r + 8 (r % 8 = lane / 4) at byte 8 (lane % 2) of chunk 2 jj + (lane % 4) / 2, stored at that chunk ^ (lane / 4);
   // 2 jj has no bit in common with (lane % 4) / 2, so the stored chunk is 2 jj ^ ((lane % 4) / 2 ^ lane / 4)
-  const uint32_t th = smem_u32(e.buf) + (((threadIdx.x >> 5) & 3) * 16 + (lane >> 2)) * 128 + 8 * (lane & 1),
-                 sw = (((lane >> 1) & 1) ^ (lane >> 2)) << 4;
+  const uint32_t th = smem_u32(e.buf) + row * 128 + 8 * (lane & 1), sw = (((lane >> 1) & 1) ^ (lane >> 2)) << 4;
+  // planes: rows r and r + 8 at byte 4 (lane % 4) of chunk jj, stored at chunk jj ^ (r / 2 % 4) = jj ^ (lane / 8)
+  const uint32_t tp = smem_u32(e.buf + EPI_SUB_BYTES) + row * 64 + 4 * (lane & 3), swp = ((lane >> 3) & 3) << 4;
 #pragma unroll
   for (int s = 0; s < NSUB; ++s) {
-    const int u = s % EPI_BUFS;
+    const int u = planes ? 0 : s % EPI_BUFS;
     uint8_t* buf = e.buf + u * EPI_SUB_BYTES;
     if (res) {
-      mbar_wait(&e.rfull[u], (s / EPI_BUFS) & 1);
-    } else if (s == 0) {                       // the previous tile's stores have read the buffers
+      mbar_wait(&e.rfull[u], (planes ? s : s / EPI_BUFS) & 1);
+    } else if (s == 0 || planes) {             // the previous stores have read the buffers
       if (leader) bulk_wait_read<0>();
       named_bar_sync(2 + e.cw, 128);
     } else if (s >= EPI_BUFS) {                // the store of subtile s - EPI_BUFS has read this buffer
@@ -293,17 +332,31 @@ __device__ __forceinline__ void epilogue_f32(const GemmParams& p, const CUtensor
           v0 += rv.x; v1 += rv.y;
         }
         st_shared_f32x2(el, v0, v1);
+        if (planes) {
+          if (elu) { v0 = elu_f(v0); v1 = elu_f(v1); }
+          const uint32_t ep = tp + h * 512 + ((16 * jj) ^ swp);
+          __half2 hv, lv;
+          split_f16(v0, hv.x, lv.x);
+          split_f16(v1, hv.y, lv.y);
+          st_shared_b32(ep, *reinterpret_cast<const uint32_t*>(&hv));
+          if (lo) st_shared_b32(ep + LO_OFF, *reinterpret_cast<const uint32_t*>(&lv));
+        }
       }
     }
     fence_proxy_async();
     named_bar_sync(2 + e.cw, 128);
     if (leader) {
       tma_store_3d(tmO, buf, e.n0 + 32 * s, e.row0, e.b);
+      if (planes) {
+        tma_store_3d(tmHi, e.buf + EPI_SUB_BYTES, e.n0 + 32 * s, e.row0, e.b);
+        if (lo) tma_store_3d(tmLo, e.buf + EPI_SUB_BYTES + LO_OFF, e.n0 + 32 * s, e.row0, e.b);
+      }
       bulk_commit();
-      if (res && s + EPI_BUFS < NSUB) {
+      const int next = s + (planes ? 1 : EPI_BUFS);
+      if (res && next < NSUB) {
         bulk_wait_read<0>();
         mbar_arrive_expect_tx(&e.rfull[u], EPI_SUB_BYTES);
-        tma_load_3d(buf, tmR, &e.rfull[u], e.n0 + 32 * (s + EPI_BUFS), e.row0, e.b);
+        tma_load_3d(buf, tmR, &e.rfull[u], e.n0 + 32 * next, e.row0, e.b);
       }
     }
   }
@@ -315,7 +368,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
                const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes,
-               const GemmParams p) {
+               const __grid_constant__ CUtensorMap tmHi, const __grid_constant__ CUtensorMap tmLo, const GemmParams p) {
   constexpr int BM = GEMM_BM, BK = GEMM_BK;
   constexpr int NPL = (NTERMS == 1) ? 1 : 2;
   constexpr uint32_t A_BYTES = BM * BK * 2, W_BYTES = BN * BK * 2;
@@ -340,7 +393,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   if (threadIdx.x == 32) {
     prefetch_tmap(&tmA_hi); prefetch_tmap(&tmW_hi);
     if (NPL == 2) { prefetch_tmap(&tmA_lo); prefetch_tmap(&tmW_lo); }
-    if (tma_epi) { prefetch_tmap(&tmOut); if (p.res.ptr) prefetch_tmap(&tmRes); }
+    if (p.epi == EPI_F32) { prefetch_tmap(&tmOut); if (p.res.ptr) prefetch_tmap(&tmRes); }
+    if (tma_epi && p.ohi.ptr) { prefetch_tmap(&tmHi); if (p.olo.ptr) prefetch_tmap(&tmLo); }
   }
   __syncthreads();
 
@@ -370,6 +424,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     setmaxnreg_inc<GEMM_CONSUMER_REGS>();
     const int cw = wg - 1, wq = warp & 3;      // consumer warpgroup: rows [cw * 64, +64) of the tile
     const bool leader = (threadIdx.x & 127) == 0, epi_res = p.epi == EPI_F32 && p.res.ptr;
+    const int res_bufs = BN == 128 && p.ohi.ptr ? 1 : EPI_BUFS;      // EPI_F32 with planes keeps the second buffer for them
     const bool epi_cols = tma_epi && (p.bias || p.gamma);
     uint32_t stage = 0, phase = 0;
     float acc[BN / 2];
@@ -398,8 +453,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           // while the first MMAs run: the previous tile's stores have left the epilogue buffers, which may now take the
           // first residual subtiles of this one
           bulk_wait_read<0>();
-#pragma unroll
-          for (int u = 0; u < EPI_BUFS; ++u) {
+          for (int u = 0; u < res_bufs; ++u) {
             uint64_t* bar = rfull + cw * EPI_BUFS + u;
             mbar_arrive_expect_tx(bar, EPI_SUB_BYTES);
             tma_load_3d(epi_smem + (cw * EPI_BUFS + u) * EPI_SUB_BYTES, &tmRes, bar, n0 + 32 * u, m0 + cw * 64, b);
@@ -421,9 +475,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       }
       const EpiCtx ec{epi_smem + cw * EPI_BUFS * EPI_SUB_BYTES, rfull + cw * EPI_BUFS, smem_u32(tile_cols), cw, b, m0 + cw * 64, n0};
       if (p.epi == EPI_HI) {
-        epilogue_hi<BN>(p, &tmOut, ec, acc);
+        if constexpr (BN == 128) {
+          if (p.act == QB_ACT_SWIGLU) epilogue_hi<BN, true>(p, &tmHi, &tmLo, ec, acc);
+          else epilogue_hi<BN, false>(p, &tmHi, &tmLo, ec, acc);
+        } else {
+          epilogue_hi<BN, false>(p, &tmHi, &tmLo, ec, acc);
+        }
       } else if (p.epi == EPI_F32) {
-        epilogue_f32<BN>(p, &tmOut, &tmRes, ec, acc);
+        epilogue_f32<BN>(p, &tmOut, &tmRes, &tmHi, &tmLo, ec, acc);
       } else {
         const int r = m0 + cw * 64 + wq * 16 + (lane >> 2), c = n0 + 2 * (lane & 3);
 #pragma unroll
@@ -497,12 +556,13 @@ static EncodeTiledFn get_encode() {
 }
 
 static int make_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                    const cuuint32_t* box, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16) {
+                    const cuuint32_t* box, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+                    CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   EncodeTiledFn enc = get_encode();
   QB_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available (no CUDA driver?)");
   cuuint32_t es[3] = {1, 1, 1};
   CUresult r = enc(m, dtype, rank, const_cast<void*>(base), dims, strides_bytes, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   QB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed: %d (rank %d dims %llu %llu %llu)", (int)r, rank,
              (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)(rank > 2 ? dims[2] : 0));
@@ -513,35 +573,47 @@ static RowMapD to_rm(const qb_rowmap& r) { return RowMapD{r.ptr, (long long)r.ld
 
 static bool aligned(const void* ptr, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(ptr) & (bytes - 1)) == 0; }
 
-// A row map TMA can address as [batch][m_per_batch][N] based at row `off`: 16-byte aligned base and row pitch, columns
-// within the pitch, batches that do not overlap, and rows of whole 16-byte chunks (a TMA store writes the last chunk of a
-// row in full, so a partial one would overwrite the columns past N).
+// Output columns of a launch: SwiGLU reduces each interleaved (gate, up) pair of the N GEMM columns to one.
+static int out_cols(const GemmParams& p) { return p.act == QB_ACT_SWIGLU ? p.N / 2 : p.N; }
+
+// A row map TMA can address as [batch][m_per_batch][out_cols] based at row `off`: 16-byte aligned base and row pitch, columns
+// within the pitch, batches that do not overlap, and rows of whole 16-byte chunks.  The last condition is measured, not
+// assumed: on an H100 a TMA store into a row that ends inside a 16-byte chunk wrote the pad columns of that chunk
+// (tests/test_gemm_tma_planes_gpu.py, SwiGLU at 100 fp16 columns), so such rows, the decoder head's 1922 fp32 columns among
+// them, stay on the generic epilogue.
 static bool tma_rows(const RowMapD& r, long long esize, const GemmParams& p) {
-  return r.ld >= p.N && (r.ld * esize) % 16 == 0 && (p.N * esize) % 16 == 0 && aligned(r.ptr, 16) &&
+  return r.ld >= out_cols(p) && (r.ld * esize) % 16 == 0 && (out_cols(p) * esize) % 16 == 0 && aligned(r.ptr, 16) &&
          (p.a_batch == 1 || r.rpb >= r.off + p.m_per_batch);
 }
 
-// The epilogues epilogue_pair computes with one vector store per pair, when the TMA requirements hold for every buffer the
-// kind reads or writes; each kind computes what epilogue_pair would.
-static int classify_epilogue(const GemmParams& p) {
-  if (p.act2 != QB_ACT_NONE) return EPI_GENERIC;
-  if (p.ohi.ptr && !p.olo.ptr && !p.o32.ptr && !p.res.ptr && !p.gamma && (p.act == QB_ACT_NONE || p.act == QB_ACT_GELU) &&
-      tma_rows(p.ohi, 2, p))
+// The epilogues the fast kinds compute, when the TMA requirements hold for every buffer the kind reads or writes; each kind
+// computes what epilogue_pair would.  The 128 x 256 tile holds 128 accumulators per thread: there the lo plane, ELU, SwiGLU and
+// the planes of EPI_F32 would take the epilogue past the consumers' 232 registers (ptxas spills), so that tile keeps bias
+// (GELU) -> hi and the fp32 kind without planes, and leaves the rest to the generic epilogue.
+static int classify_epilogue(const GemmParams& p, int BN) {
+  const bool wide = BN == 256;
+  const bool planes_ok = !p.ohi.ptr || (tma_rows(p.ohi, 2, p) && (!p.olo.ptr || tma_rows(p.olo, 2, p)));
+  if (p.ohi.ptr && !p.o32.ptr && !p.res.ptr && !p.gamma && p.act2 == QB_ACT_NONE && planes_ok &&
+      (wide ? !p.olo.ptr && (p.act == QB_ACT_NONE || p.act == QB_ACT_GELU)
+            : p.act == QB_ACT_NONE || p.act == QB_ACT_GELU || p.act == QB_ACT_ELU || p.act == QB_ACT_SWIGLU))
     return EPI_HI;
-  if (p.o32.ptr && !p.ohi.ptr && p.act == QB_ACT_NONE && tma_rows(p.o32, 4, p) && (!p.res.ptr || tma_rows(p.res, 4, p)))
+  if (p.o32.ptr && p.act == QB_ACT_NONE && (wide ? !p.ohi.ptr : p.act2 == QB_ACT_NONE || p.act2 == QB_ACT_ELU) && planes_ok &&
+      tma_rows(p.o32, 4, p) && (!p.res.ptr || tma_rows(p.res, 4, p)))
     return EPI_F32;
   return EPI_GENERIC;
 }
 
-// Output / residual map of the fast epilogue kinds: [batch][m_per_batch][N] from row `off`, one 64-row x 128-byte box per subtile.
-static int make_rows_map(CUtensorMap* m, const RowMapD& r, bool f32, const GemmParams& p) {
+// Output / residual / planes map of the fast epilogue kinds: [batch][m_per_batch][out_cols] from row `off`, one 64-row box
+// per subtile, 128 bytes wide (128-byte swizzle) or, for the planes of EPI_F32, 64 bytes (64-byte swizzle).
+static int make_rows_map(CUtensorMap* m, const RowMapD& r, bool f32, int box_bytes, const GemmParams& p) {
   const cuuint64_t es = f32 ? 4 : 2, ld = (cuuint64_t)r.ld;
   const cuuint64_t rows = p.a_batch > 1 ? (cuuint64_t)r.rpb : (cuuint64_t)p.m_per_batch;
-  cuuint64_t dims[3] = {(cuuint64_t)p.N, (cuuint64_t)p.m_per_batch, (cuuint64_t)p.a_batch};
+  cuuint64_t dims[3] = {(cuuint64_t)out_cols(p), (cuuint64_t)p.m_per_batch, (cuuint64_t)p.a_batch};
   cuuint64_t str[2] = {ld * es, rows * ld * es};
-  cuuint32_t box[3] = {(cuuint32_t)(128 / es), 64, 1};
+  cuuint32_t box[3] = {(cuuint32_t)(box_bytes / es), 64, 1};
   return make_map(m, (const char*)r.ptr + r.off * ld * es, 3, dims, str, box,
-                  f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+                  f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+                  box_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
 }
 
 static int fill_params(const qb_gemm_desc* d, GemmParams* p, int BN) {
@@ -573,7 +645,7 @@ static int fill_params(const qb_gemm_desc* d, GemmParams* p, int BN) {
   p->a_hi = (const __half*)d->a_hi; p->a_lo = (const __half*)d->a_lo;
   p->w_hi = (const __half*)d->w_hi; p->w_lo = (const __half*)d->w_lo;
   p->a_rpb = d->a_rows_per_batch; p->a_batch = (int)d->a_batch;
-  p->epi = classify_epilogue(*p);
+  p->epi = classify_epilogue(*p, BN);
   return 0;
 }
 
@@ -598,13 +670,17 @@ static int launch_tc(const qb_gemm_desc* d, cudaStream_t st, int num_sms) {
   } else {
     mA_lo = mA_hi; mW_lo = mW_hi;
   }
-  CUtensorMap mOut = mA_hi, mRes = mA_hi;             // used by the fast epilogue kinds only
-  if (p.epi == EPI_HI) {
-    if (int e = make_rows_map(&mOut, p.ohi, false, p)) return e;
-  } else if (p.epi == EPI_F32) {
-    if (int e = make_rows_map(&mOut, p.o32, true, p)) return e;
+  CUtensorMap mOut = mA_hi, mRes = mA_hi, mHi = mA_hi, mLo = mA_hi;             // used by the fast epilogue kinds only
+  if (p.epi == EPI_F32) {
+    if (int e = make_rows_map(&mOut, p.o32, true, 128, p)) return e;
     if (p.res.ptr)
-      if (int e = make_rows_map(&mRes, p.res, true, p)) return e;
+      if (int e = make_rows_map(&mRes, p.res, true, 128, p)) return e;
+  }
+  if (p.epi != EPI_GENERIC && p.ohi.ptr) {
+    const int box_bytes = p.epi == EPI_HI ? 128 : 64;
+    if (int e = make_rows_map(&mHi, p.ohi, false, box_bytes, p)) return e;
+    if (p.olo.ptr)
+      if (int e = make_rows_map(&mLo, p.olo, false, box_bytes, p)) return e;
   }
   constexpr int NPL = NTERMS == 1 ? 1 : 2;
   // pipeline stages, epilogue subtile buffers, the tile's bias / gamma, mbarriers, and up to 896 bytes that align the
@@ -620,7 +696,7 @@ static int launch_tc(const qb_gemm_desc* d, cudaStream_t st, int num_sms) {
     attr_set[dev] = true;
   }
   int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-  kern<<<grid, GEMM_THREADS, smem, st>>>(mA_hi, mA_lo, mW_hi, mW_lo, mOut, mRes, p);
+  kern<<<grid, GEMM_THREADS, smem, st>>>(mA_hi, mA_lo, mW_hi, mW_lo, mOut, mRes, mHi, mLo, p);
   g_launches++;
   QB_CHECK_CUDA(cudaGetLastError());
   return 0;
