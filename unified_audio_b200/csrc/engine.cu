@@ -49,7 +49,10 @@ struct Arena {
 };
 
 // named, size-keyed workspace: allocated (zeroed) on first use - the first call of a shape is the warm-up, later calls and
-// CUDA-graph captures only reuse.  Zero pads of the padded channel-last buffers are written once and never touched again.
+// CUDA-graph captures only reuse.  The padded channel-last buffers (`padded`) hold clips of rows_per_batch rows whose zero pad
+// rows no kernel writes: they are keyed by (B, rows_per_batch, ld, split) as well, so a buffer is only reused by calls that put
+// their pad rows in the same places and the pads, zeroed at allocation, stay zero.  A size key alone would hand a buffer to a
+// call of another (B, rows_per_batch) with the same product, whose pad rows hold the earlier call's activations.
 struct Workspace {
   Arena arena;
   std::map<std::string, void*> bufs;
@@ -71,6 +74,11 @@ struct Workspace {
     out->lo = nullptr;
     if (split) QB_TRY(get((void**)&out->lo, name + ".lo", n * 2));
     return 0;
+  }
+  // planes [B, rows_per_batch, ld] with zero pad rows, keyed by their row layout
+  int padded(PlanesD* out, const std::string& name, int64_t B, int64_t rpb, int64_t ld, bool split) {
+    const std::string key = name + "[" + std::to_string(B) + "x" + std::to_string(rpb) + "x" + std::to_string(ld) + (split ? "s]" : "]");
+    return planes(out, key, (size_t)(B * rpb * ld), split);
   }
 };
 
@@ -527,7 +535,7 @@ static int run_resnet(qb_codec* c, const ResnetW& R, float* x, int64_t B, int64_
   float *stats, *h;
   PlanesD pr;
   QB_TRY(c->ws.f32(&stats, "gn_stats", (size_t)B * 32 * 2));
-  QB_TRY(c->ws.planes(&pr, "res_pr", (size_t)B * (F + 2) * C, c->pol.conv));
+  QB_TRY(c->ws.padded(&pr, "res_pr", B, F + 2, C, c->pol.conv));
   QB_TRY(c->ws.f32(&h, "res_h", (size_t)M * C));
   QB_TRY(qb_groupnorm_stats(x, B, F, C, 32, 1e-6f, stats, st));
   QB_TRY(qb_groupnorm_apply(x, stats, R.n1w, R.n1b, B, F, C, 32, 1, nullptr, (qb_half*)pr.hi, (qb_half*)pr.lo, C, F + 2, 1, st));
@@ -547,7 +555,7 @@ static int encode_emb(qb_codec* c, const float* wav, int64_t B, int64_t T, float
   const int64_t F = T / hop, N = F / stride, M = B * F;
   PlanesD feat, fin, ga, Z;
   float *Y, *X, *x0, *x, *emb;
-  QB_TRY(c->ws.planes(&feat, "enc_feat", (size_t)B * (F + 2) * c->feat_ld, c->pol.conv));
+  QB_TRY(c->ws.padded(&feat, "enc_feat", B, F + 2, c->feat_ld, c->pol.conv));
   // two-stage DFT: gather -> P-point DFTs (GEMM, K = 64) -> twiddle -> Q-point DFTs (GEMM, K = 128) -> log-magnitude / phase
   const int P = c->stft_P, Q = c->stft_Q;
   QB_TRY(c->ws.planes(&ga, "enc_sg", (size_t)M * Q * 64, true));
@@ -571,7 +579,7 @@ static int encode_emb(qb_codec* c, const float* wav, int64_t B, int64_t T, float
   tap(c, "enc.post", x, B, F, C);
   const int k = 2 * stride + 1, pad = k / 2;
   const int64_t rpb = pad_to(F + 2 * pad, stride);
-  QB_TRY(c->ws.planes(&fin, "enc_fin", (size_t)B * rpb * C, c->pol.conv));
+  QB_TRY(c->ws.padded(&fin, "enc_fin", B, rpb, C, c->pol.conv));
   QB_TRY(qb_layernorm(x, c->e_fnorm_w, c->e_fnorm_b, 1e-6f, B, F, C, nullptr, (qb_half*)fin.hi, (qb_half*)fin.lo, C, rpb, pad, st));
   QB_TRY(c->ws.f32(&emb, "enc_emb", (size_t)B * N * Dq));
   QB_TRY(G(fin, B, rpb, C, N, c->e_out, Dq, k, stride).bias(c->e_out_b).out32(emb, Dq, N, 0).run(st));
@@ -589,11 +597,11 @@ static int encode_sem(qb_codec* c, const float* feat_in, int64_t B, int64_t F, f
   const int cin_pad = (int)pad_to(Cin, 64);
   PlanesD fin, pe, pu;
   float* sx;
-  QB_TRY(c->ws.planes(&fin, "sem_in", (size_t)B * (F + 2) * cin_pad, pc));
+  QB_TRY(c->ws.padded(&fin, "sem_in", B, F + 2, cin_pad, pc));
   QB_TRY(qb_bct_to_planes(feat_in, B, Cin, F, (qb_half*)fin.hi, (qb_half*)fin.lo, cin_pad, F + 2, 1, st));
   int64_t Tc = F;
   QB_TRY(c->ws.f32(&sx, "sem_x" + std::to_string(Tc), (size_t)B * Tc * Cs));
-  QB_TRY(c->ws.planes(&pe, "sem_pe" + std::to_string(Tc), (size_t)B * (Tc + 2) * Cs, pc));
+  QB_TRY(c->ws.padded(&pe, "sem_pe" + std::to_string(Tc), B, Tc + 2, Cs, pc));
   QB_TRY(G(fin, B, F + 2, cin_pad, F, c->s_conv, Cs, 3).out32(sx, Cs, Tc, 0).outp(pe, Cs, Tc + 2, 1).act2(QB_ACT_ELU).run(st));
   const int nb = (int)c->s_blocks.size();
   for (int bi = 0; bi < nb; ++bi) {
@@ -610,7 +618,7 @@ static int encode_sem(qb_codec* c, const float* feat_in, int64_t B, int64_t F, f
     float* sx2;
     PlanesD pe2;
     QB_TRY(c->ws.f32(&sx2, "sem_x" + std::to_string(Tn) + "_" + std::to_string(bi), (size_t)B * Tn * Cs));
-    QB_TRY(c->ws.planes(&pe2, "sem_pe" + std::to_string(Tn) + "_" + std::to_string(bi), (size_t)B * (Tn + 2) * Cs, pc));
+    QB_TRY(c->ws.padded(&pe2, "sem_pe" + std::to_string(Tn) + "_" + std::to_string(bi), B, Tn + 2, Cs, pc));
     QB_TRY(G(pe, B, Tc + 2, Cs, Tn, blk.conv, Cs, k, s).bias(blk.conv_b).out32(sx2, Cs, Tn, 0).outp(pe2, Cs, Tn + 2, 1)
                .act2(bi + 1 < nb ? QB_ACT_ELU : QB_ACT_NONE).run(st));
     sx = sx2; pe = pe2; Tc = Tn;
@@ -635,7 +643,7 @@ static int decode_z(qb_codec* c, const float* z, int64_t B, int64_t N, float* wa
   const int k = f + 1, pad = k / 2;
   PlanesD zin, t1, sp;
   float *x, *stats, *h, *head, *frames;
-  QB_TRY(c->ws.planes(&zin, "dec_zin", (size_t)B * (F + 2 * pad) * Cin, c->pol.conv));
+  QB_TRY(c->ws.padded(&zin, "dec_zin", B, F + 2 * pad, Cin, c->pol.conv));
   QB_TRY(qb_rows_to_planes(z, B, N, Cin, f, QB_ACT_NONE, (qb_half*)zin.hi, (qb_half*)zin.lo, Cin, F + 2 * pad, pad, st));
   QB_TRY(c->ws.f32(&x, "dec_x", (size_t)M * C));
   QB_TRY(G(zin, B, F + 2 * pad, Cin, F, c->d_embed, C, k).bias(c->d_embed_b).out32(x, C, F, 0).run(st));
