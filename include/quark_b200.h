@@ -284,6 +284,52 @@ int qb_lm_head_argmax_tc(const float* x, int64_t B, int32_t hidden, const qb_hal
  * accuracy -> out = {loss, accuracy}; workspace: 2*M floats.  One pass over the logits, deterministic reduction. */
 int qb_lm_loss(const float* logits, int64_t ld, int64_t M, int32_t V, const int64_t* targets, float label_smoothing, float* workspace,
                float* out, void* stream);
+/* ---- training: gradients of the teacher-forced loss (csrc/lm_train.cu) ----
+ * Deterministic: no floating-point atomics, fixed-order reductions, fp64 partials where a sum runs over tokens.  The dense
+ * contractions of the backward pass are qb_gemm calls in the 3-term split mode; these entry points are the rest.
+ *
+ * Attention dropout mask (transformers' Llama attention in train mode: dropout on the softmax output, before P V): key j of query i in
+ * head h of batch row b, decoder layer `layer`, is kept iff (r >> 8) >= round(p * 2^24), where r is word (j & 3) of
+ * Philox4x32-10(key = {seed & 0xffffffff, seed >> 32}, counter = {i, j >> 2, b * heads + h, layer}); kept probabilities are scaled by
+ * 1 / (1 - p).  The mask is a pure function of (seed, layer, b, h, i, j), so the backward pass regenerates it.
+ *
+ * qb_lm_attn_train_fwd: causal attention, head_dim 64, fp32 SIMT.  qkv [B*L, 3*heads*64] fp32 (rope tables as qb_attention_umma)
+ * -> qs = RoPE(q) / 8, kr = RoPE(k), v, each [B*heads, L, 64] (kept for the backward pass), out [B*L, heads*64] fp32 and the row
+ * log-sum-exp lse [B*heads, L] of the undropped scores.  0 <= dropout_p < 1.
+ * qb_lm_attn_train_bwd: dout [B*L, heads*64] -> dqkv [B*L, 3*heads*64] (RoPE undone on dq and dk), P recomputed from lse with the same
+ * mask; dK / dV summed per key tile and dQ per query tile.  workspace: B*heads*L floats. */
+int qb_lm_attn_train_fwd(const float* qkv, int64_t B, int64_t L, int32_t heads, const float* rope_cos, const float* rope_sin,
+                         float dropout_p, uint64_t seed, int32_t layer, float* qs, float* kr, float* v, float* out, float* lse,
+                         void* stream);
+int qb_lm_attn_train_bwd(const float* qs, const float* kr, const float* v, const float* out, const float* dout, const float* lse,
+                         int64_t B, int64_t L, int32_t heads, const float* rope_cos, const float* rope_sin, float dropout_p,
+                         uint64_t seed, int32_t layer, float* dqkv, float* workspace, void* stream);
+/* Gradient of qb_lm_loss's loss times *grad_loss (a device float) w.r.t. the logits, times M * scale: *grad_loss * (softmax(logits) - t)
+ * * scale with t the smoothed target -> out fp32 and hi / lo planes, all [M, ld_out] (columns V.. zero).  Most entries are ~1/V, below
+ * fp16's normal range: a power-of-two scale near V (<= 2^14, so that |out| <= 2^14 |*grad_loss|) keeps the planes fp32-grade.  The caller
+ * takes the scale back out (LLM_SFT: the head GEMM's gamma; qb_col_sum / qb_embedding_bwd scale the parameter gradients). */
+int qb_lm_loss_bwd(const float* logits, int64_t ld, int64_t M, int32_t V, const int64_t* targets, float label_smoothing,
+                   const float* grad_loss, float scale, float* out, qb_half* out_hi, qb_half* out_lo, int64_t ld_out, void* stream);
+/* RMSNorm backward (eps as qb_rmsnorm): dx = (accumulate ? dx : 0) + d/dx; gw [rows, C] = dy * x * rms^-1 (qb_col_sum gives dw). */
+int qb_rmsnorm_bwd(const float* x, const float* w, const float* dy, float eps, int64_t rows, int64_t C, float* dx, int32_t accumulate,
+                   float* gw, void* stream);
+/* out[c] = (accumulate ? out[c] : 0) + scale * sum over r = 0..rows-1 in order of x[r * ld + c], in fp64 (chunks of 128 rows, then the
+ * chunks in order).  workspace: qb_col_sum_workspace_bytes(rows, C). */
+int64_t qb_col_sum_workspace_bytes(int64_t rows, int64_t C);
+int qb_col_sum(const float* x, int64_t rows, int64_t C, int64_t ld, double scale, void* workspace, float* out, int32_t accumulate,
+               void* stream);
+/* gu [M, 2*inter] fp32, (gate, up) interleaved per column: qb_swiglu -> h = silu(gate) * up, fp32 and planes [M, inter];
+ * qb_swiglu_bwd: dh [M, inter] -> d(gate, up) [M, 2*inter] fp32 and planes. */
+int qb_swiglu(const float* gu, int64_t M, int64_t inter, float* h, qb_half* hi, qb_half* lo, void* stream);
+int qb_swiglu_bwd(const float* gu, const float* dh, int64_t M, int64_t inter, float* dgu, qb_half* hi, qb_half* lo, void* stream);
+/* x [rows, cols] fp32 (row pitch ldx) -> hi / lo planes [S][cols][ks], element (s, c, k) = x[s*ks + k, c], S = ceil(rows / ks), rows
+ * past `rows` zero; ks a multiple of 64.  Slice s is the A or W operand of one split-K slice of a weight gradient dW = dY^T X. */
+int qb_transpose_split(const float* x, int64_t rows, int64_t cols, int64_t ldx, int64_t ks, qb_half* hi, qb_half* lo, void* stream);
+/* Embedding gradient: out[v] (+)= scale * sum over k with ids[k] == v, in increasing k and in fp64, of dx row (k / Lt) * L + P + k % Lt
+ * (rows of H floats); ids [n] int64 in [0, V).  H <= 1024. */
+int qb_embedding_bwd(const float* dx, const int64_t* ids, int64_t n, int64_t Lt, int64_t L, int64_t P, int32_t H, int32_t V,
+                     double scale, float* out, int32_t accumulate, void* stream);
+
 /* Sampled decoding step (CustomLlamaModel.sample_logits, QuarkAudio-UniSE/model/llm/llm.py:253-289, as called from
  * llm_sft.py:155-161,184-190 with the reference defaults temperature 0.8, top_k 50, top_p 0.95, do_sample=True):
  * as qb_lm_head_argmax_tc, but the head also writes the range logits to `logits` [B][max_cols] and the token is drawn as

@@ -132,7 +132,18 @@ SIGNATURES = {
     "qb_rvq_encode_rows": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp]),
     "qb_rvq_decode_rows": (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
     "qb_lm_loss": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _f32, _vp, _vp, _vp]),
-    "qb_lm_head_sample_tc": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _i32,
+    "qb_lm_attn_train_fwd": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _vp, _f32, C.c_uint64, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "qb_lm_attn_train_bwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i32, _vp, _vp, _f32, C.c_uint64, _i32, _vp, _vp,
+                                       _vp]),
+    "qb_lm_loss_bwd": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _f32, _vp, _f32, _vp, _vp, _vp, _i64, _vp]),
+    "qb_rmsnorm_bwd": (C.c_int, [_vp, _vp, _vp, _f32, _i64, _i64, _vp, _i32, _vp, _vp]),
+    "qb_col_sum_workspace_bytes": (C.c_int64, [_i64, _i64]),
+    "qb_col_sum": (C.c_int, [_vp, _i64, _i64, _i64, C.c_double, _vp, _vp, _i32, _vp]),
+    "qb_swiglu": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "qb_swiglu_bwd": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "qb_transpose_split": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp]),
+    "qb_embedding_bwd": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, C.c_double, _vp, _i32, _vp]),
+    "qb_lm_head_sample_tc":(C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _i32,
                                        _f32, _vp, _vp, _vp]),
 }
 

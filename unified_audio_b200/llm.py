@@ -122,10 +122,17 @@ class LLM_SFT(_Face):
         super()._drop_prepared()
         self._gen_state, self._lane_views = {}, None          # captured graphs point into the dropped weights and workspace
 
+    def _param_versions(self):
+        """(version counter, storage) of every parameter: an optimizer step changes them in place, which bumps the counters"""
+        return tuple((p._version, p.data_ptr()) for p in self.parameters())
+
     def _prepare(self):
-        if self._w is not None:
+        if self._w is not None and self._w["versions"] == self._param_versions():
             return self._w
+        if self._w is not None:
+            self._drop_prepared()                  # the parameters changed in place since the weights were packed
         self._require_cuda()
+        versions = self._param_versions()
         sd = {k: v.detach().float() for k, v in self.state_dict().items()}
         layers = []
         for i in range(self.n_layers):
@@ -148,7 +155,7 @@ class LLM_SFT(_Face):
                        head_p=ops.lm_pack_weight(sd["output_head.weight"] * sd["norm.weight"][None, :]),
                        emb=sd["codec_embedding.weight"].contiguous(),
                        adapter=ops.pad_k_planes(sd["adapter.weight"], _pad_to(sd["adapter.weight"].shape[1], 64)),
-                       adapter_b=sd["adapter.bias"].contiguous(), cos=None, sin=None, rope_rows=0)
+                       adapter_b=sd["adapter.bias"].contiguous(), cos=None, sin=None, rope_rows=0, versions=versions)
         self._ensure_rope(self.max_pos)
         return self._w
 
@@ -297,15 +304,30 @@ class LLM_SFT(_Face):
         return torch.gather(z, 1, idx.to(prefix.device)[..., None].expand(B, P, H))
 
     # ------------------------------------------------------------------ teacher-forced forward (llm_sft.py:37-89)
-    @torch.no_grad()
-    def forward(self, task_name, enroll_mel, enroll_feats, mix_mel, mix_feats, global_ids, semantic_ids, return_logits=False):
-        W = self._prepare()
+    def _ids(self, global_ids, semantic_ids):
         g = global_ids.long() + self.global_offset
         s = semantic_ids.long() + self.semantic_offset
         B = g.shape[0]
         col = lambda v: torch.full((B, 1), v, dtype=torch.long, device=g.device)
-        input_ids = torch.cat([col(0), g, col(1), s], 1)
-        target_ids = torch.cat([g, col(1), s, col(2)], 1)
+        return torch.cat([col(0), g, col(1), s], 1), torch.cat([g, col(1), s, col(2)], 1)
+
+    def forward(self, task_name, enroll_mel, enroll_feats, mix_mel, mix_feats, global_ids, semantic_ids, return_logits=False,
+                dropout_seed: Optional[int] = None):
+        """llm_sft.py:37-89 -> (loss, acc[, logits]).  In eval mode with no parameter requiring grad: the inference path (no autograd).
+        In train mode, or when grad mode is on and the parameters require grad: the training path, whose loss has a grad_fn
+        (`loss.backward()` accumulates fp32 gradients into every parameter's .grad) and which applies attention dropout with
+        probability llm_base_config["dropout_p"] in train mode (mask: include/quark_b200.h, from `dropout_seed`, default a draw of
+        torch's CPU generator).  No gradient flows into enroll_feats / mix_feats (the reference detaches them, model.py:37-51)."""
+        if self.training or (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
+            return self._train_forward(task_name, enroll_feats if enroll_mel is not None else None, mix_feats, global_ids, semantic_ids,
+                                       return_logits, dropout_seed)
+        with torch.no_grad():
+            return self._eval_forward(task_name, enroll_mel, enroll_feats, mix_mel, mix_feats, global_ids, semantic_ids, return_logits)
+
+    def _eval_forward(self, task_name, enroll_mel, enroll_feats, mix_mel, mix_feats, global_ids, semantic_ids, return_logits=False):
+        W = self._prepare()
+        input_ids, target_ids = self._ids(global_ids, semantic_ids)
+        B = input_ids.shape[0]
         emb = torch.cat([self._prefix(task_name, enroll_feats if enroll_mel is not None else None, mix_feats),
                          W["emb"][input_ids]], 1)
         hs = self.llm_forward(emb).last_hidden_state[:, -target_ids.shape[1]:].contiguous()
@@ -323,6 +345,205 @@ class LLM_SFT(_Face):
         if return_logits:
             logits = logits[:, :V].reshape(B, Lt, V)
         return (loss, acc, logits) if return_logits else (loss, acc)
+
+    # ------------------------------------------------------------------ training path: forward that keeps activations, backward
+    def _train_forward(self, task_name, enroll_feats, mix_feats, global_ids, semantic_ids, return_logits, dropout_seed):
+        self._require_cuda()
+        if dropout_seed is None:
+            dropout_seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        input_ids, target_ids = self._ids(global_ids, semantic_ids)
+        run = dict(task=task_name, enroll=None if enroll_feats is None else enroll_feats.detach().float().contiguous(),
+                   mix=mix_feats.detach().float().contiguous(), input_ids=input_ids.contiguous(),
+                   targets=target_ids.reshape(-1).contiguous(), seed=int(dropout_seed),
+                   p=float(self.cfg.get("dropout_p", 0.1)) if self.training else 0.0)
+        names = list(dict(self.named_parameters()))
+        loss, acc, logits = _LMLoss.apply(self, run, names, *[p for _, p in self.named_parameters()])
+        if return_logits:
+            B, Lt = input_ids.shape
+            return loss, acc, logits[:, :self.vocab_size].reshape(B, Lt, self.vocab_size)
+        return loss, acc
+
+    def _train_rope(self, L):
+        rows = max(self.max_pos, -(-L // 1024) * 1024)
+        return self._cached(("train_rope", rows), lambda: ops.rope_tables(rows, 64, self._dev()))
+
+    @staticmethod
+    def _split(w: torch.Tensor) -> Planes:
+        """live fp32 parameter [n, k] -> hi / lo planes (k padded with zeros to a multiple of 64)"""
+        n, k = w.shape
+        kp = _pad_to(k, 64)
+        out = Planes(torch.empty(n, kp, dtype=torch.float16, device=w.device), torch.empty(n, kp, dtype=torch.float16, device=w.device))
+        if kp == k:
+            ops.split_f16(w, out)
+        else:
+            ops.rows_to_planes(w, 1, n, k, out, kp, n, 0)
+        return out
+
+    @staticmethod
+    def _transposed(w: torch.Tensor) -> Planes:
+        """live fp32 parameter [n, k] -> planes of W^T [k, pad64(n)]: the weight operand of the data gradient dX = dY W"""
+        t = ops.transpose_split(w, w.shape[0], w.shape[1], _pad_to(w.shape[0], 64))
+        return Planes(t.hi[0], t.lo[0])
+
+    def _train_fwd(self, run, prm):
+        H, heads, I, nl = self.hidden, self.heads, 4 * self.hidden, self.n_layers
+        mix, enr = run["mix"], run["enroll"]
+        B, Tm, Fd = mix.shape
+        if Fd != self.adapter.weight.shape[1]:
+            raise ValueError(f"features have {Fd} channels, the adapter takes {self.adapter.weight.shape[1]}")
+        if enr is not None and enr.shape[0] != B:
+            raise ValueError(f"enroll_feats has {enr.shape[0]} rows, mix_feats {B}")
+        Te = 0 if enr is None else enr.shape[1]
+        dev = mix.device
+        feats = mix.reshape(-1, Fd) if enr is None else torch.cat([enr.reshape(-1, Fd), mix.reshape(-1, Fd)], 0)
+        Nf = feats.shape[0]
+        fa = self._split(feats)
+        ad = torch.empty(Nf, H, device=dev)
+        ops.gemm(fa, self._split(prm["adapter.weight"]), H, a_batch=1, a_rows_per_batch=Nf, a_ld=fa.hi.shape[1], m_per_batch=Nf,
+                 bias=prm["adapter.bias"], out_f32=rowmap(ad, H, Nf, 0))
+        row = lambda w: w[None, None].expand(B, 1, H)
+        parts = [row(prm["task_embedding.weight"][self.task_map[run["task"]]])]
+        if enr is not None:
+            parts += [row(prm["enroll_sos_embedding.weight"][0]), ad[:B * Te].reshape(B, Te, H)]
+        parts += [row(prm["mix_sos_embedding.weight"][0]), ad[B * Te:].reshape(B, Tm, H)]
+        P = 2 + Tm + (1 + Te if enr is not None else 0)
+        ids = run["input_ids"]
+        Lt = ids.shape[1]
+        L, M, Mt = P + Lt, B * (P + Lt), B * Lt
+        x = torch.cat(parts + [prm["codec_embedding.weight"][ids]], 1).reshape(M, H).contiguous()
+        cos, sin = self._train_rope(L)
+        t1 = Planes(torch.empty(M, H, dtype=torch.float16, device=dev), torch.empty(M, H, dtype=torch.float16, device=dev))
+        hp = Planes(torch.empty(M, I, dtype=torch.float16, device=dev), torch.empty(M, I, dtype=torch.float16, device=dev))
+        qkv = torch.empty(M, 3 * H, device=dev)
+        lin = lambda a, w, n, K, **kw: ops.gemm(a, w, n, a_batch=1, a_rows_per_batch=M, a_ld=K, m_per_batch=M, **kw)
+        xm = rowmap(x, H, M, 0)
+        saved = []
+        for i in range(nl):
+            p = f"layers.{i}."
+            s = dict(x=x.clone())
+            ops.rmsnorm(x, prm[p + "input_layernorm.weight"], M, H, t1)
+            wqkv = torch.cat([prm[p + f"self_attn.{n}_proj.weight"] for n in "qkv"], 0)
+            lin(t1, self._split(wqkv), 3 * H, H, out_f32=rowmap(qkv, 3 * H, M, 0))
+            s.update(qs=torch.empty(B * heads, L, 64, device=dev), kr=torch.empty(B * heads, L, 64, device=dev),
+                     v=torch.empty(B * heads, L, 64, device=dev), o=torch.empty(M, H, device=dev), lse=torch.empty(B * heads, L, device=dev))
+            ops.lm_attn_train_fwd(qkv, B, L, heads, cos, sin, run["p"], run["seed"], i, s["qs"], s["kr"], s["v"], s["o"], s["lse"])
+            ops.split_f16(s["o"], t1)
+            lin(t1, self._split(prm[p + "self_attn.o_proj.weight"]), H, H, residual=xm, out_f32=xm)
+            s["xm"] = x.clone()
+            ops.rmsnorm(x, prm[p + "post_attention_layernorm.weight"], M, H, t1)
+            wgu = torch.stack([prm[p + "mlp.gate_proj.weight"], prm[p + "mlp.up_proj.weight"]], 1).reshape(2 * I, H)
+            s["gu"], s["h"] = torch.empty(M, 2 * I, device=dev), torch.empty(M, I, device=dev)
+            lin(t1, self._split(wgu), 2 * I, H, out_f32=rowmap(s["gu"], 2 * I, M, 0))
+            ops.swiglu(s["gu"], M, I, s["h"], hp)
+            lin(hp, self._split(prm[p + "mlp.down_proj.weight"]), H, I, residual=xm, out_f32=xm)
+            saved.append(s)
+        hs = torch.empty(M, H, device=dev)
+        ops.rmsnorm(x, prm["norm.weight"], M, H, out_f32=hs)
+        hst = hs.reshape(B, L, H)[:, P:].reshape(Mt, H).contiguous()
+        V = self.vocab_size
+        vpad = (V + 3) // 4 * 4
+        logits = torch.empty(Mt, vpad, device=dev)
+        lin_t = self._split(hst)
+        ops.gemm(lin_t, self._split(prm["output_head.weight"]), V, a_batch=1, a_rows_per_batch=Mt, a_ld=H, m_per_batch=Mt,
+                 out_f32=rowmap(logits, vpad, Mt, 0))
+        la = ops.lm_loss(logits, vpad, Mt, V, run["targets"], self.label_smoothing)
+        ctx = dict(layers=saved, xL=x, hst=hst, logits=logits, feats=feats, B=B, L=L, P=P, Lt=Lt, Te=Te, Tm=Tm)
+        return la[0], la[1], logits, ctx
+
+    def _train_bwd(self, run, prm, sv, grad_loss):
+        H, heads, I, nl, V = self.hidden, self.heads, 4 * self.hidden, self.n_layers, self.vocab_size
+        B, L, P, Lt, Te, Tm = (sv[k] for k in ("B", "L", "P", "Lt", "Te", "Tm"))
+        M, Mt = B * L, B * Lt
+        dev = grad_loss.device
+        cos, sin = self._train_rope(L)
+        g = {}
+        # head + loss: dlogits once, as fp32 rows (for dW) and planes (for dX), written times Mt * scale (qb_lm_loss_bwd: its ~1/V
+        # entries stay out of fp16's subnormal range).  The head's data-gradient GEMM takes `scale` back out (gamma, a power of two), so
+        # the rest of the backward pass runs in units of Mt, where a row's gradients are O(1) in fp16 planes; every parameter gradient
+        # is written times `unscale`.
+        Vp = _pad_to(V, 64)
+        scale = ops.lm_loss_scale(V)
+        unscale = 1.0 / Mt
+        dlog = torch.empty(Mt, Vp, device=dev)
+        dlp = Planes(torch.empty(Mt, Vp, dtype=torch.float16, device=dev), torch.empty(Mt, Vp, dtype=torch.float16, device=dev))
+        ops.lm_loss_bwd(sv["logits"], sv["logits"].shape[1], Mt, V, run["targets"], self.label_smoothing,
+                        grad_loss.float().contiguous(), dlog, dlp, Vp, scale)
+        g["output_head.weight"] = ops.weight_grad(dlog, sv["hst"], Mt, V, H, torch.empty(V, H, device=dev), dy_ld=Vp,
+                                                  scale=unscale / scale)
+        dhs = torch.zeros(M, H, device=dev)
+        ops.gemm(dlp, self._transposed(prm["output_head.weight"]), H, a_batch=B, a_rows_per_batch=Lt, a_ld=Vp, m_per_batch=Lt,
+                 gamma=torch.full((H,), 1.0 / scale, device=dev), out_f32=rowmap(dhs, H, L, P))
+        dx, gw = torch.empty(M, H, device=dev), torch.empty(M, H, device=dev)
+        nrm = torch.empty(M, H, device=dev)
+
+        def norm_bwd(x, name, dy, accumulate):
+            ops.rmsnorm_bwd(x, prm[name], dy, M, H, dx, gw, accumulate)
+            g[name] = torch.empty(H, device=dev)
+            ops.col_sum(gw, M, H, H, g[name], scale=unscale)
+
+        def planes(t):
+            out = Planes(torch.empty(t.shape, dtype=torch.float16, device=dev), torch.empty(t.shape, dtype=torch.float16, device=dev))
+            ops.split_f16(t, out)
+            return out
+
+        lin = lambda a, w, n, K, out: ops.gemm(a, w, n, a_batch=1, a_rows_per_batch=M, a_ld=K, m_per_batch=M, out_f32=rowmap(out, n, M, 0))
+        norm_bwd(sv["xL"], "norm.weight", dhs, False)
+        for i in reversed(range(nl)):
+            p, s = f"layers.{i}.", sv["layers"][i]
+            # MLP: x_out = xm + down(swiglu(gate_up(rmsnorm(xm))))
+            g[p + "mlp.down_proj.weight"] = ops.weight_grad(dx, s["h"], M, H, I, torch.empty(H, I, device=dev), scale=unscale)
+            dh = torch.empty(M, I, device=dev)
+            lin(planes(dx), self._transposed(prm[p + "mlp.down_proj.weight"]), I, H, dh)
+            dgu = torch.empty(M, 2 * I, device=dev)
+            dgp = Planes(torch.empty(M, 2 * I, dtype=torch.float16, device=dev), torch.empty(M, 2 * I, dtype=torch.float16, device=dev))
+            ops.swiglu_bwd(s["gu"], dh, M, I, dgu, dgp)
+            del dh
+            ops.rmsnorm(s["xm"], prm[p + "post_attention_layernorm.weight"], M, H, out_f32=nrm)
+            ggu = ops.weight_grad(dgu, nrm, M, 2 * I, H, torch.empty(2 * I, H, device=dev), scale=unscale)
+            g[p + "mlp.gate_proj.weight"], g[p + "mlp.up_proj.weight"] = ggu[0::2].contiguous(), ggu[1::2].contiguous()
+            wgu = torch.stack([prm[p + "mlp.gate_proj.weight"], prm[p + "mlp.up_proj.weight"]], 1).reshape(2 * I, H)
+            dn = torch.empty(M, H, device=dev)
+            lin(dgp, self._transposed(wgu), H, 2 * I, dn)
+            del dgu, dgp
+            norm_bwd(s["xm"], p + "post_attention_layernorm.weight", dn, True)
+            # attention: xm = x + o_proj(attn(qkv(rmsnorm(x))))
+            g[p + "self_attn.o_proj.weight"] = ops.weight_grad(dx, s["o"], M, H, H, torch.empty(H, H, device=dev), scale=unscale)
+            do = torch.empty(M, H, device=dev)
+            lin(planes(dx), self._transposed(prm[p + "self_attn.o_proj.weight"]), H, H, do)
+            dqkv = torch.empty(M, 3 * H, device=dev)
+            ops.lm_attn_train_bwd(s["qs"], s["kr"], s["v"], s["o"], do, s["lse"], B, L, heads, cos, sin, run["p"], run["seed"], i, dqkv,
+                                  torch.empty(B * heads * L, device=dev))
+            ops.rmsnorm(s["x"], prm[p + "input_layernorm.weight"], M, H, out_f32=nrm)
+            gqkv = ops.weight_grad(dqkv, nrm, M, 3 * H, H, torch.empty(3 * H, H, device=dev), scale=unscale)
+            for j, n in enumerate("qkv"):
+                g[p + f"self_attn.{n}_proj.weight"] = gqkv[j * H:(j + 1) * H]
+            wqkv = torch.cat([prm[p + f"self_attn.{n}_proj.weight"] for n in "qkv"], 0)
+            lin(planes(dqkv), self._transposed(wqkv), H, 3 * H, dn)
+            del dqkv
+            norm_bwd(s["x"], p + "input_layernorm.weight", dn, True)
+            sv["layers"][i] = None                 # free this layer's activations as soon as they are used
+        # inputs_embeds = [task | (enroll_sos, adapter(enroll)) | mix_sos, adapter(mix) | codec_embedding[input_ids]]
+        g["codec_embedding.weight"] = torch.empty(V, H, device=dev)
+        ids = run["input_ids"]
+        ops.embedding_bwd(dx, ids, ids.numel(), Lt, L, P, H, V, g["codec_embedding.weight"], scale=unscale)
+        colrow = lambda pos, out: ops.col_sum(dx[pos:], B, H, L * H, out, scale=unscale)
+        g["task_embedding.weight"] = torch.zeros_like(prm["task_embedding.weight"])
+        colrow(0, g["task_embedding.weight"][self.task_map[run["task"]]])
+        x3 = dx.reshape(B, L, H)
+        if Te:
+            g["enroll_sos_embedding.weight"] = torch.empty(1, H, device=dev)
+            colrow(1, g["enroll_sos_embedding.weight"])
+            da = torch.cat([x3[:, 2:2 + Te].reshape(-1, H), x3[:, 3 + Te:P].reshape(-1, H)], 0).contiguous()
+        else:
+            da = x3[:, 2:P].reshape(-1, H).contiguous()
+        g["mix_sos_embedding.weight"] = torch.empty(1, H, device=dev)
+        colrow(P - Tm - 1, g["mix_sos_embedding.weight"])
+        feats = sv["feats"]
+        Nf, Fd = feats.shape
+        g["adapter.weight"] = ops.weight_grad(da, feats, Nf, H, Fd, torch.empty(H, Fd, device=dev), scale=unscale)
+        g["adapter.bias"] = torch.empty(H, device=dev)
+        ops.col_sum(da, Nf, H, H, g["adapter.bias"], scale=unscale)
+        return g
 
     # ------------------------------------------------------------------ generate (llm_sft.py:93-195)
     @torch.no_grad()
@@ -512,3 +733,24 @@ class LLM_SFT(_Face):
         global_ids = out_ids[:, :global_length] - self.global_offset          # (new tensors: out_ids is reused by the next call)
         semantic_ids = out_ids[:, global_length + 1:] - self.semantic_offset
         return global_ids, semantic_ids
+
+
+class _LMLoss(torch.autograd.Function):
+    """The teacher-forced loss as one autograd node: forward runs the LM keeping the activations its backward needs, backward runs the
+    library's gradient kernels and returns an fp32 gradient for every parameter (None for one the step did not use)."""
+
+    @staticmethod
+    def forward(ctx, face, run, names, *params):
+        prm = {n: p.detach().float().contiguous() for n, p in zip(names, params)}
+        loss, acc, logits, saved = face._train_fwd(run, prm)
+        ctx.face, ctx.run, ctx.names, ctx.prm, ctx.saved = face, run, names, prm, saved
+        ctx.mark_non_differentiable(acc, logits)
+        return loss, acc, logits
+
+    @staticmethod
+    def backward(ctx, grad_loss, grad_acc, grad_logits):
+        if ctx.saved is None:
+            raise RuntimeError("LLM_SFT training forward: backward called twice on the same graph")
+        g = ctx.face._train_bwd(ctx.run, ctx.prm, ctx.saved, grad_loss)
+        ctx.saved = ctx.prm = None
+        return (None, None, None) + tuple(g.get(n) for n in ctx.names)

@@ -449,6 +449,85 @@ def lm_loss(logits, ld, M, V, targets, label_smoothing):
     return out
 
 
+# ------------------------------------------------------------------ training (csrc/lm_train.cu): gradients of the LM's loss
+def _seed64(seed: int) -> int:
+    return int(seed) & 0xFFFFFFFFFFFFFFFF
+
+
+def lm_attn_train_fwd(qkv, B, L, heads, cos, sin, dropout_p, seed, layer, qs, kr, v, out, lse):
+    _lib.check(_lib.load().qb_lm_attn_train_fwd(_p(qkv), B, L, heads, _p(cos), _p(sin), float(dropout_p), _seed64(seed), int(layer),
+                                                _p(qs), _p(kr), _p(v), _p(out), _p(lse), _stream()))
+
+
+def lm_attn_train_bwd(qs, kr, v, out, dout, lse, B, L, heads, cos, sin, dropout_p, seed, layer, dqkv, workspace):
+    _lib.check(_lib.load().qb_lm_attn_train_bwd(_p(qs), _p(kr), _p(v), _p(out), _p(dout), _p(lse), B, L, heads, _p(cos), _p(sin),
+                                                float(dropout_p), _seed64(seed), int(layer), _p(dqkv), _p(workspace), _stream()))
+
+
+def lm_loss_scale(V: int) -> float:
+    """qb_lm_loss_bwd's output scale: the power of two >= V, at most 2^14"""
+    return float(2 ** min(14, (V - 1).bit_length()))
+
+
+def lm_loss_bwd(logits, ld, M, V, targets, label_smoothing, grad_loss, out, planes: Planes, ld_out, scale):
+    _lib.check(_lib.load().qb_lm_loss_bwd(_p(logits), ld, M, V, _p(targets), float(label_smoothing), _p(grad_loss), float(scale), _p(out),
+                                          _p(planes.hi), _p(planes.lo), ld_out, _stream()))
+
+
+def rmsnorm_bwd(x, w, dy, rows, Cc, dx, gw, accumulate, eps=1e-6):
+    _lib.check(_lib.load().qb_rmsnorm_bwd(_p(x), _p(w), _p(dy), eps, rows, Cc, _p(dx), int(accumulate), _p(gw), _stream()))
+
+
+def col_sum(x, rows, Cc, ld, out, accumulate=False, scale=1.0):
+    """out[c] (+)= scale * sum_r x[r * ld + c], rows in order, fp64 partials"""
+    ws = torch.empty(int(_lib.load().qb_col_sum_workspace_bytes(rows, Cc)), dtype=torch.uint8, device=x.device)
+    _lib.check(_lib.load().qb_col_sum(_p(x), rows, Cc, ld, float(scale), _p(ws), _p(out), int(accumulate), _stream()))
+
+
+def swiglu(gu, M, inter, h, planes: Planes):
+    _lib.check(_lib.load().qb_swiglu(_p(gu), M, inter, _p(h), _p(planes.hi), _p(planes.lo), _stream()))
+
+
+def swiglu_bwd(gu, dh, M, inter, dgu, planes: Planes):
+    _lib.check(_lib.load().qb_swiglu_bwd(_p(gu), _p(dh), M, inter, _p(dgu), _p(planes.hi), _p(planes.lo), _stream()))
+
+
+def transpose_split(x, rows, cols, ks, ldx=None) -> Planes:
+    """x [rows, cols] fp32 -> planes [S, cols, ks] (S = ceil(rows / ks)): slice s holds rows s*ks .. s*ks + ks - 1 transposed"""
+    S = -(-rows // ks)
+    out = Planes(torch.empty(S, cols, ks, dtype=torch.float16, device=x.device), torch.empty(S, cols, ks, dtype=torch.float16, device=x.device))
+    _lib.check(_lib.load().qb_transpose_split(_p(x), rows, cols, cols if ldx is None else ldx, ks, _p(out.hi), _p(out.lo), _stream()))
+    return out
+
+
+def embedding_bwd(dx, ids, n, Lt, L, P, H, V, out, accumulate=False, scale=1.0):
+    _lib.check(_lib.load().qb_embedding_bwd(_p(dx), _p(ids), n, Lt, L, P, H, V, float(scale), _p(out), int(accumulate), _stream()))
+
+
+def grad_slice(tokens: int, n_out: int, n_in: int, sms: int = 132) -> int:
+    """Tokens per split-K slice of a weight gradient [n_out, n_in] contracted over `tokens`: enough slices that the persistent GEMM's
+    128 x 128-ish tiles fill every SM about twice, no slice shorter than 512 tokens (a multiple of 64)."""
+    tiles = -(-n_out // 128) * -(-n_in // 128)
+    slices = max(1, min(-(-2 * sms // tiles), -(-tokens // 512)))
+    per_slice = -(-tokens // slices)
+    return -(-per_slice // 64) * 64
+
+
+def weight_grad(dy, x, tokens, n_out, n_in, out, ks=None, dy_ld=None, scale=1.0):
+    """out [n_out, n_in] = scale * dy^T x over `tokens` rows (dy [tokens, n_out] with row pitch dy_ld, x [tokens, n_in] fp32): the transposed
+    operands cut into slices of ks tokens, one 3-term-split qb_gemm per slice into fp32 partials, the partials summed in slice order
+    in fp64."""
+    ks = grad_slice(tokens, n_out, n_in) if ks is None else ks
+    a, w = transpose_split(dy, tokens, n_out, ks, dy_ld), transpose_split(x, tokens, n_in, ks)
+    S = a.hi.shape[0]
+    part = torch.empty(S, n_out, n_in, device=dy.device)
+    for s in range(S):
+        gemm(Planes(a.hi[s], a.lo[s]), Planes(w.hi[s], w.lo[s]), n_in, a_batch=1, a_rows_per_batch=n_out, a_ld=ks, m_per_batch=n_out,
+             out_f32=rowmap(part[s], n_in, n_out, 0))
+    col_sum(part, S, n_out * n_in, n_out * n_in, out, scale=scale)
+    return out
+
+
 def launch_count() -> int:
     return int(_lib.load().qb_launch_count())
 

@@ -1,12 +1,13 @@
 """UniSE inference and validation surface (`Model.test_step`, `Model.validation_step`) on the device: the callers of the AR-LM hot path.
 
-Mirrors QuarkAudio-UniSE/model/model.py:20-286 (a LightningModule in the reference; a plain nn.Module here - the Lightning task,
-the training step and checkpoint callbacks are out of scope, SURVEY 2):
+Mirrors QuarkAudio-UniSE/model/model.py:20-286 (a LightningModule in the reference; a plain nn.Module here - the Lightning task
+and checkpoint callbacks are out of scope, SURVEY 2):
     Model(config, tokenizer=BiCodecTokenizer(BiCodec), dnn=LLM_SFT, semantic_model=SSLFrontEnd(WAVLM_BASE_PLUS))
     .extract_semantic_features(wavs [B, T] @ 16 kHz) -> [B, T/320, 768]        model.py:37-51
     .stft_logmel(x [B, T]) -> [B, ceil(T/320), 80]                               model.py:53-79
     .validation_step((mode, enroll, mix, speech, interf, fs, lengths, names))    model.py:134-160, modes 'se' / 'tse' / 'rtse'
     .validation_epoch(batches) -> batch-size-weighted epoch means, across ranks   model.py:160 (log_dict on_epoch, sync_dist)
+    .training_step(batch) -> {"loss" (differentiable), "train_acc"}, .configure_optimizers()   model.py:96-124, 327-353
     .test_step((mode, enroll, src, tgt, fs, lengths, names), batch_idx)          model.py:170-286, modes 'se' / 'tse' / 'ss'
 and audio_tokenizer.py:30-125 for `BiCodecTokenizer.detokenize(global_tokens, semantic_tokens)` and, given the wav2vec2 front end,
 `BiCodecTokenizer.tokenize(wav) -> (global_tokens, semantic_tokens)`.
@@ -188,6 +189,49 @@ class Model(nn.Module):
         loss, acc = self.dnn(task_name=mode, enroll_mel=enroll_mel, enroll_feats=enroll_feats, mix_mel=self.mel_like(mix),
                              mix_feats=mix_feats, global_ids=global_tokens.squeeze(1), semantic_ids=semantic_tokens)
         return {"valid_loss": loss, "valid_acc": acc}
+
+    # ------------------------------------------------------------------ training (model.py:96-124, 327-353)
+    def training_step(self, batch, batch_idx=0, dropout_seed: Optional[int] = None):
+        """model.py:96-124: the composition of validation_step (same inputs, same checks) with the LM in train mode, so its attention
+        dropout (llm_base_config["dropout_p"]) applies.  The tokenizer and WavLM run frozen, without autograd, in whatever mode they
+        are in (eval unless the caller changed it), as validation_step runs them.  Returns {"loss", "train_acc"}: `loss` carries the
+        LM's grad_fn, so `loss.backward()` fills the `.grad` of `dnn`'s parameters once they require grad (`configure_optimizers`
+        turns that on).  The LM's previous mode is restored before returning."""
+        self.tokenizer.require_tokenize()
+        mode, enroll, mix, wav = self._validation_inputs(batch)
+        if any(t is not None and t.device.type != "cuda" for t in (enroll, mix, wav)):
+            raise RuntimeError("unified_audio_b200.unise.Model runs on CUDA only (no CPU fallback)")
+        global_tokens, semantic_tokens = self.tokenizer.tokenize(wav)
+        mix_feats = self.extract_semantic_features(mix)
+        enroll_mel = enroll_feats = None
+        if enroll is not None:
+            enroll_mel, enroll_feats = self.mel_like(enroll), self.extract_semantic_features(enroll)
+        was_training = self.dnn.training
+        self.dnn.train()
+        try:
+            loss, acc = self.dnn(task_name=mode, enroll_mel=enroll_mel, enroll_feats=enroll_feats, mix_mel=self.mel_like(mix),
+                                 mix_feats=mix_feats, global_ids=global_tokens.squeeze(1), semantic_ids=semantic_tokens,
+                                 dropout_seed=dropout_seed)
+        finally:
+            self.dnn.train(was_training)
+        return {"loss": loss, "train_acc": acc}
+
+    def configure_optimizers(self):
+        """model.py:327-353: AdamW over the LM's parameters with config["opt"], and a per-step LambdaLR: cosine warm-up over
+        sch.warmup_steps, then step_decay ** (step - warmup_steps) floored at sch.min_factor.  Makes the LM's parameters require
+        grad first.  Returns ([optimizer], [{"scheduler", "interval": "step", "frequency": 1}]) as the reference does."""
+        self.dnn.requires_grad_(True)
+        opt = torch.optim.AdamW(self.dnn.parameters(), **self.config["opt"])
+        sch_cfg = self.config["sch"]
+
+        def warmup_lambda(step):
+            warmup_steps, step_decay = sch_cfg["warmup_steps"], sch_cfg["step_decay"]
+            if step < warmup_steps:
+                return 0.5 * (1 + math.cos(math.pi * (1 - step / warmup_steps)))
+            return max(step_decay ** (step - warmup_steps), sch_cfg["min_factor"])
+
+        sch = {"scheduler": torch.optim.lr_scheduler.LambdaLR(opt, warmup_lambda), "interval": "step", "frequency": 1}
+        return [opt], [sch]
 
     def validation_epoch(self, batches, group=None) -> dict:
         """A validation epoch as the reference logs it (`log_dict(..., on_epoch=True, sync_dist=True)`, model.py:160).  Each batch's
