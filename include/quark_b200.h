@@ -512,6 +512,56 @@ int qb_codec_set_tap(qb_codec* c, qb_tap_fn cb, void* user);
 /* Row-level access to the two quantisers of a loaded codec (which = 0 acoustic, 1 semantic). */
 qb_rvq* qb_codec_rvq(qb_codec* c, int32_t which);
 
+/* ---- UniSE training-data simulation (csrc/simulate.cu): TrainDataLoadIter.process_one_sample after the file reads
+ * (QuarkAudio-UniSE/dataloader/data_module.py:106-140,207-235) and simulate_data with everything it calls (dataloader/simulation/
+ * simulate.py:10-192, rir_utils.py:464-517, detect_non_silence.py:1-98).  Signals are packed ragged rows: one fp32 buffer, int64
+ * offsets [rows + 1] (row r = buf[offs[r] .. offs[r + 1])).  Every random parameter is drawn on the host and passed per row; `on`
+ * (int32 per row) selects the rows a stage applies to.  All reductions are fixed-order with fp64 partials: bit-reproducible. */
+/* mix_noise's rms (simulate.py:25-26) = x[detect_non_silence(x)].std(): frame variance (frame 1024, shift 512, zero padding to whole
+ * frames, boxcar window; detect_non_silence.py:1-98), frames with power / mean > 0.01, one flag per shift, the last repeated; rows
+ * shorter than 1024 or of zero mean power select every sample -> rms [rows] fp64, mask (uint8 per sample, packed as x) or NULL.
+ * frame_off [rows + 1]: frames per row (0 below 1024 samples) cumulated; power: fp64 workspace of frame_off[rows] entries. */
+int qb_sim_active_rms(const float* x, const int64_t* offs, const int64_t* frame_off, int64_t rows, int64_t max_len, int64_t max_frames,
+                      double* power, double* rms, uint8_t* mask, void* stream);
+/* mix_noise's alignment (simulate.py:13-23): dst_r[n] = src_r[(n + shift[r]) mod len(src_r)], n < len(dst_r) (dst packed by offs):
+ * wrap padding from an offset (shift = -offset mod len) or a cut at an offset (shift = offset); empty source rows give zeros. */
+int qb_sim_place(const float* src, const int64_t* src_offs, const int64_t* offs, const int64_t* shift, int64_t rows, int64_t max_len,
+                 float* dst, void* stream);
+/* mix_noise (simulate.py:28-29) in place on rows with on[r]: x = other * (10^(-snr/20) rms_x / (rms_other + 1e-10)) + x; diff (or
+ * NULL) = x_after - x_before, the interferer of simulate.py:147. */
+int qb_sim_mix(float* x, const float* other, const int64_t* offs, int64_t rows, int64_t max_len, const double* snr, const double* rms_x,
+               const double* rms_other, const int32_t* on, float* diff, void* stream);
+/* simulate.py:153 + get_rir_start_sample (rir_utils.py:483-517) on rows with on[r]: hn = h / (max|h| + 1e-5); win [rows, 2] = the
+ * early part [start, end) around the first peak of |hn| with strict thresholds at 0.1 peak (end = peak + 1 when nothing after the peak
+ * falls below); status[r] = 1 when the peak is the last sample (the reference fails there), else 0. */
+int qb_sim_rir_prep(const float* h, const int64_t* offs, int64_t rows, const int32_t* on, float* hn, int64_t* win, int32_t* status,
+                    void* stream);
+/* add_reverberation (rir_utils.py:340-350): y_r[n] = sum_{k in [k0, k1)} h_r[k] x_r[n - k] for n < len(x_r), [k0, k1) = win[r] or the
+ * whole h_r when win is NULL (estimate_early_rir's zeroed RIR is the window); rows off copy x.  y != x. */
+int qb_sim_convolve(const float* x, const int64_t* offs, int64_t rows, int64_t max_len, const float* h, const int64_t* h_offs,
+                    const int64_t* win, const int32_t* on, float* y, void* stream);
+/* bandwidth_limitation (simulate.py:33-52) in place on rows with on[r] and fs_new[r] in {4000, 8000}: 16 kHz -> fs_new -> 16 kHz,
+ * cut to the row's length, with torchaudio's sinc_interp_hann taps (soxr_hq in the reference): down taps [kd] with `wd` leading
+ * zeros of padding, up taps [o, ku] with `wu`.  tmp: a buffer packed as x. */
+int qb_sim_bandwidth(float* x, const int64_t* offs, int64_t rows, int64_t max_len, const int32_t* fs_new, const int32_t* on,
+                     const float* down4, const float* down2, int32_t kd4, int32_t wd4, int32_t kd2, int32_t wd2, const float* up4,
+                     const float* up2, int32_t ku, int32_t wu, float* tmp, void* stream);
+/* clipping (simulate.py:55-76) in place on rows with on[r]: np.quantile(x_r, q[r, 0:2]) ('linear', evaluated in fp64 from exact order
+ * statistics found by radix select -> stats [rows, 4] fp32), np.clip in fp64, rounded once to fp32. */
+int qb_sim_clip(float* x, const int64_t* offs, int64_t rows, int64_t max_len, const double* q, const int32_t* on, float* stats,
+                void* stream);
+/* packet_loss (simulate.py:115-123): x_{lost_row[i]}[lost[i] * packet .. (lost[i] + 1) * packet) = 0 for i < n_lost. */
+int qb_sim_packet_loss(float* x, const int64_t* offs, const int64_t* lost, const int32_t* lost_row, int64_t n_lost, int32_t packet,
+                       void* stream);
+/* simulate.py:181-190 then data_module.py:217-229: the 0.99 peak rule over noisy / speech / interf, the cut at cut_off[r] (wrap
+ * padding when < 0) to `cut` samples, and normalize_src_tgt (has_interf 0) or normalize_mix_speech_inferf with the host uniform
+ * norm_r[r] -> out_mix, out_speech, out_interf (NULL: not written) [rows, cut]. */
+int qb_sim_finish(const float* noisy, const float* speech, const float* interf, const int64_t* offs, int64_t rows, const int32_t* has_interf,
+                  const int64_t* cut_off, const double* norm_r, int64_t cut, float* out_mix, float* out_speech, float* out_interf,
+                  void* stream);
+/* data_module.py:231-233: enrollment cut at cut_off[r] (wrap padding when < 0) to `cut` samples, e / (max|e| + 1e-5) * 0.99. */
+int qb_sim_enroll(const float* e, const int64_t* offs, int64_t rows, const int64_t* cut_off, int64_t cut, float* out, void* stream);
+
 /* ResidualVQ (third-party vector_quantize_pytorch; call sites vq/codec.py:81-82,94-95): codebooks [nq, K, D] fp32. */
 int qb_rvq_load(qb_handle* h, const float* codebooks, int32_t nq, int32_t K, int32_t D, qb_rvq** out);
 void qb_rvq_free(qb_rvq* q);

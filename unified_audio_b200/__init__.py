@@ -17,6 +17,8 @@ Public surface mirrors the reference (alibaba/unified-audio):
                       CodecH15, length-packed codes)
   unise.Model      <- QuarkAudio-UniSE/model/model.py:20-286 (extract_semantic_features / test_step: 'se', 'tse', 'ss') with
                       unise.BiCodecTokenizer <- model/bicodec/audio_tokenizer.py:30-125 (get_ref_clip / tokenize / detokenize)
+  Simulator        <- QuarkAudio-UniSE/dataloader/simulation/simulate.py:126-192 (simulate_data) and the post-load steps of
+                      TrainDataLoadIter.process_one_sample (dataloader/data_module.py:106-140, 207-235): training batches on the GPU
 Kernels live in csrc/ behind the C ABI of include/quark_b200.h (lib/libquark_b200.so).
 """
 __version__ = "0.1.0"
@@ -31,3 +33,4 @@ from . import adaptive  # noqa: E402,F401
 from .ssl import HCodecTokenizer, HUBERT_BASE, SSLFrontEnd, WAV2VEC2_XLSR53, WAVLM_BASE_PLUS, pad_wav, wrap_segments  # noqa: E402,F401
 from .ssl import HCodecTokenizerH1, HCodecTokenizerH15, WAV2VEC2_XLSR53_RAW  # noqa: E402,F401
 from . import unise  # noqa: E402,F401
+from .simulate import Simulator  # noqa: E402,F401

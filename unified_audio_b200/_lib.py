@@ -143,6 +143,16 @@ SIGNATURES = {
     "qb_swiglu_bwd": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp]),
     "qb_transpose_split": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp]),
     "qb_embedding_bwd": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, C.c_double, _vp, _i32, _vp]),
+    "qb_sim_active_rms": (C.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "qb_sim_place": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
+    "qb_sim_mix": (C.c_int, [_vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "qb_sim_rir_prep": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "qb_sim_convolve": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "qb_sim_bandwidth": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _i32, _vp, _vp]),
+    "qb_sim_clip": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "qb_sim_packet_loss": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp]),
+    "qb_sim_finish": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "qb_sim_enroll": (C.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _vp]),
     "qb_lm_head_sample_tc":(C.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _i32,
                                        _f32, _vp, _vp, _vp]),
 }

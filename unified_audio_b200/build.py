@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libquark_b200.so")
-SOURCES = ["gemm.cu", "elementwise.cu", "attention.cu", "attention_umma.cu", "lstm_tc.cu", "rvq.cu", "llm.cu", "lm_train.cu", "engine.cu", "ssl.cu", "adaptive.cu", "speaker.cu"]
+SOURCES = ["gemm.cu", "elementwise.cu", "attention.cu", "attention_umma.cu", "lstm_tc.cu", "rvq.cu", "llm.cu", "lm_train.cu", "engine.cu", "ssl.cu", "adaptive.cu", "speaker.cu", "simulate.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-I" + os.path.join(os.path.dirname(HERE), "include"), "-I" + CSRC]
 

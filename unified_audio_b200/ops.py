@@ -534,3 +534,52 @@ def launch_count() -> int:
 
 def launch_count_reset():
     _lib.load().qb_launch_count_reset()
+
+
+# ------------------------------------------------------------------ training-data simulation (csrc/simulate.cu), packed ragged rows
+def sim_active_rms(x, offs, frame_off, rows, max_len, max_frames, rms, mask=None):
+    """rms [rows] fp64 = std of each row over its non-silent samples (mask: the uint8 flags, packed as x, or None)"""
+    power = torch.empty(max(1, rows * max(1, max_frames)), dtype=torch.float64, device=x.device)
+    _lib.check(_lib.load().qb_sim_active_rms(_p(x), _p(offs), _p(frame_off), rows, max_len, max_frames, _p(power), _p(rms), _p(mask),
+                                             _stream()))
+
+
+def sim_place(src, src_offs, offs, shift, rows, max_len, dst):
+    _lib.check(_lib.load().qb_sim_place(_p(src), _p(src_offs), _p(offs), _p(shift), rows, max_len, _p(dst), _stream()))
+
+
+def sim_mix(x, other, offs, rows, max_len, snr, rms_x, rms_other, on, diff=None):
+    _lib.check(_lib.load().qb_sim_mix(_p(x), _p(other), _p(offs), rows, max_len, _p(snr), _p(rms_x), _p(rms_other), _p(on), _p(diff),
+                                      _stream()))
+
+
+def sim_rir_prep(h, offs, rows, on, hn, win, status):
+    _lib.check(_lib.load().qb_sim_rir_prep(_p(h), _p(offs), rows, _p(on), _p(hn), _p(win), _p(status), _stream()))
+
+
+def sim_convolve(x, offs, rows, max_len, h, h_offs, win, on, y):
+    _lib.check(_lib.load().qb_sim_convolve(_p(x), _p(offs), rows, max_len, _p(h), _p(h_offs), _p(win), _p(on), _p(y), _stream()))
+
+
+def sim_bandwidth(x, offs, rows, max_len, fs_new, on, taps, tmp):
+    """taps: {'down4', 'down2', 'kd4', 'wd4', 'kd2', 'wd2', 'up4', 'up2', 'ku', 'wu'} (Simulator._taps)"""
+    t = taps
+    _lib.check(_lib.load().qb_sim_bandwidth(_p(x), _p(offs), rows, max_len, _p(fs_new), _p(on), _p(t["down4"]), _p(t["down2"]), t["kd4"],
+                                            t["wd4"], t["kd2"], t["wd2"], _p(t["up4"]), _p(t["up2"]), t["ku"], t["wu"], _p(tmp), _stream()))
+
+
+def sim_clip(x, offs, rows, max_len, q, on, stats):
+    _lib.check(_lib.load().qb_sim_clip(_p(x), _p(offs), rows, max_len, _p(q), _p(on), _p(stats), _stream()))
+
+
+def sim_packet_loss(x, offs, lost, lost_row, packet):
+    _lib.check(_lib.load().qb_sim_packet_loss(_p(x), _p(offs), _p(lost), _p(lost_row), lost.numel(), packet, _stream()))
+
+
+def sim_finish(noisy, speech, interf, offs, rows, has_interf, cut_off, norm_r, cut, out_mix, out_speech, out_interf=None):
+    _lib.check(_lib.load().qb_sim_finish(_p(noisy), _p(speech), _p(interf), _p(offs), rows, _p(has_interf), _p(cut_off), _p(norm_r), cut,
+                                         _p(out_mix), _p(out_speech), _p(out_interf), _stream()))
+
+
+def sim_enroll(e, offs, rows, cut_off, cut, out):
+    _lib.check(_lib.load().qb_sim_enroll(_p(e), _p(offs), rows, _p(cut_off), cut, _p(out), _stream()))

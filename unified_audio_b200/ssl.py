@@ -102,7 +102,8 @@ def ssl_spec(c: dict) -> Dict[str, tuple]:
 
 
 def resample_kernel(orig: int, new: int, lowpass_filter_width: int = 6, rolloff: float = 0.99):
-    """torchaudio.functional._get_sinc_resample_kernel (sinc_interp_hann) in fp64 -> ([new', k] fp32, width, orig', new')"""
+    """torchaudio.functional._get_sinc_resample_kernel (sinc_interp_hann) in fp64 -> ([new', k] fp32, width, orig', new'), for decimation
+    (orig > new) and interpolation (orig < new) alike: row j of the kernel gives output phase j of each input stride of orig' samples"""
     g = math.gcd(orig, new)
     orig, new = orig // g, new // g
     base = min(orig, new) * rolloff
