@@ -232,30 +232,56 @@ def test_precision_policies_cover_every_gemm_group():
 
 # ----------------------------------------------------------------------------- C ABI
 def test_library_builds_loads_and_exports_every_declared_symbol(lib):
+    """Every prototype of the header resolves in the library and is bound with the header's number of arguments (counted
+    here from the header text, independently of _lib's reader)."""
     import torch
-    launched = lib.qb_launch_count()           # GPU tests earlier in the same session may have launched kernels
-    hdr = open(os.path.join(ROOT, "include", "quark_b200.h")).read()
-    declared = set(re.findall(r"\b(qb_[a-z0-9_]+)\s*\(", hdr))
-    declared -= {"qb_gemm_desc", "qb_rowmap", "qb_half"}
     from unified_audio_b200 import _lib
-    assert declared == set(_lib.SIGNATURES), declared ^ set(_lib.SIGNATURES)
-    for name in declared:
-        assert getattr(lib, name) is not None
+    launched = lib.qb_launch_count()           # GPU tests earlier in the same session may have launched kernels
+    hdr = re.sub(r"/\*.*?\*/", "", open(_lib.HEADER).read(), flags=re.S)
+    arity = {name: 0 if args.strip() in ("", "void") else args.count(",") + 1
+             for name, args in re.findall(r"\b(qb_\w+)\s*\(([^()]*)\)\s*;", hdr)}
+    assert {"qb_gemm", "qb_codec_load", "qb_sim_enroll"} <= set(arity)
+    assert set(arity) == set(_lib.SIGNATURES), set(arity) ^ set(_lib.SIGNATURES)
+    for name, n in arity.items():
+        assert len(getattr(lib, name).argtypes) == n, name
     assert lib.qb_version() >= 100
     assert lib.qb_launch_count() == launched   # resolving and querying the symbols launches nothing
     if not torch.cuda.is_available():
         assert launched == 0                   # nothing computed on a machine without a GPU
 
 
-def test_gemm_desc_struct_layout_matches_header():
-    """ctypes mirror of qb_gemm_desc must have the C layout (LP64): 8-byte fields + two int32 pairs."""
+def test_struct_layouts_match_the_c_compiler(tmp_path):
+    """sizeof, and the offset and size of every field, of the four ctypes structs equal what the host C compiler makes of
+    include/quark_b200.h."""
     import ctypes as C
-    from unified_audio_b200._lib import GemmDesc, RowMap
-    assert C.sizeof(RowMap) == 32
-    assert GemmDesc.taps.offset == 40 and GemmDesc.stride.offset == 44 and GemmDesc.m_per_batch.offset == 48
-    assert GemmDesc.residual.offset == 96 and GemmDesc.act.offset == 128 and GemmDesc.out_f32.offset == 136
-    assert GemmDesc.dilation.offset == 136 + 3 * 32 and GemmDesc.act_param.offset == 136 + 3 * 32 + 8
-    assert GemmDesc.a_cols.offset == 136 + 3 * 32 + 24 and C.sizeof(GemmDesc) == 136 + 3 * 32 + 32
+    import subprocess
+    from unified_audio_b200 import _lib
+    structs = {"qb_rowmap": _lib.RowMap, "qb_gemm_desc": _lib.GemmDesc, "qb_tensor": _lib.Tensor, "qb_codec_cfg": _lib.CodecCfg}
+    lines, want = [], []
+    for cname, S in structs.items():
+        lines.append(f'printf("%zu\\n", sizeof({cname}));')
+        want.append(C.sizeof(S))
+        for f, _ in S._fields_:
+            lines.append(f'printf("%zu %zu\\n", offsetof({cname}, {f}), sizeof((({cname}*)0)->{f}));')
+            want.append(f"{getattr(S, f).offset} {getattr(S, f).size}")
+    src = tmp_path / "layout.c"
+    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "quark_b200.h"\nint main(void) {\n' + "\n".join(lines)
+                   + "\nreturn 0;\n}\n")
+    exe = tmp_path / "layout"
+    subprocess.run(["cc", "-I", os.path.dirname(_lib.HEADER), str(src), "-o", str(exe)], check=True)
+    got = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split("\n")[:-1]
+    assert got == [str(w) for w in want]
+
+
+def test_header_reader_refuses_unknown_types(tmp_path):
+    """A type without a ctypes rule is an error naming the declaration, never a guess; a missing header names its path."""
+    from unified_audio_b200 import _lib
+    hdr = tmp_path / "h.h"
+    hdr.write_text("#include <stdint.h>\nint qb_x(mystery_t v);\n")
+    with pytest.raises(RuntimeError, match="qb_x"):
+        _lib.read_header(str(hdr))
+    with pytest.raises(RuntimeError, match="nowhere.h"):
+        _lib.read_header(str(tmp_path / "nowhere.h"))
 
 
 def test_bench_reference_arm_contract():
