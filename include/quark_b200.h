@@ -337,11 +337,27 @@ int qb_embedding_bwd(const float* dx, const int64_t* ids, int64_t n, int64_t Lt,
  * -> / temperature -> softmax -> inverse-CDF draw over the kept tokens in descending-logit order at
  * u = Philox4x32-10(key = {seed[0], seed[1]}, counter = {step (= slot[0]), row, seed[2], 0}).x >> 8) * 2^-24.
  * seed: device uint32[4] {seed_lo, seed_hi, call_counter, 0}; debug: optional device float [B][4] = {u, survivors after
- * top-k, kept after top-p, sum of the kept exp((l - max)/T)} or NULL.  1 <= top_k <= 1024; 0 < temperature <= 1. */
+ * top-k, kept after top-p, sum of the kept exp((l - max)/T)} or NULL.  0 < temperature <= 1.
+ * top_k <= 0 applies no top-k filter and top_k >= the range width keeps every token of the range (llm.py:262 runs torch.topk on
+ * the range-masked row); top_p >= 1 applies no top-p filter.  1 <= top_k <= 1024 runs a kernel that stores the survivors above
+ * the k-th value and walks them on one thread; any other top_k runs one that stores and sorts every survivor (up to the whole
+ * range, max_cols <= 8192: row keys + 8 bytes per survivor slot, 96 KB of shared memory at 8192) and makes the top-p cut, the
+ * normaliser and the draw fixed-order block-wide scans.  Both are deterministic (no floating-point atomics).  The scans sum in
+ * another order than the reference's sequential torch.cumsum, so a token whose cumulative probability lies within ~1e-6 of
+ * top_p (or of the draw's target) can fall on the other side of the boundary. */
 int qb_lm_head_sample_tc(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
                          int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride,
                          int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx, float* logits,
                          float temperature, int32_t top_k, float top_p, const uint32_t* seed, float* debug, void* stream);
+/* qb_lm_head_sample_tc with one random stream per row: row_keys is device uint32[B][2] = {key_lo, key_hi} per row, and row b's
+ * uniform at step s (= slot[0]) is (Philox4x32-10(key = row_keys[b], counter = {s, 0, 0, 0}).x >> 8) * 2^-24, a function of
+ * its key and the step only (not of b, the batch size or the call), so a row draws the same tokens in any batch.  A row keyed
+ * k draws what row 0 of call 0 draws from qb_lm_head_sample_tc with seed k. */
+int qb_lm_head_sample_rows_tc(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
+                              int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride,
+                              int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx, float* logits,
+                              float temperature, int32_t top_k, float top_p, const uint32_t* row_keys, float* debug,
+                              void* stream);
 
 /* ---------------------------------------------------------------- SSL feature front ends + tokenizer glue (SURVEY 8f.2 / 8f.3)
  * HuBERT-base / WavLM-base-plus (transformers modeling_hubert / modeling_wavlm) as the reference drives them from

@@ -381,7 +381,12 @@ __global__ void lm_loss_reduce_kernel(const float* __restrict__ row_loss, const 
 // draw.  torch.multinomial's generator cannot be reproduced bit for bit, so the draw is defined here as the inverse CDF
 // over the kept tokens in descending-logit order (ties: ascending id) at u = Philox4x32-10(key = seed, counter =
 // {step, row, call, 0}).x * 2^-32 truncated to 24 bits: same distribution, replayable from (seed, call, step, row).
-constexpr int LS_MAX = 1024;             // survivors above the threshold kept (< top_k); top_k <= LS_MAX enforced by the host
+// With per-row keys (row_keys != NULL) row b's uniform is Philox4x32-10(key = row_keys[b], counter = {step, 0, 0, 0}): a
+// function of its key and the step only, so a row draws the same tokens wherever it sits in whichever batch.
+// Two kernels: lm_sample_embed for 1 <= top_k <= LS_MAX (the survivors above the k-th value fit LS_MAX slots, one thread
+// walks them), lm_sample_full_embed for top_k = 0 (no filter) or above LS_MAX, up to the whole range: every survivor is
+// stored and sorted, and the top-p cut, the normaliser and the inverse-CDF search are fixed-order block-wide scans.
+constexpr int LS_MAX = 1024;             // survivors above the threshold kept (< top_k) by lm_sample_embed_kernel
 __device__ __forceinline__ uint32_t ls_key(float v) {     // monotone float -> uint32 (NaN sorts lowest)
   if (v != v) return 0u;
   const uint32_t u = __float_as_uint(v);
@@ -401,12 +406,52 @@ __device__ __forceinline__ uint32_t philox_u32(uint32_t k0, uint32_t k1, uint32_
   }
   return c0;
 }
+__device__ __forceinline__ float ls_uniform(const unsigned* seed, const unsigned* row_keys, int step, int b) {
+  const uint32_t r = row_keys ? philox_u32(row_keys[2 * b], row_keys[2 * b + 1], (uint32_t)step, 0u, 0u, 0u)
+                              : philox_u32(seed[0], seed[1], (uint32_t)step, (uint32_t)b, seed[2], 0u);
+  return (float)(r >> 8) * (1.0f / 16777216.0f);
+}
+
+// The need-th largest of keys[0..n) (1 <= need <= n) by radix select, one byte per pass from the top, with NT threads; the
+// caller has stored keys and synchronised.  Returns the key; n_gt = the keys strictly above it, n_eq = the keys equal to it.
+template <int NT>
+__device__ __forceinline__ uint32_t ls_radix_select(const uint32_t* keys, int n, int need, int* hist, int& n_gt, int& n_eq) {
+  __shared__ uint32_t s_prefix;
+  __shared__ int s_need, s_eq;
+  const int tid = threadIdx.x;
+  if (tid == 0) { s_prefix = 0u; s_need = need; }
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int i = tid; i < 256; i += NT) hist[i] = 0;
+    __syncthreads();
+    const uint32_t prefix = s_prefix, himask = shift == 24 ? 0u : (0xFFFFFFFFu << (shift + 8));
+    for (int i = tid; i < n; i += NT) {
+      const uint32_t k = keys[i];
+      if ((k & himask) == prefix) atomicAdd(&hist[(k >> shift) & 255], 1);
+    }
+    __syncthreads();
+    if (tid == 0) {
+      int nd = s_need, bin = 255;
+      for (; bin > 0; --bin) {
+        if (hist[bin] >= nd) break;
+        nd -= hist[bin];
+      }
+      s_need = nd;
+      s_prefix = prefix | ((uint32_t)bin << shift);
+      if (shift == 0) s_eq = hist[bin];          // keys equal to the threshold
+    }
+    __syncthreads();
+  }
+  n_gt = need - s_need;
+  n_eq = s_eq;
+  return s_prefix;
+}
 
 __global__ void __launch_bounds__(256)
 lm_sample_embed_kernel(const float* __restrict__ logits, int ld, const int* __restrict__ range, int B, float inv_temp,
                        int top_k, float top_p, const unsigned* __restrict__ seed /* {seed_lo, seed_hi, call, 0} */,
-                       const float* __restrict__ emb, int Hd, float* __restrict__ x_next, int64_t* __restrict__ out_ids,
-                       int out_stride, int* __restrict__ pos, int* __restrict__ slot, float* __restrict__ dbg) {
+                       const unsigned* __restrict__ row_keys /* [B][2] or NULL */, const float* __restrict__ emb, int Hd,
+                       float* __restrict__ x_next, int64_t* __restrict__ out_ids, int out_stride, int* __restrict__ pos,
+                       int* __restrict__ slot, float* __restrict__ dbg) {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
   extern __shared__ uint32_t ls_smem[];
@@ -415,38 +460,16 @@ lm_sample_embed_kernel(const float* __restrict__ logits, int ld, const int* __re
   uint32_t* skey = keys + ((n + 3) & ~3);         // [LS_MAX] survivors: key
   int* sidx = (int*)(skey + LS_MAX);              // [LS_MAX] survivors: column
   __shared__ int hist[256];
-  __shared__ uint32_t sh_prefix;
-  __shared__ int sh_need, sh_eq, sh_cnt, sh_tok, sh_rank;
+  __shared__ int sh_cnt, sh_tok, sh_rank;
   for (int i = tid; i < n; i += 256) keys[i] = ls_key(logits[(size_t)b * ld + i]);
-  if (tid == 0) { sh_prefix = 0u; sh_need = top_k < n ? top_k : n; sh_cnt = 0; }
+  if (tid == 0) sh_cnt = 0;
   __syncthreads();
-  // ---- radix select of the top_k-th largest key, one byte per pass from the top
-  for (int shift = 24; shift >= 0; shift -= 8) {
-    hist[tid] = 0;
-    __syncthreads();
-    const uint32_t prefix = sh_prefix, himask = shift == 24 ? 0u : (0xFFFFFFFFu << (shift + 8));
-    for (int i = tid; i < n; i += 256) {
-      const uint32_t k = keys[i];
-      if ((k & himask) == prefix) atomicAdd(&hist[(k >> shift) & 255], 1);
-    }
-    __syncthreads();
-    if (tid == 0) {
-      int need = sh_need, bin = 255;
-      for (; bin > 0; --bin) {
-        if (hist[bin] >= need) break;
-        need -= hist[bin];
-      }
-      sh_need = need;
-      sh_prefix = prefix | ((uint32_t)bin << shift);
-      if (shift == 0) sh_eq = hist[bin];          // keys equal to the threshold
-    }
-    __syncthreads();
-  }
-  const uint32_t thr = sh_prefix;
+  // ---- radix select of the top_k-th largest key
+  int n_gt, n_eq;
+  const uint32_t thr = ls_radix_select<256>(keys, n, top_k < n ? top_k : n, hist, n_gt, n_eq);
   // ---- survivors: every key >= threshold (ties at the k-th value stay, llm.py:263-264).  Those strictly above it (at most
   // top_k - 1) are collected and bitonic-sorted descending; the n_eq tied ones, however many, share one value and follow them
   // in ascending column order, so they are counted rather than stored.
-  const int n_gt = (top_k < n ? top_k : n) - sh_need, n_eq = sh_eq;
   for (int i = tid; i < n; i += 256) {
     const uint32_t k = keys[i];
     if (k > thr) {
@@ -504,8 +527,7 @@ lm_sample_embed_kernel(const float* __restrict__ logits, int ld, const int* __re
     float S = 0.f;
     for (int i = 0; i < k_gt; ++i) S += expf((ls_val(skey[i]) - m) * inv_temp);
     S += (float)k_eq * et;
-    const uint32_t r = philox_u32(seed[0], seed[1], (uint32_t)*slot, (uint32_t)b, seed[2], 0u);
-    const float u = (float)(r >> 8) * (1.0f / 16777216.0f);
+    const float u = ls_uniform(seed, row_keys, *slot, b);
     const float target = u * S;
     float run = 0.f;
     int pick = -1;
@@ -547,6 +569,137 @@ lm_sample_embed_kernel(const float* __restrict__ logits, int ld, const int* __re
   const int tok = sh_tok;
   if (tid == 0) { out_ids[(size_t)b * out_stride + *slot] = (int64_t)tok; pos[b] += 1; }
   for (int k = tid; k < Hd; k += 256) x_next[(size_t)b * Hd + k] = emb[(size_t)tok * Hd + k];
+  __syncthreads();
+  if (tid == 0) {
+    __threadfence();
+    const int done = atomicAdd(slot + 1, 1);
+    if (done == B - 1) { slot[1] = 0; *slot += 1; }
+  }
+}
+
+// Fixed-order scan over w[0..n) by LSF_NT threads, thread t owning the contiguous slice [i0, i1): per-slice sums, a warp scan of
+// them, a scan of the warp totals.  Returns the sum of the slices before this thread's; total = the sum of all of them.
+constexpr int LSF_NT = 1024;
+__device__ __forceinline__ float lsf_scan(const float* w, int i0, int i1, float* red /* [32] */, float& total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float s = 0.f;
+  for (int i = i0; i < i1; ++i) s += w[i];
+  float inc = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float y = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += y;
+  }
+  float ex = __shfl_up_sync(0xffffffffu, inc, 1);
+  if (lane == 0) ex = 0.f;
+  __syncthreads();                                  // red may still be read by the previous scan
+  if (lane == 31) red[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    float v = red[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const float y = __shfl_up_sync(0xffffffffu, v, o);
+      if (lane >= o) v += y;
+    }
+    red[lane] = v;
+  }
+  __syncthreads();
+  total = red[31];
+  return (warp > 0 ? red[warp - 1] : 0.f) + ex;
+}
+
+// The index of the first element whose running sum (the scan above, then this slice in order) exceeds `limit`, or n if none.
+__device__ __forceinline__ int lsf_first_above(const float* w, int n, int per, float limit, float* red, int* first) {
+  const int i0 = min(n, (int)threadIdx.x * per), i1 = min(n, i0 + per);
+  if (threadIdx.x == 0) *first = n;
+  float total;
+  float run = lsf_scan(w, i0, i1, red, total);
+  for (int i = i0; i < i1; ++i) {
+    run += w[i];
+    if (run > limit) { atomicMin(first, i); break; }
+  }
+  __syncthreads();
+  return *first;
+}
+
+__global__ void __launch_bounds__(LSF_NT, 1)
+lm_sample_full_embed_kernel(const float* __restrict__ logits, int ld, const int* __restrict__ range, int B, float inv_temp,
+                            int top_k, float top_p, const unsigned* __restrict__ seed, const unsigned* __restrict__ row_keys,
+                            const float* __restrict__ emb, int Hd, float* __restrict__ x_next, int64_t* __restrict__ out_ids,
+                            int out_stride, int* __restrict__ pos, int* __restrict__ slot, float* __restrict__ dbg) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  extern __shared__ uint32_t ls_smem[];
+  const int lo = range[0], n = range[1] - lo, b = blockIdx.x, tid = threadIdx.x;
+  int cap = 1;
+  while (cap < ld) cap <<= 1;
+  uint32_t* keys = ls_smem;                       // [ld] keys of the row; after the sort, float scratch
+  uint32_t* skey = keys + ((ld + 3) & ~3);        // [cap] survivors: key
+  int* sidx = (int*)(skey + cap);                 // [cap] survivors: column
+  float* w = reinterpret_cast<float*>(keys);
+  __shared__ int hist[256];
+  __shared__ float red[32];
+  __shared__ int sh_cnt, sh_first;
+  for (int i = tid; i < n; i += LSF_NT) keys[i] = ls_key(logits[(size_t)b * ld + i]);
+  if (tid == 0) sh_cnt = 0;
+  __syncthreads();
+  // ---- top-k threshold (top_k <= 0 or >= n: every key, the radix select then returns the smallest), every survivor stored
+  int n_gt, n_eq;
+  const uint32_t thr = ls_radix_select<LSF_NT>(keys, n, top_k >= 1 && top_k < n ? top_k : n, hist, n_gt, n_eq);
+  const int cnt = n_gt + n_eq;
+  for (int i = tid; i < n; i += LSF_NT) {
+    const uint32_t k = keys[i];
+    if (k >= thr) {
+      const int s = atomicAdd(&sh_cnt, 1);
+      skey[s] = k; sidx[s] = i;
+    }
+  }
+  int P = 1;
+  while (P < cnt) P <<= 1;
+  for (int i = cnt + tid; i < P; i += LSF_NT) { skey[i] = 0u; sidx[i] = 0x7fffffff; }
+  __syncthreads();
+  // ---- bitonic sort, descending by key, ascending by column on ties: a total order, so the atomic slots above do not matter
+  for (int k2 = 2; k2 <= P; k2 <<= 1)
+    for (int j = k2 >> 1; j > 0; j >>= 1) {
+      for (int q = tid; q < (P >> 1); q += LSF_NT) {
+        const int i = ((q & ~(j - 1)) << 1) | (q & (j - 1)), l = i + j;
+        const uint32_t ka = skey[i], kb = skey[l];
+        const int ia = sidx[i], ib = sidx[l];
+        const bool a_first = ka > kb || (ka == kb && ia < ib);
+        const bool up = (i & k2) == 0;
+        if (up != a_first) { skey[i] = kb; skey[l] = ka; sidx[i] = ib; sidx[l] = ia; }
+      }
+      __syncthreads();
+    }
+  // ---- top-p: a token goes once the softmax mass of the tokens before it exceeds top_p (the first always stays)
+  const float m = ls_val(skey[0]);
+  const int per = (cnt + LSF_NT - 1) / LSF_NT, i0 = min(cnt, tid * per), i1 = min(cnt, i0 + per);
+  int nk = cnt;
+  if (top_p < 1.0f) {
+    for (int i = i0; i < i1; ++i) w[i] = expf(ls_val(skey[i]) - m);
+    float Z;
+    lsf_scan(w, i0, i1, red, Z);
+    for (int i = i0; i < i1; ++i) w[i] = w[i] / Z;        // each thread rescales the slice it summed
+    const int f = lsf_first_above(w, cnt, per, top_p, red, &sh_first);
+    nk = f < cnt ? f + 1 : cnt;
+  }
+  // ---- temperature, normaliser, inverse-CDF draw over the nk kept tokens
+  const int per_k = (nk + LSF_NT - 1) / LSF_NT, j0 = min(nk, tid * per_k), j1 = min(nk, j0 + per_k);
+  __syncthreads();                                        // every thread is past its reads of w
+  for (int i = j0; i < j1; ++i) w[i] = expf((ls_val(skey[i]) - m) * inv_temp);
+  float S;
+  lsf_scan(w, j0, j1, red, S);
+  const float u = ls_uniform(seed, row_keys, *slot, b);
+  int pick = lsf_first_above(w, nk, per_k, u * S, red, &sh_first);
+  if (pick >= nk) pick = nk - 1;
+  const int tok = m != m ? lo : lo + sidx[pick];          // all-NaN row: first column of the range (see arg-max kernel)
+  if (tid == 0) {
+    if (dbg) { dbg[b * 4 + 0] = u; dbg[b * 4 + 1] = (float)cnt; dbg[b * 4 + 2] = (float)nk; dbg[b * 4 + 3] = S; }
+    out_ids[(size_t)b * out_stride + *slot] = (int64_t)tok;
+    pos[b] += 1;
+  }
+  for (int k = tid; k < Hd; k += LSF_NT) x_next[(size_t)b * Hd + k] = emb[(size_t)tok * Hd + k];
   __syncthreads();
   if (tid == 0) {
     __threadfence();
@@ -976,28 +1129,60 @@ extern "C" int qb_lm_head_argmax_tc(const float* x, int64_t B, int32_t hidden, c
 }
 
 // Sampled decoding step: as qb_lm_head_argmax_tc, but the head writes the full range logits [B][max_cols] and the token is
-// drawn by lm_sample_embed_kernel (top-k -> top-p -> temperature -> multinomial, llm.py:253-289).
+// drawn by lm_sample_embed_kernel (1 <= top_k <= LS_MAX) or lm_sample_full_embed_kernel (any other top_k) (top-k -> top-p ->
+// temperature -> multinomial, llm.py:253-289).  Exactly one of seed (one stream for the call) and row_keys (one per row).
+static int head_sample(const char* name, const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
+                       int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids, int32_t out_stride, int32_t* pos,
+                       int32_t* slot, float* part_val, int32_t* part_idx, float* logits, float temperature, int32_t top_k,
+                       float top_p, const uint32_t* seed, const uint32_t* row_keys, float* debug, cudaStream_t st) {
+  QB_REQUIRE(B >= 1 && B <= 32 && max_cols % 16 == 0, "%s: bad args (max_cols must be a multiple of 16)", name);
+  QB_REQUIRE(logits && (seed || row_keys), "%s: logits / seed buffers required", name);
+  QB_REQUIRE(temperature > 0.f && temperature <= 1.0f, "%s: temperature must be in (0, 1] (llm.py:278)", name);
+  SkParams p = {};
+  p.B = (int)B; p.eps = 1e-6f; p.x = x; p.K = hidden; p.W = (const uint4*)w_head; p.range = range;
+  p.part_val = part_val; p.part_idx = part_idx; p.logits = logits; p.logits_ld = max_cols;
+  if (int e = launch_skinny<SK_HEAD>(p, max_cols / 16, st)) return e;
+  const size_t smem_cap = 160 * 1024;
+  if (top_k >= 1 && top_k <= LS_MAX) {
+    const size_t smem = ((size_t)((max_cols + 3) & ~3) + 2 * LS_MAX) * 4;
+    QB_CHECK_CUDA(cudaFuncSetAttribute(lm_sample_embed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap));   // per-device state: set on every launch (cheap)
+    QB_REQUIRE(smem <= smem_cap, "%s: range too wide (%d columns)", name, max_cols);
+    QB_CHECK_CUDA(launch_pdl(lm_sample_embed_kernel, dim3((unsigned)B), dim3(256), smem, st, (const float*)logits, (int)max_cols,
+                             (const int*)range, (int)B, 1.0f / temperature, (int)top_k, top_p, (const unsigned*)seed,
+                             (const unsigned*)row_keys, embedding, (int)hidden, x_next, out_ids, (int)out_stride, (int*)pos, (int*)slot,
+                             debug));
+    return 0;
+  }
+  size_t cap = 1;
+  while (cap < (size_t)max_cols) cap <<= 1;
+  const size_t smem = ((size_t)((max_cols + 3) & ~3) + 2 * cap) * 4;      // row keys + every column as a survivor (key, id)
+  QB_CHECK_CUDA(cudaFuncSetAttribute(lm_sample_full_embed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap));
+  QB_REQUIRE(smem <= smem_cap, "%s: range too wide for top_k = %d (%d columns)", name, (int)top_k, max_cols);
+  QB_CHECK_CUDA(launch_pdl(lm_sample_full_embed_kernel, dim3((unsigned)B), dim3(LSF_NT), smem, st, (const float*)logits,
+                           (int)max_cols, (const int*)range, (int)B, 1.0f / temperature, (int)top_k, top_p, (const unsigned*)seed,
+                           (const unsigned*)row_keys, embedding, (int)hidden, x_next, out_ids, (int)out_stride, (int*)pos, (int*)slot,
+                           debug));
+  return 0;
+}
+
 extern "C" int qb_lm_head_sample_tc(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
                                     int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids,
                                     int32_t out_stride, int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx,
                                     float* logits, float temperature, int32_t top_k, float top_p, const uint32_t* seed,
                                     float* debug, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  QB_REQUIRE(B >= 1 && B <= 32 && max_cols % 16 == 0, "lm_head_sample_tc: bad args (max_cols must be a multiple of 16)");
-  QB_REQUIRE(logits && seed, "lm_head_sample_tc: logits / seed buffers required");
-  QB_REQUIRE(temperature > 0.f && temperature <= 1.0f, "lm_head_sample_tc: temperature must be in (0, 1] (llm.py:278)");
-  QB_REQUIRE(top_k >= 1 && top_k <= LS_MAX, "lm_head_sample_tc: top_k must be in 1..%d (got %d)", LS_MAX, top_k);
-  SkParams p = {};
-  p.B = (int)B; p.eps = 1e-6f; p.x = x; p.K = hidden; p.W = (const uint4*)w_head; p.range = range;
-  p.part_val = part_val; p.part_idx = part_idx; p.logits = logits; p.logits_ld = max_cols;
-  if (int e = launch_skinny<SK_HEAD>(p, max_cols / 16, st)) return e;
-  const size_t smem = ((size_t)((max_cols + 3) & ~3) + 2 * LS_MAX) * 4;
-    QB_CHECK_CUDA(cudaFuncSetAttribute(lm_sample_embed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));   // per-device state: set on every launch (cheap)
-  QB_REQUIRE(smem <= 160 * 1024, "lm_head_sample_tc: range too wide (%d columns)", max_cols);
-  QB_CHECK_CUDA(launch_pdl(lm_sample_embed_kernel, dim3((unsigned)B), dim3(256), smem, st, (const float*)logits, (int)max_cols,
-                           (const int*)range, (int)B, 1.0f / temperature, (int)top_k, top_p, (const unsigned*)seed, embedding,
-                           (int)hidden, x_next, out_ids, (int)out_stride, (int*)pos, (int*)slot, debug));
-  return 0;
+  QB_REQUIRE(seed, "lm_head_sample_tc: seed buffer required");
+  return head_sample("lm_head_sample_tc", x, B, hidden, w_head, range, max_cols, embedding, x_next, out_ids, out_stride, pos, slot,
+                     part_val, part_idx, logits, temperature, top_k, top_p, seed, nullptr, debug, (cudaStream_t)stream);
+}
+
+extern "C" int qb_lm_head_sample_rows_tc(const float* x, int64_t B, int32_t hidden, const qb_half* w_head, const int32_t* range,
+                                         int32_t max_cols, const float* embedding, float* x_next, int64_t* out_ids,
+                                         int32_t out_stride, int32_t* pos, int32_t* slot, float* part_val, int32_t* part_idx,
+                                         float* logits, float temperature, int32_t top_k, float top_p, const uint32_t* row_keys,
+                                         float* debug, void* stream) {
+  QB_REQUIRE(row_keys, "lm_head_sample_rows_tc: row_keys buffer required");
+  return head_sample("lm_head_sample_rows_tc", x, B, hidden, w_head, range, max_cols, embedding, x_next, out_ids, out_stride, pos,
+                     slot, part_val, part_idx, logits, temperature, top_k, top_p, nullptr, row_keys, debug, (cudaStream_t)stream);
 }
 
 extern "C" int qb_lm_loss(const float* logits, int64_t ld, int64_t M, int32_t V, const int64_t* targets, float label_smoothing,

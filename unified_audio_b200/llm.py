@@ -17,6 +17,7 @@ setting U/model/model.py:173) or sampled on the device.  No PyTorch / CPU fallba
 from __future__ import annotations
 
 import copy
+import operator
 from dataclasses import dataclass
 import os
 from typing import Optional
@@ -549,11 +550,22 @@ class LLM_SFT(_Face):
     @torch.no_grad()
     def generate(self, task_name, enroll_mel, enroll_feats, mix_mel, mix_feats, global_length: int = 32,
                  temperature: float = 0.8, top_k: int = 50, top_p: float = 0.95, do_sample: bool = True,
-                 use_cuda_graph: bool = True, seed: Optional[int] = None, enroll_lengths=None):
+                 use_cuda_graph: bool = True, seed: Optional[int] = None, enroll_lengths=None, row_seeds=None):
         """llm_sft.py:93-195 with the reference's signature and defaults.  do_sample=True draws every token on the device
-        (top-k -> top-p -> temperature -> multinomial, csrc/llm.cu lm_sample_embed_kernel); `seed` (default: torch's
-        global generator) makes the draw reproducible.  Greedy decoding ignores temperature / top_k / top_p exactly as the
-        reference's arg-max does (filters never remove the arg-max, llm.py:263-287).
+        (top-k -> top-p -> temperature -> multinomial, csrc/llm.cu lm_sample_embed_kernel / lm_sample_full_embed_kernel); `seed`
+        (default: torch's global generator) makes the draw reproducible.  Greedy decoding ignores temperature / top_k / top_p /
+        seed / row_seeds exactly as the reference's arg-max does (filters never remove the arg-max, llm.py:263-287).
+
+        top_k takes what the reference's `torch.topk` over the range-masked vocabulary row takes: 0 (or below) applies no top-k
+        filter, any k up to the vocabulary size (12 291 at the shipped widths) is valid, and a k at or above the range width
+        (4096 global / 8192 semantic tokens) keeps every token of the range; a k above the vocabulary raises as torch.topk does
+        (except k <= 1024, which a reduced-width model keeps accepting as it always has).
+        top_p >= 1 applies no top-p filter.
+
+        `row_seeds` (ints [B], tensor or sequence; not together with `seed`): one 64-bit key per row.  Row b's uniforms are then a
+        function of row_seeds[b] and the decode step only, so its tokens do not depend on its place in the batch, the chunk of 32
+        it falls in, the lane or the batch size: a row draws the same tokens in any batch, and alone.  With `seed` the stream is
+        one per call, and a row's uniforms depend on its row and chunk.
 
         `enroll_lengths` (ints [B], tensor or sequence): the valid frames of each row of a right-padded enroll_feats [B, Te_max, F],
         for rows whose enrollments differ in length.  Row b then decodes exactly as if it were generated alone with
@@ -562,15 +574,20 @@ class LLM_SFT(_Face):
         decode writes position P_b + s before it reads it, so the tail is never read.  None keeps the uniform path."""
         if enroll_lengths is not None:
             enroll_lengths = self._check_enroll_lengths(enroll_lengths, enroll_mel, enroll_feats, mix_feats.shape[0])
+        if row_seeds is not None:
+            row_seeds = self._check_row_seeds(row_seeds, seed, mix_feats.shape[0])
         sampling = None
         if do_sample:
             if not (0.0 < temperature <= 1.0):
                 raise AssertionError("0 < temperature <= 1.0 (llm.py:278)")
-            if top_k <= 0 or top_k > 1024:
-                raise NotImplementedError("native sampling supports 1 <= top_k <= 1024 (reference default 50)")
-            if seed is None:
-                seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-            sampling = dict(temperature=float(temperature), top_k=int(top_k), top_p=float(top_p), seed=int(seed))
+            if top_k > max(self.vocab_size, 1024):     # 1..1024 were accepted at every width before the full-range sampler
+                raise RuntimeError(f"top_k = {top_k} is out of range for the vocabulary of {self.vocab_size} tokens "
+                                   "(torch.topk, llm.py:262)")
+            sampling = dict(temperature=float(temperature), top_k=max(0, int(top_k)), top_p=float(top_p))
+            if row_seeds is not None:
+                sampling["row_keys"] = ops.row_keys_words(row_seeds)
+            else:
+                sampling["seed"] = int(torch.randint(0, 2 ** 62, (1,)).item()) if seed is None else int(seed)
         semantic_length = mix_mel.size(1)
         Ball = mix_feats.shape[0]
         starts = list(range(0, Ball, self.chunk))         # decode kernels keep <= 32 sequences' rows in registers
@@ -582,6 +599,7 @@ class LLM_SFT(_Face):
                 sl = slice(b0, min(b0 + self.chunk, Ball))
                 if sampling is not None:
                     sampling["call"] = ci
+                    sampling["rows"] = sl
                 outs.append(self._generate_chunk(task_name, None if enroll_mel is None else enroll_feats[sl], mix_feats[sl],
                                                  semantic_length, global_length, use_cuda_graph, sampling, lens(sl)))
         else:
@@ -596,6 +614,7 @@ class LLM_SFT(_Face):
                 view, stream = views[ci % n_lanes]
                 if sampling is not None:
                     sampling["call"] = ci
+                    sampling["rows"] = sl
                 if ci < n_lanes:
                     stream.wait_event(ready)             # the inputs were produced on the caller's stream
                 with torch.cuda.stream(stream):
@@ -618,6 +637,22 @@ class LLM_SFT(_Face):
         if len(lens) != B or any(n < 1 or n > te_max for n in lens):
             raise ValueError(f"enroll_lengths must hold {B} lengths in 1..{te_max} (the padded enrollment), got {lens}")
         return lens
+
+    @staticmethod
+    def _check_row_seeds(row_seeds, seed, B):
+        """-> host list of B ints (one 64-bit key per row)"""
+        if seed is not None:
+            raise ValueError("give either `seed` (one random stream per call) or `row_seeds` (one per row), not both")
+        if torch.is_tensor(row_seeds) and (row_seeds.is_floating_point() or row_seeds.is_complex()):
+            raise ValueError(f"row_seeds must be integers, got a {row_seeds.dtype} tensor")
+        keys = row_seeds.reshape(-1).tolist() if torch.is_tensor(row_seeds) else list(row_seeds)
+        try:
+            keys = [operator.index(k) for k in keys]
+        except TypeError:
+            raise ValueError(f"row_seeds must be integers, got {keys}") from None
+        if len(keys) != B:
+            raise ValueError(f"row_seeds must hold {B} keys, one per row, got {len(keys)}")
+        return keys
 
     def _lanes(self, n: int, n_positions: int):
         """Lane = (shallow view of this module with its own workspace, decode state and captured graphs; its own stream).  The
@@ -650,7 +685,7 @@ class LLM_SFT(_Face):
         self._ensure_rope(P + n_steps)
         W = self._w
         max_cols = _pad_to(max(self.global_size, self.semantic_size), 16)     # the head runs 16 columns per CTA
-        samp_key = None if sampling is None else (sampling["temperature"], sampling["top_k"], sampling["top_p"])
+        samp_key = None if sampling is None else (sampling["temperature"], sampling["top_k"], sampling["top_p"], "row_keys" in sampling)
         # Decode state (KV cache, counters, output ids) and the captured graphs are kept per shape: capturing and
         # instantiating ~560 kernel nodes costs the host 10-50 ms, as much as the whole generation takes on the device.
         key = (B, P, n_steps, bool(use_graph), int(self.graph_steps), str(dev), samp_key)
@@ -664,13 +699,16 @@ class LLM_SFT(_Face):
                       pv=torch.zeros(max_cols // 16 + 1, 32, device=dev),
                       pi=torch.zeros(max_cols // 16 + 1, 32, dtype=torch.int32, device=dev), g1=None, gk=None, captured=False,
                       logits=torch.zeros(B, max_cols, device=dev) if sampling is not None else None,
-                      seed=torch.zeros(4, dtype=torch.int32, device=dev), dbg=torch.zeros(B, 4, device=dev))
+                      seed=torch.zeros(4, dtype=torch.int32, device=dev), row_keys=torch.zeros(B, 2, dtype=torch.int32, device=dev),
+                      dbg=torch.zeros(B, 4, device=dev))
             self._gen_state[key] = st
         cache, xs, rng, slot, out_ids, pv, pi = (st[k] for k in ("cache", "xs", "rng", "slot", "out_ids", "pv", "pi"))
         cache.length = 0
         cache.pos.zero_()
         slot.zero_()
-        if sampling is not None:        # Philox key / call counter live in device memory: the captured graph is reused across seeds
+        if sampling is not None and "row_keys" in sampling:       # per-row Philox keys, also in device memory
+            st["row_keys"].copy_(sampling["row_keys"][sampling["rows"]], non_blocking=True)
+        elif sampling is not None:      # Philox key / call counter live in device memory: the captured graph is reused across seeds
             sd_ = sampling["seed"]
             to_i32 = lambda v: v - (1 << 32) if v >= (1 << 31) else v
             st["seed"].copy_(torch.tensor([to_i32(sd_ & 0xFFFFFFFF), to_i32((sd_ >> 32) & 0xFFFFFFFF), sampling["call"], 0],
@@ -688,7 +726,11 @@ class LLM_SFT(_Face):
 
         def step():
             self._decode_layers(xs, B, cache)
-            if sampling is not None:
+            if sampling is not None and "row_keys" in sampling:
+                ops.lm_head_sample_rows_tc(xs, B, H, W["head_p"], rng, max_cols, W["emb"], xs, out_ids, n_steps, cache.pos, slot, pv,
+                                           pi, st["logits"], sampling["temperature"], sampling["top_k"], sampling["top_p"],
+                                           st["row_keys"], st["dbg"])
+            elif sampling is not None:
                 ops.lm_head_sample_tc(xs, B, H, W["head_p"], rng, max_cols, W["emb"], xs, out_ids, n_steps, cache.pos, slot, pv, pi,
                                       st["logits"], sampling["temperature"], sampling["top_k"], sampling["top_p"], st["seed"], st["dbg"])
             else:

@@ -354,6 +354,26 @@ def lm_head_sample_tc(x, B, hidden, w_head_p, rng, max_cols, emb, x_next, out_id
                                                 float(temperature), int(top_k), float(top_p), _p(seed), _p(debug), _stream()))
 
 
+def lm_head_sample_rows_tc(x, B, hidden, w_head_p, rng, max_cols, emb, x_next, out_ids, out_stride, pos, slot, pv, pi, logits,
+                           temperature, top_k, top_p, row_keys, debug=None):
+    """lm_head_sample_tc with one random stream per row: row_keys = contiguous int32 [>= B, 2] device tensor, {lo, hi} 32-bit
+    words of row b's 64-bit key (row_keys_words)"""
+    _check_pos(pos, B)
+    if row_keys.dtype != torch.int32 or row_keys.numel() < 2 * B or not row_keys.is_contiguous():
+        raise ValueError(f"row_keys must be a contiguous int32 tensor of >= {2 * B} elements, got {row_keys.dtype} {tuple(row_keys.shape)}")
+    _lib.check(_lib.load().qb_lm_head_sample_rows_tc(_p(x), B, hidden, _p(w_head_p), _p(rng), max_cols, _p(emb), _p(x_next),
+                                                     _p(out_ids), out_stride, _p(pos), _p(slot), _p(pv), _p(pi), _p(logits),
+                                                     float(temperature), int(top_k), float(top_p), _p(row_keys), _p(debug), _stream()))
+
+
+def row_keys_words(keys) -> torch.Tensor:
+    """64-bit row keys (Python ints, any sign: taken mod 2^64) -> host int32 [n, 2] = {low word, high word} per key, the layout
+    qb_lm_head_sample_rows_tc reads"""
+    to_i32 = lambda v: v - (1 << 32) if v >= (1 << 31) else v
+    words = [(to_i32(k & 0xFFFFFFFF), to_i32((k >> 32) & 0xFFFFFFFF)) for k in (int(k) & 0xFFFFFFFFFFFFFFFF for k in keys)]
+    return torch.tensor(words, dtype=torch.int32).reshape(-1, 2)
+
+
 def ssl_conv0_gn_gelu(x, w, gn_w, gn_b, eps, k, stride, out: Planes, ld, rows_per_batch, row_off, y_scratch, workspace):
     B, T_in = x.shape
     _lib.check(_lib.load().qb_ssl_conv0_gn_gelu(_p(x), B, T_in, _p(w), w.shape[0], k, stride, _p(gn_w), _p(gn_b), float(eps), _p(y_scratch),

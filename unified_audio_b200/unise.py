@@ -36,6 +36,34 @@ SEG_LEN = 5 * 16000                                                            #
 # per shape, and at shipped widths 128 segments per call ran out of an 80 GB H100 (in the BiCodec decoder's buffers); 32 is one LM
 # decode chunk.  Measured peak device memory: README (scripts/unise_enhance_bench.py).
 MAX_SEGMENTS = 32
+# the generate passes of test_step (model.py:174-286): 'se', 'tse', and in 'ss' an 'se' pass followed by 'tse' and 'rtse'
+GENERATE_PASSES = ("se", "tse", "rtse")
+_M64 = (1 << 64) - 1
+
+
+def _mix64(z: int) -> int:
+    """SplitMix64's finaliser (Steele, Lea and Flood 2014): a bijection of 64-bit ints"""
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return z ^ (z >> 31)
+
+
+def segment_key(utterance_seed: int, generate_pass: str, segment: int) -> int:
+    """The 64-bit key of one generate row of a sampled `Model.enhance` / `enhance_batch` (LLM_SFT.generate's `row_seeds`): a pure
+    function of the utterance's seed, the generate pass ('se', 'tse' or 'rtse') and the row's 5 s segment index in that pass,
+        h = mix64((utterance_seed + G) mod 2^64);  then h = mix64(((h XOR x) + G) mod 2^64) for x = the pass index (se 0, tse 1,
+        rtse 2), then for x = the segment,
+    with mix64 SplitMix64's finaliser and G = 0x9E3779B97F4A7C15.  'ss' draws its first pass (one row: the first 5 s) as 'se'
+    segment 0."""
+    if generate_pass not in GENERATE_PASSES:
+        raise ValueError(f"generate_pass must be one of {GENERATE_PASSES}, got {generate_pass!r}")
+    if segment < 0:
+        raise ValueError(f"segment must be >= 0, got {segment}")
+    G = 0x9E3779B97F4A7C15
+    h = _mix64((int(utterance_seed) + G) & _M64)
+    for x in (GENERATE_PASSES.index(generate_pass), int(segment)):
+        h = _mix64(((h ^ x) + G) & _M64)
+    return h
 
 
 class BiCodecTokenizer(nn.Module):
@@ -259,11 +287,18 @@ class Model(nn.Module):
     def _segments(self, src: torch.Tensor) -> torch.Tensor:
         return wrap_segments(src.float().contiguous(), SEG_LEN)          # np.pad(..., 'wrap') + reshape(-1, seg_len) on the device
 
-    def _generate(self, task, enroll_feats, seg_src, do_sample, **gen_kw):
+    def _generate(self, task, enroll_feats, seg_src, do_sample, utterance_seed=None, **gen_kw):
         if enroll_feats is not None:                                    # torch.cat([enroll] * n_segments) (model.py:207-208)
             n = seg_src.size(0)
             enroll_feats = torch.cat([enroll_feats for _ in range(n)], 0)
+        if utterance_seed is not None:
+            gen_kw = dict(gen_kw, row_seeds=[segment_key(utterance_seed, task, i) for i in range(seg_src.size(0))])
         return self._generate_rows(task, enroll_feats, None, seg_src, do_sample, **gen_kw)
+
+    @staticmethod
+    def _check_seed_args(gen_kw, name):
+        if "seed" in gen_kw or "row_seeds" in gen_kw:
+            raise ValueError(f"`{name}` sets generate's random streams: it cannot be combined with `seed` / `row_seeds`")
 
     def _generate_rows(self, task, enroll_feats, enroll_lengths, seg_src, do_sample, **gen_kw):
         """WavLM features of the segments, then generate with one enrollment row per segment (right-padded to the longest when
@@ -285,12 +320,19 @@ class Model(nn.Module):
 
     @torch.no_grad()
     def enhance(self, mode: str, enroll: Optional[torch.Tensor], src: torch.Tensor, do_sample: bool = False, return_ids: bool = False,
-                **gen_kw):
+                utterance_seed: Optional[int] = None, **gen_kw):
         """The body of test_step with tensors in and a device tensor out.  src [1, T] (the reference's test loader yields one
         utterance per batch; like the reference, a batch of several is folded into the segment axis), enroll [1, Te] for 'tse'.
-        'ss' returns (s1, s2)."""
+        'ss' returns (s1, s2).
+
+        `utterance_seed` (with do_sample=True; not together with `seed` / `row_seeds` in gen_kw): every generate row draws from
+        its own stream, keyed `segment_key(utterance_seed, pass, segment)`, so `enhance_batch` with this seed for the utterance
+        returns the same result.  Greedy decoding ignores it."""
         if src.device.type != "cuda":
             raise RuntimeError("unified_audio_b200.unise.Model runs on CUDA only (no CPU fallback)")
+        if utterance_seed is not None:
+            self._check_seed_args(gen_kw, "utterance_seed")
+            gen_kw = dict(gen_kw, utterance_seed=int(utterance_seed))
         return self._enhance(mode, enroll, src, do_sample, return_ids, **gen_kw)
 
     def _enhance(self, mode, enroll, src, do_sample=False, return_ids=False, **gen_kw):
@@ -326,7 +368,7 @@ class Model(nn.Module):
     # ------------------------------------------------------------------ batched inference: many utterances per call
     @torch.no_grad()
     def enhance_batch(self, mode: str, enrolls, srcs, do_sample: bool = False, return_ids: bool = False,
-                      max_segments: int = MAX_SEGMENTS, **gen_kw):
+                      max_segments: int = MAX_SEGMENTS, utterance_seeds=None, **gen_kw):
         """`enhance` over many utterances at once: srcs = list of [1, T_u] device tensors (any lengths), enrolls = list of [1, Te_u]
         ('tse', any lengths) or None.  Returns a list with, for each utterance, what `enhance` returns for it alone.
 
@@ -335,11 +377,15 @@ class Model(nn.Module):
         features are taken alone (WavLM's first GroupNorm spans time: padding would change them) and the LM prefixes differ in length
         (generate's `enroll_lengths`).  Greedy tokens are those of `enhance` when the LM's decode attention keeps the same number of
         keys in flight on both sides (LLM_SFT.att_unroll / lane_att_unroll; lanes only run when generate gets more than 32 rows).
-        With do_sample the draws differ from `enhance`'s: a row's uniforms depend on where it sits in the batch."""
+
+        With do_sample, `utterance_seeds` (one int per utterance) gives every generate row its own random stream, keyed
+        `segment_key(utterance_seeds[u], pass, segment)`: each utterance then gets exactly what `enhance(..., do_sample=True,
+        utterance_seed=utterance_seeds[u])` gives it alone (same condition on the decode attention).  Without it the draws
+        differ from `enhance`'s: with `seed` a row's uniforms depend on where it sits in the batch."""
         srcs = list(srcs) if srcs is not None else []
         if any(t is not None and t.device.type != "cuda" for t in srcs + list(enrolls or [])):
             raise RuntimeError("unified_audio_b200.unise.Model runs on CUDA only (no CPU fallback)")
-        return self._enhance_batch(mode, enrolls, srcs, do_sample, return_ids, max_segments, **gen_kw)
+        return self._enhance_batch(mode, enrolls, srcs, do_sample, return_ids, max_segments, utterance_seeds, **gen_kw)
 
     @staticmethod
     def _check_batch(mode, enrolls, srcs, max_segments):
@@ -361,20 +407,32 @@ class Model(nn.Module):
             raise ValueError(f"max_segments must be >= 1, got {max_segments}")
         return enrolls
 
-    def _enhance_batch(self, mode, enrolls, srcs, do_sample=False, return_ids=False, max_segments=MAX_SEGMENTS, **gen_kw):
+    def _enhance_batch(self, mode, enrolls, srcs, do_sample=False, return_ids=False, max_segments=MAX_SEGMENTS, utterance_seeds=None,
+                       **gen_kw):
         """_enhance's control flow per mode (model.py:174-286), applied per utterance, with the segments of all utterances batched;
         pinned against the reference's `test_step` fixture and against `_enhance` (tests/test_unise_batch_host.py)."""
         enrolls = self._check_batch(mode, enrolls, srcs, max_segments)
+        if utterance_seeds is not None:
+            utterance_seeds = [int(s) for s in utterance_seeds]
+            if len(utterance_seeds) != len(srcs):
+                raise ValueError(f"{len(utterance_seeds)} utterance_seeds for {len(srcs)} utterances")
+            self._check_seed_args(gen_kw, "utterance_seeds")
         lens = [s.size(-1) for s in srcs]
         segs = [self._segments(s) for s in srcs]
         rows = [0]
         for sg in segs:
             rows.append(rows[-1] + sg.size(0))
+
+        def keyed(task, n_rows=None):      # generate's keyword arguments for one pass: row u's segments keyed by its utterance's seed
+            if utterance_seeds is None:
+                return gen_kw
+            n_rows = n_rows or [rows[u + 1] - rows[u] for u in range(len(srcs))]
+            return dict(gen_kw, row_seeds=[segment_key(s, task, i) for s, n in zip(utterance_seeds, n_rows) for i in range(n)])
         cut = lambda x, u: x[rows[u]:rows[u + 1]]
         trim = lambda est, u: cut(est, u).reshape(-1)[:lens[u]]
         if mode == "se":                                                 # model.py:174-193, per utterance its own peak
             seg = torch.cat([sg / s.abs().max(dim=-1, keepdim=True)[0] for sg, s in zip(segs, srcs)], 0)
-            est, gids, sids = self._run_segments("se", None, None, seg, do_sample, max_segments, **gen_kw)
+            est, gids, sids = self._run_segments("se", None, None, seg, do_sample, max_segments, **keyed("se"))
             return [(trim(est, u), cut(gids, u), cut(sids, u)) if return_ids else trim(est, u) for u in range(len(srcs))]
         if mode == "tse":                                                # model.py:197-224
             feats = [self.extract_semantic_features(e) for e in enrolls]          # each enrollment alone
@@ -383,17 +441,17 @@ class Model(nn.Module):
             per_row = [torch.cat([f, pad[:, :max(te) - f.size(1)]], 1) for f in feats]
             ef = torch.cat([per_row[u] for u in range(len(srcs)) for _ in range(rows[u + 1] - rows[u])], 0)
             el = [te[u] for u in range(len(srcs)) for _ in range(rows[u + 1] - rows[u])]
-            est, gids, sids = self._run_segments("tse", ef, el, torch.cat(segs, 0), do_sample, max_segments, **gen_kw)
+            est, gids, sids = self._run_segments("tse", ef, el, torch.cat(segs, 0), do_sample, max_segments, **keyed("tse"))
             return [(trim(est, u), cut(gids, u), cut(sids, u)) if return_ids else trim(est, u) for u in range(len(srcs))]
         # 'ss', model.py:225-286: se on each utterance's first 5 s, then tse and rtse with that as the enrollment
         first = torch.cat([s[:, :SEG_LEN] if n > SEG_LEN else sg[:1] for s, sg, n in zip(srcs, segs, lens)], 0)
-        enr = self._run_segments("se", None, None, first, do_sample, max_segments, **gen_kw)[0][:, :SEG_LEN]
+        enr = self._run_segments("se", None, None, first, do_sample, max_segments, **keyed("se", [1] * len(srcs)))[0][:, :SEG_LEN]
         enr = enr / (torch.amax(torch.abs(enr), dim=-1, keepdim=True) + 1e-5) * 0.99       # each utterance by its own peak
         ef = self.extract_semantic_features(enr)
         ef = torch.cat([ef[u:u + 1] for u in range(len(srcs)) for _ in range(rows[u + 1] - rows[u])], 0)
         seg = torch.cat(segs, 0)
-        est1, _, _ = self._run_segments("tse", ef, None, seg, do_sample, max_segments, **gen_kw)
-        est2, _, _ = self._run_segments("rtse", ef, None, seg, do_sample, max_segments, **gen_kw)
+        est1, _, _ = self._run_segments("tse", ef, None, seg, do_sample, max_segments, **keyed("tse"))
+        est2, _, _ = self._run_segments("rtse", ef, None, seg, do_sample, max_segments, **keyed("rtse"))
         return [(trim(est1, u), trim(est2, u)) for u in range(len(srcs))]
 
     def _run_segments(self, task, enroll_feats, enroll_lengths, seg, do_sample, max_segments, **gen_kw):
@@ -402,8 +460,9 @@ class Model(nn.Module):
         est, gids, sids = [], [], []
         for s0 in range(0, seg.size(0), max_segments):
             sl = slice(s0, s0 + max_segments)
+            kw = gen_kw if "row_seeds" not in gen_kw else dict(gen_kw, row_seeds=gen_kw["row_seeds"][sl])
             g, s = self._generate_rows(task, None if enroll_feats is None else enroll_feats[sl],
-                                       None if enroll_lengths is None else enroll_lengths[sl], seg[sl], do_sample, **gen_kw)
+                                       None if enroll_lengths is None else enroll_lengths[sl], seg[sl], do_sample, **kw)
             est.append(self.tokenizer.detokenize(g.unsqueeze(1), s).squeeze(1))
             gids.append(g)
             sids.append(s)
