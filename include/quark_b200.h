@@ -289,9 +289,10 @@ int qb_lm_loss(const float* logits, int64_t ld, int64_t M, int32_t V, const int6
  * contractions of the backward pass are qb_gemm calls in the 3-term split mode; these entry points are the rest.
  *
  * Attention dropout mask (transformers' Llama attention in train mode: dropout on the softmax output, before P V): key j of query i in
- * head h of batch row b, decoder layer `layer`, is kept iff (r >> 8) >= round(p * 2^24), where r is word (j & 3) of
- * Philox4x32-10(key = {seed & 0xffffffff, seed >> 32}, counter = {i, j >> 2, b * heads + h, layer}); kept probabilities are scaled by
- * 1 / (1 - p).  The mask is a pure function of (seed, layer, b, h, i, j), so the backward pass regenerates it.
+ * head h of batch row b, decoder layer `layer`, is kept iff (r >> 8) >= thr, where r is word (j & 3) of
+ * Philox4x32-10(key = {seed & 0xffffffff, seed >> 32}, counter = {i, j >> 2, b * heads + h, layer}) and thr is the float dropout_p as
+ * received times 2^24, rounded to the nearest integer with ties to even (so a caller's double p counts as (float)p); kept probabilities
+ * are scaled by 1 / (1 - p).  The mask is a pure function of (seed, layer, b, h, i, j), so the backward pass regenerates it.
  *
  * qb_lm_attn_train_fwd: causal attention, head_dim 64, fp32 SIMT.  qkv [B*L, 3*heads*64] fp32 (rope tables as qb_attention_umma)
  * -> qs = RoPE(q) / 8, kr = RoPE(k), v, each [B*heads, L, 64] (kept for the backward pass), out [B*L, heads*64] fp32 and the row
@@ -306,7 +307,9 @@ int qb_lm_attn_train_bwd(const float* qs, const float* kr, const float* v, const
                          uint64_t seed, int32_t layer, float* dqkv, float* workspace, void* stream);
 /* Gradient of qb_lm_loss's loss times *grad_loss (a device float) w.r.t. the logits, times M * scale: *grad_loss * (softmax(logits) - t)
  * * scale with t the smoothed target -> out fp32 and hi / lo planes, all [M, ld_out] (columns V.. zero).  Most entries are ~1/V, below
- * fp16's normal range: a power-of-two scale near V (<= 2^14, so that |out| <= 2^14 |*grad_loss|) keeps the planes fp32-grade.  The caller
+ * fp16's normal range: a power-of-two scale near V (<= 2^14, so that |out| <= 2^14 |*grad_loss|) keeps the planes fp32-grade while
+ * |*grad_loss| * 2^14 stays well inside fp16's range (lo overflows from |out| ~ 2^17, and at |*grad_loss| ~ 2^-16 the ~1/V entries fall
+ * into fp16 subnormals).  LLM_SFT passes a unit *grad_loss and multiplies the finished parameter gradients by the real one.  The caller
  * takes the scale back out (LLM_SFT: the head GEMM's gamma; qb_col_sum / qb_embedding_bwd scale the parameter gradients). */
 int qb_lm_loss_bwd(const float* logits, int64_t ld, int64_t M, int32_t V, const int64_t* targets, float label_smoothing,
                    const float* grad_loss, float scale, float* out, qb_half* out_hi, qb_half* out_lo, int64_t ld_out, void* stream);

@@ -31,19 +31,29 @@ def philox4x32_10_np(key, c0, c1, c2, c3):
     return c0, c1, c2, c3
 
 
-def dropout_keep(seed: int, layer: int, B: int, heads: int, L: int, p: float) -> np.ndarray:
-    """bool [B, heads, L, L]: key j of query i kept iff (word (j & 3) of Philox4x32-10(key = seed lo / hi, counter = {i, j >> 2,
-    b * heads + h, layer}) >> 8) >= round(p * 2^24)"""
-    thr = int(round(p * 2 ** 24))
+def dropout_threshold(p: float) -> int:
+    """the mask's 24-bit threshold: float32(p) * 2^24 (exact in a double) rounded to the nearest integer, ties to even.  The library
+    receives p as a C float, so a Python double that float32 rounds (0.09, 0.058, 0.16, ...) can land one step away from round(p * 2^24)."""
+    return int(np.rint(np.float64(np.float32(p)) * 2.0 ** 24))
+
+
+def dropout_words(seed: int, layer: int, B: int, heads: int, L: int) -> np.ndarray:
+    """uint64 [B, heads, L, L]: the 24-bit word of key j of query i, word (j & 3) of Philox4x32-10(key = seed lo / hi, counter = {i,
+    j >> 2, b * heads + h, layer}) >> 8"""
     J4 = -(-L // 4)
     bh = np.arange(B * heads, dtype=np.uint64)[:, None, None]
     i = np.arange(L, dtype=np.uint64)[None, :, None]
     j4 = np.arange(J4, dtype=np.uint64)[None, None, :]
     shape = (B * heads, L, J4)
     words = philox4x32_10_np((seed & _MASK, (seed >> 32) & _MASK), np.broadcast_to(i, shape), np.broadcast_to(j4, shape),
-                             np.broadcast_to(bh, shape), np.full(shape, layer, dtype=np.uint64))
+                             np.broadcast_to(bh, shape), np.full(shape, layer & _MASK, dtype=np.uint64))
     r = np.stack(words, -1).reshape(B * heads, L, 4 * J4)[..., :L]
-    return ((r >> np.uint64(8)) >= np.uint64(thr)).reshape(B, heads, L, L)
+    return (r >> np.uint64(8)).reshape(B, heads, L, L)
+
+
+def dropout_keep(seed: int, layer: int, B: int, heads: int, L: int, p: float) -> np.ndarray:
+    """bool [B, heads, L, L]: key j of query i kept iff its dropout_words word >= dropout_threshold(p)"""
+    return dropout_words(seed, layer, B, heads, L) >= np.uint64(dropout_threshold(p))
 
 
 def llm_forward(sd, cfg, x, masks=None, p=0.0):

@@ -19,7 +19,8 @@ extern std::atomic<long long> g_launches;
 
 // ------------------------------------------------------------------------------------------ dropout mask
 // keep(seed, layer, b, h, i, j) = (Philox4x32-10(key = {seed_lo, seed_hi}, counter = {i, j >> 2, b * heads + h, layer}).word[j & 3]
-// >> 8) >= thr, thr = round(p * 2^24): one Philox call gives the mask of four consecutive keys (include/quark_b200.h).
+// >> 8) >= thr, thr = (float)p * 2^24 rounded half-to-even (llrint of an exact double): one Philox call gives the mask of four
+// consecutive keys (include/quark_b200.h).
 __device__ __forceinline__ uint4 philox4(uint32_t k0, uint32_t k1, uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3) {
 #pragma unroll
   for (int r = 0; r < 10; ++r) {

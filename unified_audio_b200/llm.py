@@ -461,14 +461,16 @@ class LLM_SFT(_Face):
         # head + loss: dlogits once, as fp32 rows (for dW) and planes (for dX), written times Mt * scale (qb_lm_loss_bwd: its ~1/V
         # entries stay out of fp16's subnormal range).  The head's data-gradient GEMM takes `scale` back out (gamma, a power of two), so
         # the rest of the backward pass runs in units of Mt, where a row's gradients are O(1) in fp16 planes; every parameter gradient
-        # is written times `unscale`.
+        # is written times `unscale`.  The pass runs for a unit loss gradient: grad_loss (a loss weight, 1 / N of an accumulation, a
+        # GradScaler's 2^16) multiplies the finished gradients, so the planes never see it and (c * loss).backward() is c times the
+        # gradient for any c.
         Vp = _pad_to(V, 64)
         scale = ops.lm_loss_scale(V)
         unscale = 1.0 / Mt
         dlog = torch.empty(Mt, Vp, device=dev)
         dlp = Planes(torch.empty(Mt, Vp, dtype=torch.float16, device=dev), torch.empty(Mt, Vp, dtype=torch.float16, device=dev))
         ops.lm_loss_bwd(sv["logits"], sv["logits"].shape[1], Mt, V, run["targets"], self.label_smoothing,
-                        grad_loss.float().contiguous(), dlog, dlp, Vp, scale)
+                        self._cached(("unit_grad", dev), lambda: torch.ones(1, device=dev)), dlog, dlp, Vp, scale)
         g["output_head.weight"] = ops.weight_grad(dlog, sv["hst"], Mt, V, H, torch.empty(V, H, device=dev), dy_ld=Vp,
                                                   scale=unscale / scale)
         dhs = torch.zeros(M, H, device=dev)
@@ -544,6 +546,7 @@ class LLM_SFT(_Face):
         g["adapter.weight"] = ops.weight_grad(da, feats, Nf, H, Fd, torch.empty(H, Fd, device=dev), scale=unscale)
         g["adapter.bias"] = torch.empty(H, device=dev)
         ops.col_sum(da, Nf, H, H, g["adapter.bias"], scale=unscale)
+        torch._foreach_mul_(list(g.values()), grad_loss.float().reshape(()))          # on the device: no host read of grad_loss
         return g
 
     # ------------------------------------------------------------------ generate (llm_sft.py:93-195)
@@ -779,13 +782,16 @@ class LLM_SFT(_Face):
 
 class _LMLoss(torch.autograd.Function):
     """The teacher-forced loss as one autograd node: forward runs the LM keeping the activations its backward needs, backward runs the
-    library's gradient kernels and returns an fp32 gradient for every parameter (None for one the step did not use)."""
+    library's gradient kernels and returns an fp32 gradient for every parameter (None for one the step did not use).  The backward
+    reads the parameters the forward saw (aliases, not copies), so it refuses to run once one of them has been changed in place or
+    replaced since the forward, as torch's own saved-tensor check does."""
 
     @staticmethod
     def forward(ctx, face, run, names, *params):
         prm = {n: p.detach().float().contiguous() for n, p in zip(names, params)}
         loss, acc, logits, saved = face._train_fwd(run, prm)
         ctx.face, ctx.run, ctx.names, ctx.prm, ctx.saved = face, run, names, prm, saved
+        ctx.params, ctx.versions = params, tuple((p._version, p.data_ptr()) for p in params)
         ctx.mark_non_differentiable(acc, logits)
         return loss, acc, logits
 
@@ -793,6 +799,10 @@ class _LMLoss(torch.autograd.Function):
     def backward(ctx, grad_loss, grad_acc, grad_logits):
         if ctx.saved is None:
             raise RuntimeError("LLM_SFT training forward: backward called twice on the same graph")
+        changed = [n for n, p, v in zip(ctx.names, ctx.params, ctx.versions) if (p._version, p.data_ptr()) != v]
+        if changed:
+            raise RuntimeError(f"LLM_SFT training forward: {len(changed)} parameter(s) changed in place between the forward and the "
+                               f"backward (first: {changed[0]}); run the backward before the optimizer step")
         g = ctx.face._train_bwd(ctx.run, ctx.prm, ctx.saved, grad_loss)
-        ctx.saved = ctx.prm = None
+        ctx.saved = ctx.prm = ctx.params = None
         return (None, None, None) + tuple(g.get(n) for n in ctx.names)
