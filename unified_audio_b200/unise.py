@@ -8,6 +8,7 @@ and checkpoint callbacks are out of scope, SURVEY 2):
     .validation_step((mode, enroll, mix, speech, interf, fs, lengths, names))    model.py:134-160, modes 'se' / 'tse' / 'rtse'
     .validation_epoch(batches) -> batch-size-weighted epoch means, across ranks   model.py:160 (log_dict on_epoch, sync_dist)
     .training_step(batch) -> {"loss" (differentiable), "train_acc"}, .configure_optimizers()   model.py:96-124, 327-353
+    .broadcast_parameters(), .sync_gradients()    data-parallel training as train.py:35's DDP strategy averages gradients
     .test_step((mode, enroll, src, tgt, fs, lengths, names), batch_idx)          model.py:170-286, modes 'se' / 'tse' / 'ss'
 and audio_tokenizer.py:30-125 for `BiCodecTokenizer.detokenize(global_tokens, semantic_tokens)` and, given the wav2vec2 front end,
 `BiCodecTokenizer.tokenize(wav) -> (global_tokens, semantic_tokens)`.
@@ -260,6 +261,21 @@ class Model(nn.Module):
 
         sch = {"scheduler": torch.optim.lr_scheduler.LambdaLR(opt, warmup_lambda), "interval": "step", "frequency": 1}
         return [opt], [sch]
+
+    # ------------------------------------------------------------------ data-parallel training (train.py:35, strategy 'ddp')
+    def broadcast_parameters(self, group=None) -> None:
+        """Copy rank 0's LM parameters to every rank of `group` (`parallel.broadcast_parameters`), as DDP does when it wraps the
+        model; the LM repacks its inference weights at its next call.  No-op without torch.distributed or with one rank."""
+        from .parallel import broadcast_parameters
+        broadcast_parameters(self.dnn, group)
+
+    def sync_gradients(self, group=None) -> None:
+        """Average the LM's gradients across the ranks of `group` with one all-reduce (`parallel.average_gradients`): what DDP with
+        find_unused_parameters=True leaves in `.grad`, including `.grad is None` on a parameter no rank used (`enroll_sos_embedding`
+        when every rank ran 'se').  Call it after `loss.backward()` and before clipping; every rank then holds the same gradients,
+        so clipping and the optimizer step keep the ranks' parameters equal.  No-op without torch.distributed or with one rank."""
+        from .parallel import average_gradients
+        average_gradients(self.dnn, group)
 
     def validation_epoch(self, batches, group=None) -> dict:
         """A validation epoch as the reference logs it (`log_dict(..., on_epoch=True, sync_dist=True)`, model.py:160).  Each batch's
