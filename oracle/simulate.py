@@ -7,6 +7,8 @@ TEST INFRASTRUCTURE.  A NumPy / SciPy restatement in two halves:
   apply(p, waves, fp64)   the signal path for those parameters.  fp64=False preserves the reference's dtypes: float32 in, float32
                           through mixing and reverberation, float64 from the clipping stage on (np.quantile returns float64 and
                           np.clip promotes), float32 out as data_iter_fn's `.float()`.  fp64=True runs every stage in float64.
+                          Its last stages are `finish` (peak rule, cut, normalisation) and `enroll`, which the kernel tests call
+                          directly.
 Bandwidth limitation uses torchaudio's sinc_interp_hann resampler (the taps of unified_audio_b200.ssl.resample_kernel, fp32) in
 place of the reference's soxr_hq, which is not available offline (DESIGN.md section 3).
 tests/golden/simulation_small.npz (oracle/make_golden_simulation.py) pins `apply` bit for bit against the reference's own code."""
@@ -268,6 +270,18 @@ def apply(p, speech, noise, rir=None, interf=None, enroll=None, cut=80000, enrol
             noisy = clip(noisy, p["min_q"], p["max_q"])
         else:
             noisy = packet_loss(noisy, p["lost"], fs)
+    noisy, speech, interf = finish(noisy, speech, interf, cut, p["cut_offset"], p["norm_r"])
+    if enroll is not None:
+        enroll = _enroll(enroll, enroll_len, p["enroll_offset"])
+    out = lambda w: None if w is None else w[0].astype(dt)
+    return out(enroll), out(noisy), out(speech), out(interf)
+
+
+def finish(noisy, speech, interf, cut, cut_offset, norm_r):
+    """The peak rule (above 0.99 every signal becomes v / peak * 0.99), pad_or_cut to `cut` samples, then normalize_src_tgt (interf
+    None) or normalize_mix_speech_inferf with the uniform's underlying random() `norm_r` -> (noisy, speech, interf), each [1, cut].
+    In float32 with a Python float norm_r every operation stays in float32 (NEP 50) except 0.1 + (0.99 - 0.1) * norm_r, which is
+    Python arithmetic in double: the rounding csrc/simulate.cu's finish_kernel reproduces."""
     peak = max(np.max(np.abs(noisy)), np.max(np.abs(speech)))
     if interf is not None:
         peak = max(peak, np.max(np.abs(interf)))
@@ -275,22 +289,27 @@ def apply(p, speech, noise, rir=None, interf=None, enroll=None, cut=80000, enrol
         noisy, speech = noisy / peak * 0.99, speech / peak * 0.99
         if interf is not None:
             interf = interf / peak * 0.99
-    noisy, speech = pad_or_cut(noisy, cut, p["cut_offset"]), pad_or_cut(speech, cut, p["cut_offset"])
+    noisy, speech = pad_or_cut(noisy, cut, cut_offset), pad_or_cut(speech, cut, cut_offset)
     if interf is None:
         tgt, src = np.max(np.abs(speech)) + 1e-5, np.max(np.abs(noisy)) + 1e-5
-        factor = min((0.1 + (0.99 - 0.1) * p["norm_r"]) / tgt, 0.99 / max(tgt, src))
+        factor = min((0.1 + (0.99 - 0.1) * norm_r) / tgt, 0.99 / max(tgt, src))
         noisy, speech = noisy * factor, speech * factor
     else:
-        interf = pad_or_cut(interf, cut, p["cut_offset"])
+        interf = pad_or_cut(interf, cut, cut_offset)
         a, b, c = np.max(np.abs(noisy)), np.max(np.abs(speech)), np.max(np.abs(interf))
         factor = 0.99 / (max(a, b, c) + 1e-5)
         least = min(a, b, c)
         if least * factor > 0.1:
             lo = 0.1 / (least * factor)
-            factor = (lo + (1 - lo) * p["norm_r"]) * factor
+            factor = (lo + (1 - lo) * norm_r) * factor
         noisy, speech, interf = noisy * factor, speech * factor, interf * factor
-    if enroll is not None:
-        enroll = pad_or_cut(enroll, enroll_len, p["enroll_offset"])
-        enroll = enroll / (np.max(np.abs(enroll)) + 1e-5) * 0.99
-    out = lambda w: None if w is None else w[0].astype(dt)
-    return out(enroll), out(noisy), out(speech), out(interf)
+    return noisy, speech, interf
+
+
+def enroll(e, enroll_len, offset):
+    """The enrollment: pad_or_cut to `enroll_len` samples at `offset`, then e / (max|e| + 1e-5) * 0.99 -> [1, enroll_len]"""
+    e = pad_or_cut(e, enroll_len, offset)
+    return e / (np.max(np.abs(e)) + 1e-5) * 0.99
+
+
+_enroll = enroll          # apply's argument `enroll` shadows the function there

@@ -415,7 +415,10 @@ __global__ void finish_kernel(const float* __restrict__ noisy, const float* __re
   if (!hi) {
     const float tgt = __fadd_rn(b, 1e-5f), src = __fadd_rn(a, 1e-5f);
     const float thr = __fdiv_rn(0.99f, fmaxf(tgt, src));
-    factor = fminf(__fdiv_rn((float)(0.1 + (0.99 - 0.1) * norm_r[r]), tgt), thr);
+    // the reference's uniform(0.1, 0.99) level, rounded as Python rounds it: product, then sum.  A contracted fma moves the fp32
+    // level by an ulp for some norm_r (tests/test_simulation_stages_gpu.py, FMA_NORM_R).
+    const float level = (float)__dadd_rn(0.1, __dmul_rn(0.99 - 0.1, norm_r[r]));
+    factor = fminf(__fdiv_rn(level, tgt), thr);
   } else {
     factor = __fdiv_rn(0.99f, __fadd_rn(fmaxf(fmaxf(a, b), c), 1e-5f));
     const float least = __fmul_rn(fminf(fminf(a, b), c), factor);
