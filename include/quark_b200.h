@@ -141,6 +141,10 @@ int qb_adalayernorm(const float* x, const float* scale, const float* shift, int6
  * rows [B, T, C] (clip b at x + b * x_batch_stride) -> planes in a padded buffer; channels C..ld-1 zeroed. */
 int qb_snake_planes(const float* x, int64_t x_batch_stride, const float* alpha, int64_t B, int64_t T, int64_t C,
                     qb_half* hi, qb_half* lo, int64_t ld, int64_t rows_per_batch, int64_t row_off, void* stream);
+/* ELU of fp32 rows [B, T, C] (clip b at x + b * x_batch_stride) -> planes in a padded buffer; channels C..ld-1 zeroed.  Reads the
+ * up-sampled frames of a transposed conv's phase GEMM (the ResidualUnit's first ELU, vq/semantic_module.py:78-79). */
+int qb_elu_planes(const float* x, int64_t x_batch_stride, int64_t B, int64_t T, int64_t C, qb_half* hi, qb_half* lo, int64_t ld,
+                  int64_t rows_per_batch, int64_t row_off, void* stream);
 /* x[b,t,:] + vec[b,:] -> planes (prenet output + speaker d-vector, bicodec/bicodec.py:196-197). */
 int qb_addvec_planes(const float* x, const float* vec, int64_t B, int64_t T, int64_t C, qb_half* hi, qb_half* lo,
                      int64_t ld, int64_t rows_per_batch, int64_t row_off, void* stream);
@@ -528,6 +532,20 @@ int qb_codec_decode(qb_codec* c, const int64_t* ac_codes, const int64_t* sem_cod
  * the named intermediate ([B, rows, C] fp32, channel-last); the callee may enqueue a copy on the same stream.  NULL disables. */
 typedef void (*qb_tap_fn)(void* user, const char* name, const float* data, int64_t B, int64_t rows, int64_t C);
 int qb_codec_set_tap(qb_codec* c, qb_tap_fn cb, void* user);
+/* Semantic decoder of a loaded codec (HCodec-2.0/vq/semantic_module.py:252-299, built at vq/codec.py:50-52 and called by
+ * Codec.forward only, vq/codec.py:71): k3 conv -> per block {k3 conv at stride 1 | ConvTranspose1d(2s, s) otherwise} +
+ * 2 x ResidualUnit(ELU, k3 conv, ELU, 1x1 conv, + x) -> k3 conv.  Its own cfg, so qb_codec_cfg keeps its layout.  `named` holds
+ * the reference's semantic_decoder.* tensors (block widths are read from their shapes); the transposed convs are repacked into
+ * phase GEMM weights here, at the codec's semantic-encoder precision.  A codec holds one semantic decoder: a second load fails. */
+typedef struct {
+  int32_t code_dim, output_channels;                 /* 512 -> 768 (semantic_decoder_config) */
+  int32_t n_blocks;                                  /* len(strides) <= 8 */
+  int32_t strides[8];
+} qb_semantic_decoder_cfg;
+int qb_codec_load_semantic_decoder(qb_codec* c, const qb_semantic_decoder_cfg* cfg, const qb_tensor* named, int32_t n);
+/* pred_feat [B, output_channels, N * prod(strides)] fp32 channel-first = the semantic decoder on the semantic codes' codebook-row
+ * sums (vq/codec.py:65-71 with get_output_from_indices); sem_codes int64 [B, nq, N]. */
+int qb_codec_semantic_decode(qb_codec* c, const int64_t* sem_codes, int64_t B, int64_t N, float* pred_feat, void* stream);
 /* Row-level access to the two quantisers of a loaded codec (which = 0 acoustic, 1 semantic). */
 qb_rvq* qb_codec_rvq(qb_codec* c, int32_t which);
 

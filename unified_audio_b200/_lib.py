@@ -74,7 +74,8 @@ def read_header(path):
 
 
 _TYPES, _ENUMS, SIGNATURES = read_header(HEADER)
-RowMap, GemmDesc, Tensor, CodecCfg, TAP_FN = (_TYPES[n] for n in ("qb_rowmap", "qb_gemm_desc", "qb_tensor", "qb_codec_cfg", "qb_tap_fn"))
+RowMap, GemmDesc, Tensor, CodecCfg, SemanticDecoderCfg, TAP_FN = (_TYPES[n] for n in ("qb_rowmap", "qb_gemm_desc", "qb_tensor", "qb_codec_cfg",
+                                                                                 "qb_semantic_decoder_cfg", "qb_tap_fn"))
 globals().update((k.removeprefix("QB_"), v) for k, v in _ENUMS.items() if k.startswith("QB_ACT_"))    # ACT_NONE ... ACT_RELU
 PRECISION_CODES = {k.removeprefix("QB_PRECISION_").lower(): v for k, v in _ENUMS.items() if k.startswith("QB_PRECISION_")}
 

@@ -306,19 +306,6 @@ class BiCodec(_Face):
             v, g = sd[prefix + "weight_v"], sd[prefix + "weight_g"]
             return v * (g / v.reshape(v.shape[0], -1).norm(dim=1).reshape(g.shape))
 
-        def convt_pack(w, s_, split):
-            """ConvTranspose1d weight [Cin, Cout, k], stride s -> [s * Cout, J * Cin_pad], J = ceil(k / s):
-            row (r, co), GEMM tap t multiplies x[q + t - (J-1)] with w[:, co, r + (J-1-t) * s]."""
-            ci, co, k = w.shape
-            J = -(-k // s_)
-            cp = _pad_to(ci, 64)
-            wp = torch.zeros(ci, co, J * s_, device=dev)
-            wp[:, :, :k] = w
-            wp = wp.reshape(ci, co, J, s_)                          # [ci, co, j, r]
-            out = torch.zeros(s_, co, J, cp, device=dev)
-            out[:, :, :, :ci] = wp.permute(3, 1, 2, 0).flip(2)       # tap t <-> j = J-1-t
-            return Planes.from_f32(out.reshape(s_ * co, J * cp), split), J
-
         W = {}
         # ---- gathers
         W["zq_table"] = (sd["quantizer.codebook.weight"] @ wnw("quantizer.out_project.")[:, :, 0].t()
@@ -356,7 +343,7 @@ class BiCodec(_Face):
         for i, (k, r) in enumerate(zip(d["kernel_sizes"], d["rates"])):
             cin, cout = ch // 2 ** i, ch // 2 ** (i + 1)
             b = f"decoder.model.{i + 1}.block."
-            wt, J = convt_pack(wnw(b + "1."), r, sp_gen)
+            wt, J = ops.convt_planes(wnw(b + "1."), r, sp_gen)
             st = dict(alpha=sd[b + "0.alpha"].reshape(-1).contiguous(), wt=wt, J=J, k=k, s=r, cin=cin, cout=cout,
                       bt=sd[b + "1.bias"].repeat(r).contiguous(), units=[])
             for j, dil in enumerate((1, 3, 9)):

@@ -4,8 +4,9 @@ Mirrors QuarkAudio-HCodec/HCodec-2.0/vq/codec.py:17-99:
     Codec(encoder_kwargs, decoder_kwargs, quantizer_kwargs, semantic_encoder_kwargs, semantic_decoder_kwargs)
     Codec.encode(x [B,T], feat [B,768,T50]) -> (acoustic_codes, semantic_codes)  int64 [B,nq,N]
     Codec.decode(acoustic_codes, semantic_codes)  -> wav [B, N*3840]
-state_dict keys/shapes are the reference's (spec.py); `semantic_decoder.*` keys (training-only module,
-codec.py:71) are accepted by load_state_dict and ignored.
+    Codec.forward(x, feat) -> (recon, pred_feat, commit_loss), evaluation mode, with semantic_decoder=True
+state_dict keys/shapes are the reference's (spec.py); `semantic_decoder.*` keys (the module only forward calls, codec.py:71) are
+accepted by load_state_dict and ignored unless the face is built with semantic_decoder=True.
 
 `encode` / `decode` are one call each into the C ABI (csrc/engine.cu through engine.py): the engine owns the repacked
 weights, the workspace and the ~340-kernel orchestration, with activations channel-last [B*T, C] end to end.  There is no
@@ -114,10 +115,32 @@ class _Face(nn.Module):
 
 
 class _CodecFace(_Face):
-    """The codec faces add CUDA-graph capture, the encode -> decode round trip and the refusal of the training forward; their
-    checkpoints carry the training-only `semantic_decoder.*`."""
+    """The codec faces add CUDA-graph capture, the encode -> decode round trip and the evaluation-mode `forward`.  Their
+    checkpoints carry `semantic_decoder.*` (vq/semantic_module.py:252-299, which only `forward` calls): a face built with
+    `semantic_decoder=True` holds those parameters under the reference's names and a strict load requires them; without it
+    they are accepted at load and not kept, and `forward` is refused."""
 
     _IGNORED_KEYS = ("semantic_decoder.",)
+
+    def _add_semantic_decoder(self, enabled: bool, kwargs: dict):
+        """Decoder(**kwargs) of vq/semantic_module.py:252-292 as parameters, when `enabled`."""
+        self.sem_dec_cfg = dict(kwargs) if enabled else None
+        if enabled:
+            self.semantic_decoder = _Tree.build(spec.semantic_decoder_spec(**kwargs))
+            self._IGNORED_KEYS = ()
+
+    def _check_forward(self):
+        if self.sem_dec_cfg is None:
+            raise RuntimeError(f"unified_audio_b200.{type(self).__name__}.forward needs the semantic decoder: construct the face with "
+                               "semantic_decoder=True and load a checkpoint that carries semantic_decoder.*")
+        if self.training:
+            raise RuntimeError(f"unified_audio_b200.{type(self).__name__}.forward runs in evaluation mode only: call .eval() "
+                               "(quantize dropout, codebook updates and gradients through the codec are not built)")
+
+    def _commit_loss(self):
+        """vector_quantize_pytorch's ResidualVQ returns zero commitment losses in eval mode (oracle/rvq.py states the same; the package
+        itself is not pinned), so the reference's (commit_loss + commit_loss_semantic).mean() is a 0-d fp32 zero."""
+        return torch.zeros((), dtype=torch.float32, device=self._dev())
 
     # ------------------------------------------------------------------ CUDA-graph replay of a fixed-shape call
     def graphed(self, fn_name: str, *example_inputs, warmup: int = 2) -> "GraphedCall":
@@ -134,16 +157,13 @@ class _CodecFace(_Face):
         ac, sc = self.encode(x, feat)
         return ac, sc, self.decode(ac, sc)
 
-    def forward(self, x, feat):
-        raise RuntimeError("unified_audio_b200.Codec implements the inference path only (encode / decode); "
-                           "training forward (codec.py:51-72) is out of scope")
-
-
 class Codec(_CodecFace):
     def __init__(self, encoder_kwargs: dict, decoder_kwargs: dict, quantizer_kwargs: dict,
                  semantic_encoder_kwargs: dict, semantic_decoder_kwargs: Optional[dict] = None,
-                 precision: str = "mixed"):
+                 precision: str = "mixed", semantic_decoder: bool = False):
         super().__init__()
+        if semantic_decoder and not semantic_decoder_kwargs:
+            raise ValueError("semantic_decoder=True needs semantic_decoder_kwargs (the reference's semantic_decoder_config)")
         if precision not in PRECISION_POLICIES:
             raise KeyError(f"unknown precision policy {precision!r} (one of {', '.join(PRECISION_POLICIES)})")
         self.enc_cfg, self.dec_cfg = dict(encoder_kwargs), dict(decoder_kwargs)
@@ -153,6 +173,7 @@ class Codec(_CodecFace):
         self.quantizer = ResidualVQ(**quantizer_kwargs)
         self.semantic_quantizer = ResidualVQ(**quantizer_kwargs)
         self.semantic_encoder = _Tree.build(spec.semantic_encoder_spec(**semantic_encoder_kwargs))
+        self._add_semantic_decoder(semantic_decoder, semantic_decoder_kwargs or {})
         self.precision = precision
         self._engine = None
         self.eval()
@@ -166,9 +187,13 @@ class Codec(_CodecFace):
         if self._engine is None:
             from .engine import CodecEngine
             dev = self._require_cuda()
+            sd = self.state_dict()
             self._engine = CodecEngine(dev, self.enc_cfg, self.dec_cfg, dict(num_quantizers=self.quantizer.num_quantizers,
                                                                              codebook_size=self.quantizer.codebook_size),
-                                       self.sem_cfg, self.precision, {k: v for k, v in self.state_dict().items()})
+                                       self.sem_cfg, self.precision,
+                                       {k: v for k, v in sd.items() if not k.startswith("semantic_decoder.")})
+            if self.sem_dec_cfg is not None:
+                self._engine.load_semantic_decoder(self.sem_dec_cfg, {k: v for k, v in sd.items() if k.startswith("semantic_decoder.")})
         return self._engine
 
     @torch.no_grad()
@@ -194,6 +219,23 @@ class Codec(_CodecFace):
             return eng.decode(acoustic_codes, semantic_codes)
         finally:
             eng.set_taps(None)
+
+    @torch.no_grad()
+    def semantic_decode(self, semantic_codes):
+        """vq/codec.py:71 on the codes' quantised rows: int64 [B,nq,N] -> pred_feat fp32 [B, output_channels, N*prod(strides)]
+        (one qb_codec_semantic_decode).  Needs semantic_decoder=True."""
+        if self.sem_dec_cfg is None:
+            raise RuntimeError("Codec.semantic_decode needs the semantic decoder: construct the face with semantic_decoder=True")
+        return self.engine().semantic_decode(semantic_codes)
+
+    def forward(self, x, feat):
+        """vq/codec.py:54-72 in evaluation mode: (recon [B, T], pred_feat fp32 [B, C_ssl, T_feat], commit_loss 0-d fp32).  recon is
+        decode(*encode(x, feat)) - the reference's quantised sum of codebook rows is get_output_from_indices(codes) - and pred_feat
+        the semantic decoder on the semantic stream's codebook rows."""
+        self._check_forward()
+        with torch.no_grad():
+            ac, sc = self.encode(x, feat)
+            return self.decode(ac, sc), self.semantic_decode(sc), self._commit_loss()
 
 
 class GraphedCall:

@@ -117,9 +117,18 @@ def h1_spec(c) -> Dict[str, Dict[str, tuple]]:
     return dict(encoder=enc, decoder=dec, semantic_encoder=sem)
 
 
+def semantic_decoder_config(c) -> dict:
+    """Decoder kwargs of the semantic decoder: the config's own `sem_dec` (H-Codec-1.5's decoder_kwargs["semantic_decoder"]), else
+    the sizes H-Codec-1.0 hard-codes (vq/codec.py:130-136: code_dim -> semantic encoder width -> SSL width, its strides)."""
+    if c.get("sem_dec") is not None:
+        return dict(c["sem_dec"])
+    return dict(code_dim=c["dimension"], output_channels=c["sem_in"], decode_channels=c["sem_ch"],
+                channel_ratios=[1] * len(c["sem_strides"]), strides=list(c["sem_strides"]))
+
+
 class CodecH1(_CodecFace):
     def __init__(self, encoder_kwargs: dict = None, decoder_kwargs: dict = None, quantizer_kwargs: dict = None,
-                 precision: str = "mixed", _cfg: dict = None):
+                 precision: str = "mixed", _cfg: dict = None, semantic_decoder: bool = False):
         super().__init__()
         c = dict(_cfg or H1)
         self.c = c
@@ -130,6 +139,7 @@ class CodecH1(_CodecFace):
         self.quantizer = ResidualVQ(**q)
         self.semantic_quantizer = ResidualVQ(**q)
         self.semantic_encoder = _Tree.build(sp["semantic_encoder"])
+        self._add_semantic_decoder(semantic_decoder, semantic_decoder_config(c))
         self.sem_cfg = dict(encode_channels=c["sem_ch"], out_channels=c["dimension"], strides=c["sem_strides"],
                             channel_ratios=[1] * len(c["sem_strides"]))
         self.dec_cfg = dict(dim=c["dec_dim"], intermediate_dim=c["dec_inter"])
@@ -214,8 +224,90 @@ class CodecH1(_CodecFace):
                         head=Planes.from_f32(sd["decoder.head.out.weight"].float().contiguous(), pol["head"]),
                         head_b=f32("decoder.head.out.bias"), dft_inv=_planes_from_f64(inv, True),
                         window=sd["decoder.head.istft.window"].float().contiguous(), nf=nf, kin=kin, spec_ld=_pad_to(2 * nf, 4))
+        if self.sem_dec_cfg is not None:
+            W["sem_dec"] = self._pack_semantic_decoder(sd)
         self._w = W
         return W
+
+    def _pack_semantic_decoder(self, sd):
+        """semantic_decoder.* -> GEMM weights at the semantic encoder's precision: k3 convs as tap-major planes, each
+        ConvTranspose1d(2s, s) as the phase weight of ops.convt_planes with its bias repeated per phase."""
+        split, p = self.policy["conv"], "semantic_decoder."
+        blocks = []
+        for i, st in enumerate(self.sem_dec_cfg["strides"]):
+            b = f"{p}conv_blocks.{i}."
+            units = [dict(c1=ops.conv_planes(sd[b + f"res_units.{u}.conv1.conv.weight"].float(), split),
+                          c2=ops.conv_planes(sd[b + f"res_units.{u}.conv2.weight"].float(), split)) for u in (0, 1)]
+            if st == 1:
+                w = sd[b + "conv.conv.weight"].float()
+                blocks.append(dict(stride=1, w=ops.conv_planes(w, split), b=sd[b + "conv.conv.bias"].float().contiguous(),
+                                   cin=w.shape[1], cout=w.shape[0], units=units))
+            else:
+                w = sd[b + "conv.deconv.weight"].float()
+                wt, J = ops.convt_planes(w, st, split)
+                blocks.append(dict(stride=st, w=wt, J=J, b=sd[b + "conv.deconv.bias"].float().repeat(st).contiguous(),
+                                   cin=w.shape[0], cout=w.shape[1], units=units))
+        w1, w2 = sd[p + "conv1.conv.weight"].float(), sd[p + "conv2.conv.weight"].float()
+        return dict(conv1=ops.conv_planes(w1, split), code_dim=w1.shape[1], c0=w1.shape[0], blocks=blocks,
+                    conv2=ops.conv_planes(w2, split), cout=w2.shape[0])
+
+    def _semantic_decode_rows(self, z, B, N):
+        """vq/semantic_module.py:294-299 (Decoder), :245-249 (DecoderBlock), :78-81 (ResidualUnit) on quantised rows
+        z [B*N, code_dim] fp32 -> pred_feat fp32 [B, C_ssl, T].  Channel-last planes end to end: every conv input sits in a
+        buffer zero-padded by one frame on each side, the fp32 trunk of a block is updated in place by the 1x1 convs' residual
+        epilogues, and each epilogue writes the planes (ELU'd where the next conv wants it) its consumer reads."""
+        D = self._prepare()["sem_dec"]
+        split = self.policy["conv"]
+        cd = _pad_to(D["code_dim"], 64)
+        zp = self._planes(f"sd_z{N}", (B, N + 2, cd), split)
+        ops.rows_to_planes(z, B, N, D["code_dim"], zp, cd, N + 2, 1)
+        cp = _pad_to(D["c0"], 64)
+        xin = self._planes("sd_in0", (B, N + 2, cp), split)
+        ops.gemm(zp, D["conv1"], D["c0"], a_batch=B, a_rows_per_batch=N + 2, a_ld=cd, m_per_batch=N, taps=3, out_planes=xin,
+                 out_planes_map=(cp, N + 2, 1))
+        T = N
+        for bi, blk in enumerate(D["blocks"]):
+            st, co = blk["stride"], blk["cout"]
+            cpi, cpo = cp, _pad_to(co, 64)
+            pe = None
+            if st == 1:
+                Tn = T
+                trunk = self._buf(f"sd_x{bi}", (B * T, co))
+                tr = rowmap(trunk, co, T, 0)
+                pe = self._planes(f"sd_pe{bi}", (B, T + 2, cpo), split)
+                ops.gemm(xin, blk["w"], co, a_batch=B, a_rows_per_batch=T + 2, a_ld=cpi, m_per_batch=T, taps=3, bias=blk["b"],
+                         out_f32=tr, out_planes=pe, out_planes_map=(cpo, T + 2, 1), act2=ACT_ELU)
+            else:
+                # ConvTranspose1d(2s, s, padding (s+1)//2, output_padding s%2) as a J-tap GEMM (the input buffer's one-frame pads are
+                # the J - 1 = 1 zero rows it needs): row q holds the s phases of uncropped frames q*s.., and the output clip is
+                # frames [pad, pad + T*s) of those rows read as [(T + 1) * s, co]
+                J, pad, Tn = blk["J"], (st + 1) // 2, T * st
+                if J != 2:
+                    raise ValueError(f"semantic decoder block {bi}: a {J}-tap transposed conv is not built (kernel 2 * stride has 2)")
+                up = self._buf(f"sd_up{bi}", (B, T + 1, st * co))
+                ops.gemm(xin, blk["w"], st * co, a_batch=B, a_rows_per_batch=T + 2, a_ld=cpi, m_per_batch=T + 1, taps=J,
+                         bias=blk["b"], out_f32=rowmap(up, st * co, T + 1, 0))
+                tr = rowmap(up, co, (T + 1) * st, pad)
+                pe = self._planes(f"sd_pe{bi}", (B, Tn + 2, cpo), split)
+                ops.elu_planes(up.view(-1)[pad * co:], (T + 1) * st * co, B, Tn, co, pe, cpo, Tn + 2, 1)
+            T = Tn
+            pu = self._planes(f"sd_pu{bi}", (B * T, cpo), split)
+            nxt = self._planes(f"sd_in{bi + 1}", (B, T + 2, cpo), split)
+            for u, un in enumerate(blk["units"]):
+                ops.gemm(pe, un["c1"], co, a_batch=B, a_rows_per_batch=T + 2, a_ld=cpo, m_per_batch=T, taps=3, act=ACT_ELU,
+                         out_planes=pu, out_planes_map=(cpo, T, 0))
+                last = u == len(blk["units"]) - 1
+                ops.gemm(pu, un["c2"], co, a_batch=B, a_rows_per_batch=T, a_ld=cpo, m_per_batch=T, residual=tr,
+                         out_f32=None if last else tr, out_planes=nxt if last else pe, out_planes_map=(cpo, T + 2, 1),
+                         act2=ACT_NONE if last else ACT_ELU)
+            xin, cp = nxt, cpo
+        Co = D["cout"]
+        rows = self._buf("sd_out", (B * T, Co))
+        ops.gemm(xin, D["conv2"], Co, a_batch=B, a_rows_per_batch=T + 2, a_ld=cp, m_per_batch=T, taps=3,
+                 out_f32=rowmap(rows, Co, T, 0))
+        pred = torch.empty(B, Co, T, device=z.device)
+        ops.ssl_compress(rows, B, T, Co, 0.0, True, pred)          # power 0: the plain [B, T, C] -> [B, C, T] copy
+        return pred
 
     def _pack_tf(self, sd, prefix, n):
         pol = self.policy
@@ -486,6 +578,29 @@ class CodecH1(_CodecFace):
         self.quantizer.decode_rows(ia, z, 2 * Dq, 0)
         self.semantic_quantizer.decode_rows(isem, z, 2 * Dq, Dq)
         return self._decode_z(z, B, N, taps)
+
+    def _require_semantic_decoder(self):
+        if self.sem_dec_cfg is None:
+            raise RuntimeError(f"{type(self).__name__}.semantic_decode needs the semantic decoder: construct the face with "
+                               "semantic_decoder=True")
+
+    @torch.no_grad()
+    def semantic_decode(self, semantic_codes):
+        """vq/codec.py:161 on the codes' quantised rows: int64 [B,nq,N] -> pred_feat fp32 [B, 768, N*prod(strides)]."""
+        self._require_semantic_decoder()
+        B, nq, N = semantic_codes.shape
+        z = self._buf("sd_zrows", (B * N, self.semantic_quantizer.dim))
+        self.semantic_quantizer.decode_rows(semantic_codes.transpose(1, 2).reshape(B * N, nq).long().contiguous(), z,
+                                            self.semantic_quantizer.dim, 0)
+        return self._semantic_decode_rows(z, B, N)
+
+    def forward(self, x, feat, use_mask=False, domain_split=None):
+        """vq/codec.py:138-163 in evaluation mode: (recon [B, T], pred_feat fp32 [B, 768, T_feat], commit_loss 0-d fp32), recon =
+        decode(*encode(x, feat)).  use_mask / domain_split are unused by the reference's forward too."""
+        self._check_forward()
+        with torch.no_grad():
+            ac, sc = self.encode(x, feat)
+            return self.decode(ac, sc), self.semantic_decode(sc), self._commit_loss()
 
 
 def _planes_from_f64(w: torch.Tensor, split: bool) -> Planes:

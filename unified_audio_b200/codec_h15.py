@@ -91,10 +91,12 @@ def mimi_spec(t) -> Dict[str, tuple]:
 
 class CodecH15(CodecH1):
     def __init__(self, encoder_kwargs: dict = None, decoder_kwargs: dict = None, quantizer_kwargs: dict = None,
-                 adaptive_kwargs: dict = None, precision: str = "mixed", _cfg: dict = None):
+                 adaptive_kwargs: dict = None, precision: str = "mixed", _cfg: dict = None, semantic_decoder: bool = False):
         c = dict(_cfg) if _cfg is not None else (
             config_from_kwargs(encoder_kwargs, decoder_kwargs, quantizer_kwargs, adaptive_kwargs) if adaptive_kwargs else dict(H15))
-        CodecH1.__init__(self, precision=precision, _cfg=c)
+        if adaptive_kwargs and decoder_kwargs.get("semantic_decoder") is not None:     # conf/config_adaptive_v3.yaml:38-43
+            c["sem_dec"] = dict(decoder_kwargs["semantic_decoder"])
+        CodecH1.__init__(self, precision=precision, _cfg=c, semantic_decoder=semantic_decoder)
         agg = dict(mimi_spec(c["agg"]), query_embedding=(1, c["agg"]["dim"], 1))
         self.semantic_aggregator = _Tree.build(agg)
         self.acoustic_aggregator = _Tree.build(agg)
@@ -251,5 +253,26 @@ class CodecH15(CodecH1):
         out = self.encode(x, feat)
         return out["acoustic_codes"], out["semantic_codes"], self.decode(out["acoustic_codes"], out["semantic_codes"])
 
-    def forward(self, x, feat):
-        raise RuntimeError("CodecH15 is inference-only: use .encode / .decode (training forward of codec_adaptive.py:107-148 is not built)")
+    @torch.no_grad()
+    def semantic_decode(self, semantic_codes, token_lengths=None):
+        """codec_adaptive.py:132,139: the semantic decoder on the de-aggregated semantic stream.  semantic_codes: the length-packed
+        int64 [B,nq,G] of `encode` (or plain codes with token_lengths [B,G]) -> pred_feat fp32 [B, 1024, T * prod(strides)]."""
+        self._require_semantic_decoder()
+        if token_lengths is None:
+            semantic_codes, token_lengths = adaptive.extract_lengths(semantic_codes, self.codebook_size)
+        sc = adaptive.deaggregate_by_lengths(semantic_codes.long(), token_lengths)          # [B, nq, T]
+        B, nq, T = sc.shape
+        z = self._buf(f"sd_zrows{T}", (B * T, self.semantic_quantizer.dim))
+        self.semantic_quantizer.decode_rows(sc.transpose(1, 2).reshape(B * T, nq).contiguous(), z, self.semantic_quantizer.dim, 0)
+        return self._semantic_decode_rows(z, B, T)
+
+    def forward(self, x, feat, use_mask=False, domain_split=None):
+        """codec_adaptive.py:100-147 in evaluation mode, at the threshold encode(threshold=0.0) uses: {'recon' [B, T],
+        'pred_feat' fp32 [B, 1024, T_feat], 'commit_loss' 0-d fp32, 'token_lengths' int64 [B, G]}, recon = decode(**encode(x, feat))."""
+        self._check_forward()
+        with torch.no_grad():
+            codes = self.encode(x, feat)
+            plain, lens = adaptive.extract_lengths(codes["semantic_codes"], self.codebook_size)
+            return dict(recon=self.decode(codes["acoustic_codes"], codes["semantic_codes"]),
+                        pred_feat=self.semantic_decode(plain, token_lengths=lens), commit_loss=self._commit_loss(),
+                        token_lengths=lens)

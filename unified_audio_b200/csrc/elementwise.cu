@@ -658,6 +658,20 @@ __global__ void snake_planes_kernel(const float* __restrict__ x, long long x_bst
   store_planes(hi, lo, (b * rpb + off + t) * ld + c, v);
 }
 
+// ELU of rows with a batch pitch -> planes: the up-sampled frames of a transposed conv sit inside its phase GEMM's output rows,
+// offset by the padding, so clip b starts at x + b * x_bstride rather than at b * T * C
+__global__ void elu_planes_kernel(const float* __restrict__ x, long long x_bstride, int T, int C, __half* __restrict__ hi,
+                                  __half* __restrict__ lo, long long ld, long long rpb, long long off, long long total) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int c = (int)(i % ld);
+  const long long r = i / ld;
+  const int t = (int)(r % T);
+  const long long b = r / T;
+  const float v = c < C ? elu_f(x[b * x_bstride + (long long)t * C + c]) : 0.f;
+  store_planes(hi, lo, (b * rpb + off + t) * ld + c, v);
+}
+
 // x[b, t, c] + vec[b, c] -> planes (the speaker d-vector added to every frame, bicodec/bicodec.py:197)
 __global__ void addvec_planes_kernel(const float* __restrict__ x, const float* __restrict__ vec, int T, int C,
                                      __half* __restrict__ hi, __half* __restrict__ lo, long long ld, long long rpb,
@@ -686,6 +700,15 @@ extern "C" int qb_snake_planes(const float* x, int64_t x_batch_stride, const flo
   }
   snake_planes_kernel<<<(unsigned)ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(
       x, x_batch_stride, alpha, (int)T, (int)C, (__half*)hi, (__half*)lo, ld, rows_per_batch, row_off, total);
+  QB_LAUNCH_END();
+}
+
+extern "C" int qb_elu_planes(const float* x, int64_t x_batch_stride, int64_t B, int64_t T, int64_t C, qb_half* hi, qb_half* lo,
+                             int64_t ld, int64_t rows_per_batch, int64_t row_off, void* stream) {
+  QB_REQUIRE(x && hi && T >= 1 && C <= ld && row_off + T <= rows_per_batch && x_batch_stride >= T * C, "elu_planes: bad args");
+  const long long total = B * T * ld;
+  elu_planes_kernel<<<(unsigned)ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(
+      x, x_batch_stride, (int)T, (int)C, (__half*)hi, (__half*)lo, ld, rows_per_batch, row_off, total);
   QB_LAUNCH_END();
 }
 

@@ -100,6 +100,24 @@ __global__ void repack_conv_kernel(const float* __restrict__ w, int Cout, int Ci
     if (lo) lo[i] = l;
   }
 }
+// ConvTranspose1d weight [Cin, Cout, k], stride s -> phase GEMM weight [s * Cout, J * Cpad] planes (J = ceil(k / s) taps): row
+// (r, co), tap t holds w[:, co, r + (J-1-t) * s] (zero beyond k and in the channel pad) - ops.convt_planes, same layout
+__global__ void repack_convt_kernel(const float* __restrict__ w, int Cin, int Cout, int k, int s, int J, int Cpad,
+                                    __half* __restrict__ hi, __half* __restrict__ lo) {
+  const long long total = (long long)s * Cout * J * Cpad;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % Cpad);
+    const int t = (int)((i / Cpad) % J);
+    const long long row = i / ((long long)Cpad * J);
+    const int co = (int)(row % Cout), r = (int)(row / Cout);
+    const int j = r + (J - 1 - t) * s;
+    const float v = (c < Cin && j < k) ? w[((long long)c * Cout + co) * k + j] : 0.f;
+    __half h, l;
+    split_f16(v, h, l);
+    hi[i] = h;
+    if (lo) lo[i] = l;
+  }
+}
 // rows of a and b interleaved: out[2j] = a[j], out[2j+1] = b[j]  (SwiGLU gate/up pairs)
 __global__ void interleave_rows_kernel(const float* __restrict__ a, const float* __restrict__ b, long long rows, int cols,
                                        float* __restrict__ out) {
@@ -274,6 +292,11 @@ struct SemBlockW {
   const float* conv_b;
   int stride, k;
 };
+struct SemDecBlockW {
+  PlanesD conv, u_c1[2], u_c2[2];   // conv: k3 conv (stride 1) or the transposed conv's phase weight
+  const float* b;                   // bias, repeated per phase for a transposed conv
+  int stride, cout;
+};
 struct Policy {
   bool convnext, lstm_attn, mlp, mlp_dec, conv, head, dft;
 };
@@ -332,6 +355,11 @@ struct qb_codec {
   PlanesD d_embed, d_head;
   const float *d_embed_b, *d_gn_w, *d_gn_b, *d_norm_w, *d_norm_b, *d_fnorm_w, *d_fnorm_b, *d_head_b;
   ResnetW d_res[4];
+  // semantic decoder (qb_codec_load_semantic_decoder; absent until loaded)
+  bool has_sdec = false;
+  int sd_code_dim = 0, sd_c0 = 0, sd_out = 0;
+  PlanesD sd_conv1, sd_conv2;
+  std::vector<SemDecBlockW> sd_blocks;
   // RoPE tables by sequence length
   std::map<int, std::pair<const float*, const float*>> rope;
   qb_rvq* q[2] = {nullptr, nullptr};
@@ -632,6 +660,60 @@ static int encode_sem(qb_codec* c, const float* feat_in, int64_t B, int64_t F, f
   *out_p = out;
   *N_out = Tc;
   return 0;
+}
+
+// vq/semantic_module.py:294-299 (Decoder), :245-249 (DecoderBlock), :78-81 (ResidualUnit).  z [B*N, code_dim] fp32 -> pred_feat
+// [B, output_channels, T] fp32.  Every conv input sits in a planes buffer padded by one zero frame on each side; a block's fp32
+// trunk is updated in place by the 1x1 convs' residual epilogues, and each epilogue writes the planes its consumer reads.
+static int semantic_decode_z(qb_codec* c, const float* z, int64_t B, int64_t N, float* pred, void* st) {
+  const bool pc = c->pol.conv;
+  const int cd = (int)pad_to(c->sd_code_dim, 64);
+  PlanesD zp, xin;
+  QB_TRY(c->ws.padded(&zp, "sd_z", B, N + 2, cd, pc));
+  QB_TRY(qb_rows_to_planes(z, B, N, c->sd_code_dim, 1, QB_ACT_NONE, (qb_half*)zp.hi, (qb_half*)zp.lo, cd, N + 2, 1, st));
+  int cp = (int)pad_to(c->sd_c0, 64);
+  QB_TRY(c->ws.padded(&xin, "sd_in0", B, N + 2, cp, pc));
+  QB_TRY(G(zp, B, N + 2, cd, N, c->sd_conv1, c->sd_c0, 3).outp(xin, cp, N + 2, 1).run(st));
+  int64_t T = N;
+  for (size_t bi = 0; bi < c->sd_blocks.size(); ++bi) {
+    const SemDecBlockW& blk = c->sd_blocks[bi];
+    const int co = blk.cout, cpo = (int)pad_to(co, 64), s = blk.stride;
+    const std::string id = std::to_string(bi);
+    float* trunk;
+    int64_t tr_rpb, tr_off, Tn;
+    PlanesD pe, pu, nxt;
+    if (s == 1) {
+      Tn = T; tr_rpb = T; tr_off = 0;
+      QB_TRY(c->ws.f32(&trunk, "sd_x" + id, (size_t)B * T * co));
+      QB_TRY(c->ws.padded(&pe, "sd_pe" + id, B, T + 2, cpo, pc));
+      QB_TRY(G(xin, B, T + 2, cp, T, blk.conv, co, 3).bias(blk.b).out32(trunk, co, T, 0).outp(pe, cpo, T + 2, 1).act2(QB_ACT_ELU).run(st));
+    } else {
+      // ConvTranspose1d(2s, s, padding (s+1)/2, output_padding s%2) as a 2-tap GEMM over the one-frame-padded input: row q holds the
+      // s phases of uncropped frames q*s.., and the output clip is frames [pad, pad + T*s) of the rows read as [(T+1)*s, co]
+      const int pad = (s + 1) / 2;
+      Tn = T * s; tr_rpb = (T + 1) * s; tr_off = pad;
+      QB_TRY(c->ws.f32(&trunk, "sd_up" + id, (size_t)B * (T + 1) * s * co));
+      QB_TRY(G(xin, B, T + 2, cp, T + 1, blk.conv, (int64_t)s * co, 2).bias(blk.b).out32(trunk, (int64_t)s * co, T + 1, 0).run(st));
+      QB_TRY(c->ws.padded(&pe, "sd_pe" + id, B, Tn + 2, cpo, pc));
+      QB_TRY(qb_elu_planes(trunk + (int64_t)pad * co, (T + 1) * s * co, B, Tn, co, (qb_half*)pe.hi, (qb_half*)pe.lo, cpo, Tn + 2, 1, st));
+    }
+    T = Tn;
+    QB_TRY(c->ws.planes(&pu, "sd_pu" + id, (size_t)B * T * cpo, pc));
+    QB_TRY(c->ws.padded(&nxt, "sd_in" + std::to_string(bi + 1), B, T + 2, cpo, pc));
+    for (int u = 0; u < 2; ++u) {
+      QB_TRY(G(pe, B, T + 2, cpo, T, blk.u_c1[u], co, 3).act(QB_ACT_ELU).outp(pu, cpo, T, 0).run(st));
+      G g2(pu, B, T, cpo, T, blk.u_c2[u], co);
+      g2.residual(trunk, co, tr_rpb, tr_off);
+      if (u == 0) g2.out32(trunk, co, tr_rpb, tr_off).outp(pe, cpo, T + 2, 1).act2(QB_ACT_ELU);
+      else g2.outp(nxt, cpo, T + 2, 1);
+      QB_TRY(g2.run(st));
+    }
+    xin = nxt; cp = cpo;
+  }
+  float* rows;
+  QB_TRY(c->ws.f32(&rows, "sd_out", (size_t)B * T * c->sd_out));
+  QB_TRY(G(xin, B, T + 2, cp, T, c->sd_conv2, c->sd_out, 3).out32(rows, c->sd_out, T, 0).run(st));
+  return qb_ssl_compress(rows, B, T, c->sd_out, 0.f, 1, pred, st);      // power 0: the plain [B, T, C] -> [B, C, T] copy
 }
 
 // vq/codec_decoder.py:62-72.  z [B*N, input_channels] fp32 -> wav [B, N*factor*hop]
@@ -941,4 +1023,97 @@ extern "C" int qb_codec_decode(qb_codec* c, const int64_t* ac_codes, const int64
   g_launches++;
   QB_TRY(qb_rvq_decode(rows, c->q[1]->cb, B * N, Dq, c->cfg.codebook_size, nq, z, 2 * Dq, Dq, stream));
   return decode_z(c, z, B, N, wav, stream);
+}
+
+extern "C" int qb_codec_load_semantic_decoder(qb_codec* c, const qb_semantic_decoder_cfg* cfg, const qb_tensor* named, int32_t n) {
+  QB_REQUIRE(c && cfg && named && n > 0, "codec_load_semantic_decoder: bad args");
+  QB_REQUIRE(!c->has_sdec, "codec_load_semantic_decoder: this codec already holds a semantic decoder");
+  QB_REQUIRE(cfg->n_blocks >= 0 && cfg->n_blocks <= 8 && cfg->code_dim > 0 && cfg->output_channels > 0,
+             "codec_load_semantic_decoder: n_blocks must be in [0, 8]");
+  QB_CHECK_CUDA(cudaSetDevice(c->h->device));
+  WeightTable wt;
+  QB_TRY(wt.init(named, n));
+  Loader L(wt, c->arena);
+  const bool pc = c->pol.conv;
+  const std::string p = "semantic_decoder.";
+  const qb_tensor* t;
+  QB_TRY(L.get(&t, p + "conv1.conv.weight", 3));
+  QB_REQUIRE(t->shape[1] == cfg->code_dim && t->shape[2] == 3, "codec_load_semantic_decoder: conv1 must be [C, code_dim %d, 3]", cfg->code_dim);
+  c->sd_code_dim = cfg->code_dim;
+  c->sd_c0 = (int)t->shape[0];
+  QB_TRY(L.conv(&c->sd_conv1, p + "conv1.conv.weight", pc));
+  std::vector<SemDecBlockW> blocks(cfg->n_blocks);
+  int cin = c->sd_c0;
+  for (int i = 0; i < cfg->n_blocks; ++i) {
+    const std::string b = p + "conv_blocks." + std::to_string(i) + ".";
+    SemDecBlockW& w = blocks[i];
+    w.stride = cfg->strides[i];
+    QB_REQUIRE(w.stride >= 1, "codec_load_semantic_decoder: block %d stride %d", i, w.stride);
+    if (w.stride == 1) {
+      QB_TRY(L.get(&t, b + "conv.conv.weight", 3));
+      QB_REQUIRE(t->shape[1] == cin && t->shape[2] == 3, "codec_load_semantic_decoder: block %d conv must be [Cout, %d, 3]", i, cin);
+      w.cout = (int)t->shape[0];
+      QB_TRY(L.conv(&w.conv, b + "conv.conv.weight", pc));
+      QB_TRY(L.f32(&w.b, b + "conv.conv.bias"));
+    } else {
+      const int s = w.stride;
+      QB_TRY(L.get(&t, b + "conv.deconv.weight", 3));
+      QB_REQUIRE(t->shape[0] == cin && t->shape[2] == 2 * s, "codec_load_semantic_decoder: block %d deconv must be [%d, Cout, %d]", i, cin, 2 * s);
+      w.cout = (int)t->shape[1];
+      const int Cpad = (int)pad_to(cin, 64), J = 2;
+      const long long nel = (long long)s * w.cout * J * Cpad;
+      QB_TRY(c->arena.alloc((void**)&w.conv.hi, (size_t)nel * 2, false));
+      w.conv.lo = nullptr;
+      if (pc) QB_TRY(c->arena.alloc((void**)&w.conv.lo, (size_t)nel * 2, false));
+      repack_convt_kernel<<<grid_for(nel), 256>>>(t->data, cin, w.cout, 2 * s, s, J, Cpad, w.conv.hi, w.conv.lo);
+      QB_CHECK_CUDA(cudaGetLastError());
+      const qb_tensor* bt;
+      QB_TRY(L.get(&bt, b + "conv.deconv.bias", 1));
+      QB_REQUIRE(bt->shape[0] == w.cout, "codec_load_semantic_decoder: block %d deconv bias must have %d entries", i, w.cout);
+      std::vector<float> hb(w.cout), rep((size_t)s * w.cout);
+      QB_CHECK_CUDA(cudaMemcpy(hb.data(), bt->data, (size_t)w.cout * 4, cudaMemcpyDeviceToHost));
+      for (int r = 0; r < s; ++r) std::copy(hb.begin(), hb.end(), rep.begin() + (size_t)r * w.cout);
+      float* db;
+      QB_TRY(c->arena.alloc((void**)&db, rep.size() * 4, false));
+      QB_CHECK_CUDA(cudaMemcpy(db, rep.data(), rep.size() * 4, cudaMemcpyHostToDevice));
+      w.b = db;
+    }
+    for (int u = 0; u < 2; ++u) {
+      const std::string r = b + "res_units." + std::to_string(u) + ".";
+      QB_TRY(L.get(&t, r + "conv1.conv.weight", 3));
+      QB_REQUIRE(t->shape[0] == w.cout && t->shape[1] == w.cout && t->shape[2] == 3, "codec_load_semantic_decoder: %sconv1 shape", r.c_str());
+      QB_TRY(L.conv(&w.u_c1[u], r + "conv1.conv.weight", pc));
+      QB_TRY(L.get(&t, r + "conv2.weight", 3));
+      QB_REQUIRE(t->shape[0] == w.cout && t->shape[1] == w.cout && t->shape[2] == 1, "codec_load_semantic_decoder: %sconv2 shape", r.c_str());
+      QB_TRY(L.conv(&w.u_c2[u], r + "conv2.weight", pc));
+    }
+    cin = w.cout;
+  }
+  QB_TRY(L.get(&t, p + "conv2.conv.weight", 3));
+  QB_REQUIRE(t->shape[0] == cfg->output_channels && t->shape[1] == cin && t->shape[2] == 3,
+             "codec_load_semantic_decoder: conv2 must be [%d, %d, 3]", cfg->output_channels, cin);
+  QB_TRY(L.conv(&c->sd_conv2, p + "conv2.conv.weight", pc));
+  c->sd_out = cfg->output_channels;
+  c->sd_blocks = blocks;
+  QB_CHECK_CUDA(cudaDeviceSynchronize());
+  c->has_sdec = true;
+  return 0;
+}
+
+extern "C" int qb_codec_semantic_decode(qb_codec* c, const int64_t* sem_codes, int64_t B, int64_t N, float* pred_feat, void* stream) {
+  QB_REQUIRE(c && sem_codes && pred_feat && B >= 1 && N >= 1, "codec_semantic_decode: bad args");
+  QB_REQUIRE(c->has_sdec, "codec_semantic_decode: no semantic decoder loaded (qb_codec_load_semantic_decoder)");
+  QB_REQUIRE(c->sd_code_dim == c->cfg.dimension, "codec_semantic_decode: decoder code_dim %d != quantiser dim %d", c->sd_code_dim,
+             c->cfg.dimension);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int nq = c->cfg.num_quantizers, Dq = c->cfg.dimension;
+  int64_t* rows;
+  float* z;
+  QB_TRY(c->ws.get((void**)&rows, "codes_rows", (size_t)B * N * nq * 8));
+  QB_TRY(c->ws.f32(&z, "sd_zrows", (size_t)B * N * Dq));
+  codes_bqn_to_rows_kernel<<<grid_for((long long)B * N * nq), 256, 0, st>>>(sem_codes, (int)B, (int)N, nq, rows);
+  g_launches++;
+  QB_CHECK_CUDA(cudaGetLastError());
+  QB_TRY(qb_rvq_decode(rows, c->q[1]->cb, B * N, Dq, c->cfg.codebook_size, nq, z, Dq, 0, stream));
+  return semantic_decode_z(c, z, B, N, pred_feat, stream);
 }

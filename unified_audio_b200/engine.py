@@ -132,6 +132,31 @@ class CodecEngine:
         _lib.check(self.lib.qb_codec_decode(self.h, ac.data_ptr(), sc.data_ptr(), B, N, wav.data_ptr(), _stream()))
         return wav
 
+    def load_semantic_decoder(self, cfg: dict, state_dict: Dict[str, torch.Tensor]):
+        """qb_codec_load_semantic_decoder: cfg = the reference's semantic_decoder_config, state_dict = its semantic_decoder.* tensors"""
+        if len(cfg["strides"]) > 8:
+            raise ValueError("semantic decoder: at most 8 blocks")
+        c = _lib.SemanticDecoderCfg()
+        c.code_dim, c.output_channels, c.n_blocks = cfg["code_dim"], cfg["output_channels"], len(cfg["strides"])
+        for i, s in enumerate(cfg["strides"]):
+            c.strides[i] = s
+        arr, keep = _tensor_array(state_dict)
+        _lib.check(self.lib.qb_codec_load_semantic_decoder(self.h, C.byref(c), arr, len(state_dict)))
+        del keep
+        self.sem_dec_out, self.sem_dec_up = cfg["output_channels"], 1
+        for s in cfg["strides"]:
+            self.sem_dec_up *= s
+
+    def semantic_decode(self, sc: torch.Tensor):
+        """int64 [B, nq, N] -> pred_feat fp32 [B, output_channels, N * prod(strides)]"""
+        B, nq, N = sc.shape
+        if nq != self.cfg.num_quantizers:
+            raise ValueError(f"semantic codes must have {self.cfg.num_quantizers} quantiser layers, got {nq}")
+        sc = sc.long().contiguous()
+        out = torch.empty(B, self.sem_dec_out, N * self.sem_dec_up, device=sc.device)
+        _lib.check(self.lib.qb_codec_semantic_decode(self.h, sc.data_ptr(), B, N, out.data_ptr(), _stream()))
+        return out
+
     def rvq(self, which: int) -> "RvqEngine":
         return RvqEngine(handle=self.lib.qb_codec_rvq(self.h, which), owner=self, nq=self.cfg.num_quantizers, D=self.cfg.dimension)
 

@@ -55,6 +55,22 @@ def conv_planes(w: torch.Tensor, split: bool = True) -> Planes:
     return Planes.from_f32(out.reshape(co, -1), split)
 
 
+def convt_planes(w: torch.Tensor, s: int, split: bool = True):
+    """ConvTranspose1d weight [Cin, Cout, k], stride s -> (planes [s * Cout, J * pad64(Cin)], J = ceil(k / s)): the weight of a
+    J-tap GEMM over the input zero-padded by J - 1 rows on both sides whose output row q holds all s phases of output frames
+    q*s .. q*s + s - 1 of the uncropped transposed conv (a ConvTranspose1d with padding p is rows shifted by p).
+    Row (r, co), GEMM tap t multiplies x[q + t - (J-1)] with w[:, co, r + (J-1-t) * s]."""
+    ci, co, k = w.shape
+    J = -(-k // s)
+    cp = (ci + 63) // 64 * 64
+    wp = w.new_zeros(ci, co, J * s)
+    wp[:, :, :k] = w
+    wp = wp.reshape(ci, co, J, s)                              # [ci, co, j, r]
+    out = w.new_zeros(s, co, J, cp)
+    out[:, :, :, :ci] = wp.permute(3, 1, 2, 0).flip(2)         # tap t <-> j = J-1-t
+    return Planes.from_f32(out.reshape(s * co, J * cp), split), J
+
+
 def pad_k_planes(w: torch.Tensor, kp: int, split: bool = True) -> Planes:
     """Dense weight [N, K] -> planes [N, kp], columns K..kp zero (K padded to the GEMM's multiple of 64)."""
     out = w.new_zeros(w.shape[0], kp)
@@ -175,6 +191,11 @@ def adalayernorm(x, scale, shift, cond_stride, B, rows, Cc, eps=1e-6, out_f32=No
 def snake_planes(x, x_batch_stride, alpha, B, T, Cc, out: Planes, ld, rows_per_batch, row_off):
     _lib.check(_lib.load().qb_snake_planes(_p(x), x_batch_stride, _p(alpha), B, T, Cc, _p(out.hi), _p(out.lo), ld,
                                            rows_per_batch, row_off, _stream()))
+
+
+def elu_planes(x, x_batch_stride, B, T, Cc, out: Planes, ld, rows_per_batch, row_off):
+    _lib.check(_lib.load().qb_elu_planes(_p(x), x_batch_stride, B, T, Cc, _p(out.hi), _p(out.lo), ld, rows_per_batch, row_off,
+                                         _stream()))
 
 
 def addvec_planes(x, vec, B, T, Cc, out: Planes, ld, rows_per_batch, row_off):

@@ -113,4 +113,32 @@ def semantic_encoder_spec(input_channels, encode_channels, out_channels, channel
     return out
 
 
+def semantic_decoder_spec(code_dim, output_channels, decode_channels, channel_ratios=(1, 1), strides=(1, 1), kernel_size=3,
+                          bias=True, block_dilations=(1, 1), unit_kernel_size=3):
+    """vq/semantic_module.py:252-292 (Decoder), :205-249 (DecoderBlock: k3 conv at stride 1, ConvTranspose1d(2s, s) otherwise)."""
+    if not (kernel_size == 3 and unit_kernel_size == 3 and tuple(block_dilations) == (1, 1) and bias):
+        raise ValueError("semantic decoder: only kernel_size 3, unit_kernel_size 3, block_dilations (1, 1) and bias=True (the shipped "
+                         "configs) are built")
+    if len(channel_ratios) != len(strides) or any(int(s) < 1 for s in strides):
+        raise ValueError(f"semantic decoder: one channel ratio per stride and strides >= 1, got {list(channel_ratios)} / {list(strides)}")
+    out = OrderedDict()
+    out["conv1.conv.weight"] = (int(decode_channels * channel_ratios[0]), code_dim, 3)
+    cout = decode_channels
+    for i, st in enumerate(strides):
+        cin = int(decode_channels * channel_ratios[i])
+        cout = int(decode_channels * channel_ratios[i + 1]) if i + 1 < len(strides) else decode_channels
+        p = f"conv_blocks.{i}."
+        if st == 1:
+            out[p + "conv.conv.weight"] = (cout, cin, 3)
+            out[p + "conv.conv.bias"] = (cout,)
+        else:
+            out[p + "conv.deconv.weight"] = (cin, cout, 2 * st)
+            out[p + "conv.deconv.bias"] = (cout,)
+        for u in (0, 1):
+            out[p + f"res_units.{u}.conv1.conv.weight"] = (cout, cout, 3)
+            out[p + f"res_units.{u}.conv2.weight"] = (cout, cout, 1)
+    out["conv2.conv.weight"] = (output_channels, cout, 3)
+    return out
+
+
 BUFFERS = ("stft.window", "head.istft.window")
