@@ -237,6 +237,11 @@ int qb_rvq_decode(const int64_t* idx, const float* codebooks, int64_t M, int32_t
  * output, before normalisation) if not NULL.  1 <= cdim <= 16. */
 int qb_fvq_tokenize(const float* z, int64_t M, int32_t D_in, const float* w_in, const float* b_in, const double* codebook_n,
                     int32_t K, int32_t cdim, int64_t* idx, float* z_e, void* stream);
+/* FactorizedVectorQuantize.forward's code usage in eval mode (factorized_vector_quantize.py:97-103): idx [n] int64 ->
+ * perplexity = exp(-sum_k p_k log(p_k + 1e-10)), p_k = count_k / n (fp64, rounded to fp32), and active = the number of codes used at
+ * least once (fp32), each a single device float.  counts: K int32 of scratch (the histogram, integer atomics).  n >= 1 and K >= 1
+ * are checked; an index outside [0, K) is not counted (the indices come from qb_fvq_tokenize, which writes none). */
+int qb_fvq_usage(const int64_t* idx, int64_t n, int32_t K, int32_t* counts, float* perplexity, float* active, void* stream);
 
 /* ---------------------------------------------------------------- UniSE AR-LM (decoder-only Llama-style LM)
  * Reference: QuarkAudio-UniSE/model/llm/llm.py:150-228 (llm_forward over HF Llama decoder layers),
@@ -438,6 +443,20 @@ int qb_cross_attention(const float* q, const float* kv, int64_t B, int64_t Nq, i
  * `levels` is a HOST array of n_levels <= 8 entries; num_quantizers other than 1 is refused. */
 int qb_fsq_tokenize(const float* x, int64_t rows, int32_t dim, const float* gamma, const float* w_in, const float* b_in, int32_t n_levels,
                     const int32_t* levels, int32_t num_quantizers, int32_t* idx, float* z, float* xn, void* stream);
+/* ASTP with global context (pooling_layers.py:119-144), the pooling of ECAPA_TDNN's x-vector (ecapa_tdnn.py:205-207), around qb_gemm:
+ * x is the fp32 latent [B, T, C] channel-last.  Per (clip, channel) every time sum runs over the T frames in order in fp64.
+ * qb_asp_context: [mean | sqrt(var + 1e-7)] with the unbiased variance (torch.var, divisor T - 1; T >= 2) -> out [B, 2C] fp32 and
+ *   planes [B, ld] (columns 0..2C-1), the A operand of linear1's context part.
+ * qb_asp_tanh_planes: tanh(h[b*T + t, :] + row[b, :]) over N columns -> planes [B*T, ld], zero past N: linear1 split into its x
+ *   part h (a GEMM over the frames) and its context part plus bias (one row per clip), which a GEMM epilogue cannot add (act comes
+ *   before residual, and a row map has no per-clip broadcast).
+ * qb_asp_pool: alpha = softmax over T of logits [B, T, C] (maximum subtracted), mean = sum alpha x, std = sqrt(max(sum alpha x^2 -
+ *   mean^2, 1e-7)) -> out [B, 2C] = [mean | std] fp32 and planes [B, ld], the input of the BatchNorm-folded final linear. */
+int qb_asp_context(const float* x, int64_t B, int64_t T, int32_t C, float* out, qb_half* hi, qb_half* lo, int64_t ld, void* stream);
+int qb_asp_tanh_planes(const float* h, const float* row, int64_t B, int64_t T, int32_t N, qb_half* hi, qb_half* lo, int64_t ld,
+                       void* stream);
+int qb_asp_pool(const float* x, const float* logits, int64_t B, int64_t T, int32_t C, float* out, qb_half* hi, qb_half* lo, int64_t ld,
+                void* stream);
 
 /* ---------------------------------------------------------------- H-Codec-1.5 adaptive frame-rate primitives (SURVEY 8f.4)
  * FlexiCodec._perform_similarity_alignment_vectorized (HCodec-1.5/adaptive/modeling_flexicodec_new.py:828-921): h [B, T, D] fp32 ->

@@ -23,8 +23,17 @@ and a strict load requires `encoder.*` (feat_encoder.py:29-90) and `quantizer.in
 run on the same GEMM / ConvNeXt kernels as the prenet, SamplingBlock(1)'s 3 x folded into the downsample backbones' embed convs, and
 `project` is one GEMM; `qb_fvq_tokenize` (csrc/rvq.cu) does in_project, the normalisation and the codebook arg-max in fp64.  Every
 encoder contraction is a 3-term split whatever `precision` says (the tokens are discrete; `precision` governs detokenize).  With
-both flags, `tokenize(batch)` returns (semantic_tokens, global_tokens).  `postnet.*` (training only) and `quantizer.cluster_size`
-are always ignored.  ENCODER_PARAMS restates the published encoder section for a config without an "encoder" entry.
+both flags, `tokenize(batch)` returns (semantic_tokens, global_tokens).  `postnet.*` and `quantizer.cluster_size` are ignored.
+ENCODER_PARAMS restates the published encoder section for a config without an "encoder" entry.
+
+With `full=True` (both token paths implied) the module is the reference's whole BiCodec and runs its eval-mode forward,
+bicodec.py:113-149:
+    BiCodec.forward({"feat", "ref_wav", "wav"}) -> {"recons", "pred_feat", "x_vector", "d_vector", "perplexity", "cluster_size",
+                                                    "vq_loss", "audios", "with_speaker_loss"}
+and a strict load also requires `postnet.*` (POSTNET_PARAMS restates the published section) and the x-vector branch
+`speaker_encoder.speaker_encoder.{pool,bn,linear}.*`; only `mel_transformer.*`, `quantizer.cluster_size` and BatchNorm's
+`num_batches_tracked` stay ignored.  The postnet runs on the prenet's kernels; ASTP pooling and the codebook usage statistics are
+kernels of csrc/speaker.cu and csrc/rvq.cu around 3-term GEMMs.
 
 How the path maps onto the library (every arithmetic op is a libquark_b200 kernel; channel-last activations):
   * FactorizedVectorQuantize.detokenize (modules/vq/factorized_vector_quantize.py:154-167) and the residual-FSQ de-quantiser
@@ -40,7 +49,7 @@ How the path maps onto the library (every arithmetic op is a libquark_b200 kerne
 from __future__ import annotations
 
 import math
-from typing import Dict
+from typing import Dict, Optional
 
 import torch
 
@@ -64,7 +73,13 @@ MEL_PARAMS = dict(sample_rate=16000, n_fft=1024, win_length=640, hop_length=320,
 # MEL_PARAMS and likewise not verifiable offline.  A config without an "encoder" entry uses these.
 ENCODER_PARAMS = dict(input_channels=1024, vocos_dim=384, vocos_intermediate_dim=2048, vocos_num_layers=12, out_channels=1024,
                       sample_ratios=[1, 1])
+# BiCodec's `postnet` section (feat_decoder.Decoder without a condition, which only forward runs): restated from the published
+# Spark-TTS-0.5B configuration as well as it can be recalled - it is not in the reference tree and cannot be checked offline.  A
+# config with a "postnet" entry overrides it.
+POSTNET_PARAMS = dict(input_channels=1024, vocos_dim=384, vocos_intermediate_dim=2048, vocos_num_layers=6, out_channels=1024,
+                      sample_ratios=[1, 1], use_tanh_at_final=False)
 ECAPA_C, ECAPA_SCALE, ECAPA_OUT, HEADS = 512, 8, 1536, 8   # ECAPA_TDNN_GLOB_c512, dim_context = 512 * 3, 8 heads x 64 (fixed)
+ASTP_BOTTLENECK = 128                                      # ASTP's bottleneck_dim (pooling_layers.py:119), fixed
 
 # 3-term split (True) or single-pass fp16 (False) per GEMM group; "accurate" is the default until the error budget of the
 # 26-conv generator is mapped (DESIGN.md)
@@ -104,6 +119,20 @@ def _backbone_spec(out, prefix, cin, dim, inter, layers, cond):
     out[prefix + "final_layer_norm.weight"] = (dim,); out[prefix + "final_layer_norm.bias"] = (dim,)
 
 
+def _feat_decoder_spec(out, prefix, p, cond):
+    """feat_decoder.Decoder (feat_decoder.py:29-79) under `prefix`: linear_pre, the SamplingBlock(1) + 2-layer backbones, the main
+    backbone (AdaLayerNorm on a `cond`-wide condition, or LayerNorm when cond is None) and linear"""
+    dim, inter = p["vocos_dim"], p["vocos_intermediate_dim"]
+    name = prefix.rstrip(".")
+    out[prefix + "linear_pre.weight"] = (dim, p["input_channels"]); out[prefix + "linear_pre.bias"] = (dim,)
+    for i, r in enumerate(p["sample_ratios"]):
+        if r != 1:
+            raise NotImplementedError(f"{name} SamplingBlock ratios other than 1 (the shipped configuration uses [1, 1])")
+        _backbone_spec(out, f"{prefix}downsample.{i}.1.", dim, dim, inter, 2, None)
+    _backbone_spec(out, prefix + "vocos_backbone.", dim, dim, inter, p["vocos_num_layers"], cond)
+    out[prefix + "linear.weight"] = (p["out_channels"], dim); out[prefix + "linear.bias"] = (p["out_channels"],)
+
+
 def bicodec_spec(c) -> Dict[str, tuple]:
     """Reference state-dict keys -> shapes of the detokenize path."""
     out: Dict[str, tuple] = {}
@@ -116,14 +145,7 @@ def bicodec_spec(c) -> Dict[str, tuple]:
     out["speaker_encoder.quantizer.project_out.bias"] = (s["latent_dim"],)
     out["speaker_encoder.project.weight"] = (s["out_dim"], s["latent_dim"] * s["token_num"])
     out["speaker_encoder.project.bias"] = (s["out_dim"],)
-    dim, inter = p["vocos_dim"], p["vocos_intermediate_dim"]
-    out["prenet.linear_pre.weight"] = (dim, p["input_channels"]); out["prenet.linear_pre.bias"] = (dim,)
-    for i, r in enumerate(p["sample_ratios"]):
-        if r != 1:
-            raise NotImplementedError("prenet SamplingBlock ratios other than 1 (the shipped configuration uses [1, 1])")
-        _backbone_spec(out, f"prenet.downsample.{i}.1.", dim, dim, inter, 2, None)
-    _backbone_spec(out, "prenet.vocos_backbone.", dim, dim, inter, p["vocos_num_layers"], p["condition_dim"])
-    out["prenet.linear.weight"] = (p["out_channels"], dim); out["prenet.linear.bias"] = (p["out_channels"],)
+    _feat_decoder_spec(out, "prenet.", p, p["condition_dim"])
     ch = d["channels"]
     wn("decoder.model.0.", (ch, d["input_channel"], 7))
     for i, (k, r) in enumerate(zip(d["kernel_sizes"], d["rates"])):
@@ -201,10 +223,38 @@ def encoder_spec(c) -> Dict[str, tuple]:
     return out
 
 
-def _ignored_prefixes(global_tokens: bool, semantic_tokens: bool) -> tuple:
-    """Checkpoint keys a BiCodec face accepts at load and does not hold: the training-only postnet, the mel transformer's buffers
+def postnet_spec(c) -> Dict[str, tuple]:
+    """Reference state-dict keys -> shapes of the postnet (feat_decoder.Decoder without a condition, bicodec.py:86,135), from the
+    config's "postnet" entry or POSTNET_PARAMS"""
+    p = c.get("postnet", POSTNET_PARAMS)
+    if p.get("use_tanh_at_final", False):
+        raise NotImplementedError("postnet use_tanh_at_final (False in the shipped configuration)")
+    if p.get("condition_dim") is not None:
+        raise NotImplementedError("a conditioned postnet (BiCodec.forward calls it without a condition, bicodec.py:135)")
+    out: Dict[str, tuple] = {}
+    _feat_decoder_spec(out, "postnet.", p, None)
+    return out
+
+
+def xvector_spec(c) -> Dict[str, tuple]:
+    """Reference state-dict keys -> shapes of ECAPA_TDNN's x-vector branch (ecapa_tdnn.py:186-192,206-208): ASTP with global context
+    (pooling_layers.py:119-132), BatchNorm1d over [mean | std] and the final Linear, without num_batches_tracked"""
+    E = "speaker_encoder.speaker_encoder."
+    out: Dict[str, tuple] = {E + "pool.linear1.weight": (ASTP_BOTTLENECK, 3 * ECAPA_OUT, 1), E + "pool.linear1.bias": (ASTP_BOTTLENECK,),
+                             E + "pool.linear2.weight": (ECAPA_OUT, ASTP_BOTTLENECK, 1), E + "pool.linear2.bias": (ECAPA_OUT,)}
+    for k in ("weight", "bias", "running_mean", "running_var"):
+        out[E + "bn." + k] = (2 * ECAPA_OUT,)
+    out[E + "linear.weight"], out[E + "linear.bias"] = (c["speaker"]["out_dim"], 2 * ECAPA_OUT), (c["speaker"]["out_dim"],)
+    return out
+
+
+def _ignored_prefixes(global_tokens: bool, semantic_tokens: bool, full: bool = False) -> tuple:
+    """Checkpoint keys a BiCodec face accepts at load and does not hold: the postnet (forward only), the mel transformer's buffers
     (rebuilt from mel_params), the FVQ usage statistics, the side of tokenize that is not built, and with the global-token path
-    the x-vector branch the reference computes and discards (speaker_encoder.py:104-109)."""
+    the x-vector branch the reference computes and discards (speaker_encoder.py:104-109).  The whole module (`full`) holds the
+    postnet and the x-vector branch; the cluster_size EMA is training state and stays ignored."""
+    if full:
+        return ("mel_transformer.", "quantizer.cluster_size")
     out = ("postnet.", "mel_transformer.", "quantizer.cluster_size")
     if not semantic_tokens:
         out += ("encoder.", "quantizer.in_project.")
@@ -263,25 +313,34 @@ def _backbone_weights(sd, prefix, layers, cond, in_scale, split):
 
 class BiCodec(_Face):
     """`global_tokens=True` adds the global-token path (`mel_spectrogram`, `get_global_tokens`) and `semantic_tokens=True` the
-    semantic-token path (`get_semantic_tokens`); with both, `tokenize` returns the pair.  Each flag makes its reference keys part of
-    the module, required by a strict load.  The default object is the detokenize path alone."""
+    semantic-token path (`get_semantic_tokens`); with both, `tokenize` returns the pair.  `full=True` is the whole reference module:
+    both token paths plus the postnet and ECAPA's x-vector branch, which only `forward` runs.  Each flag makes its reference keys part
+    of the module, required by a strict load.  The default object is the detokenize path alone."""
 
-    def __init__(self, config: dict = None, precision: str = "accurate", global_tokens: bool = False, semantic_tokens: bool = False):
+    def __init__(self, config: dict = None, precision: str = "accurate", global_tokens: Optional[bool] = None,
+                 semantic_tokens: Optional[bool] = None, full: bool = False):
         super().__init__()
         self.cfg = dict(config or BICODEC_CONFIG)
         self.policy = PRECISION[precision]
-        self.global_tokens, self.semantic_tokens = bool(global_tokens), bool(semantic_tokens)
+        self.full = bool(full)
+        if self.full and False in (global_tokens, semantic_tokens):
+            raise ValueError("BiCodec(full=True) holds both token paths: global_tokens and semantic_tokens cannot be False")
+        self.global_tokens, self.semantic_tokens = self.full or bool(global_tokens), self.full or bool(semantic_tokens)
         spec = bicodec_spec(self.cfg)
         if self.global_tokens:
             spec.update(speaker_spec(self.cfg))
         if self.semantic_tokens:
             spec.update(encoder_spec(self.cfg))
+        if self.full:
+            spec.update(postnet_spec(self.cfg))
+            spec.update(xvector_spec(self.cfg))
         tree = _Tree.build(spec)
         for name, child in tree.named_children():
             self.add_module(name, child)
-        self._ignored = _ignored_prefixes(self.global_tokens, self.semantic_tokens)
+        self._ignored = _ignored_prefixes(self.global_tokens, self.semantic_tokens, self.full)
         self._wg = None                 # prepared weights of the global-token path
         self._we = None                 # prepared weights of the semantic-token path
+        self._wf = None                 # prepared weights of what only forward runs (postnet, x-vector)
         self.eval()
 
     # ------------------------------------------------------------------ state
@@ -290,7 +349,7 @@ class BiCodec(_Face):
 
     def _drop_prepared(self):
         super()._drop_prepared()
-        self._wg = self._we = None
+        self._wg = self._we = self._wf = None
 
     # ------------------------------------------------------------------ load-time weight preparation
     def _prepare(self):
@@ -401,16 +460,21 @@ class BiCodec(_Face):
     @torch.no_grad()
     def detokenize(self, semantic_tokens: torch.Tensor, global_tokens: torch.Tensor, taps=None) -> torch.Tensor:
         """bicodec.py:182-199"""
+        pre, dvec = self._prenet(semantic_tokens, global_tokens, taps)
+        return self._wave(pre, dvec, *semantic_tokens.shape, taps)
+
+    def _prenet(self, semantic_tokens, global_tokens, taps=None):
+        """the gathers (z_q, d_vector) and prenet(z_q, d_vector) of bicodec.py:193-195 -> (prenet output [B*T, out_channels], d_vector
+        [B, out_dim]), both fp32 scratch"""
         W = self._prepare()
         c = self.cfg
-        q, s, p, d = c["quantizer"], c["speaker"], c["prenet"], c["decoder"]
-        dev = self._dev()
+        q, s, p = c["quantizer"], c["speaker"], c["prenet"]
         B, T = semantic_tokens.shape
         M = B * T
         D_in, dim, inter = q["input_dim"], p["vocos_dim"], p["vocos_intermediate_dim"]
         if dim % 64 or inter % 64 or D_in % 64 or p["out_channels"] % 64 or p["condition_dim"] % 64:
             raise ValueError("BiCodec widths must be multiples of 64")
-        sp_pre, sp_gen = self.policy["prenet"], self.policy["gen"]
+        sp_pre = self.policy["prenet"]
         # ---- z_q: codebook row @ out_project, gathered  (factorized_vector_quantize.py:154-167)
         zq = self._buf("zq", (M, D_in))
         ops.rvq_decode(semantic_tokens.reshape(M, 1).long().contiguous(), W["zq_table"], M, D_in, q["codebook_size"], 1, zq, D_in, 0)
@@ -451,6 +515,16 @@ class BiCodec(_Face):
                  out_f32=rowmap(pre, C0, M, 0))
         if p["use_tanh_at_final"]:
             raise NotImplementedError("prenet use_tanh_at_final (False in the shipped configuration)")
+        if taps is not None:
+            taps["z_q"], taps["d_vector"], taps["prenet.out"] = zq.clone(), dvec.clone(), pre.clone()
+        return pre, dvec
+
+    def _wave(self, pre, dvec, B, T, taps=None):
+        """WaveGenerator(prenet output + d_vector) (bicodec.py:196-197) -> fresh wav [B, 1, T * hop]"""
+        W = self._prepare()
+        C0, d = self.cfg["prenet"]["out_channels"], self.cfg["decoder"]
+        dev = self._dev()
+        sp_gen = self.policy["gen"]
         # ---- WaveGenerator (wave_generator.py:59-91)
         # Every Snake but one per stage rides in a GEMM epilogue: a conv's fp32 output is the residual trunk, its fp16-plane
         # output is Snake_alpha(trunk) written straight into the interior of the NEXT convolution's zero-padded buffer
@@ -471,8 +545,6 @@ class BiCodec(_Face):
         nxt_pl, nxt_ld, nxt_rpb, nxt_off = up_in(0, Tc)
         self._conv(a0, G["conv0"], ch, B, T + 6, C0, T, 7, bias=G["conv0_b"], act2=ACT_SNAKE, act2_param=stages[0]["alpha"],
                    out_planes=nxt_pl, out_planes_map=(nxt_ld, nxt_rpb, nxt_off))
-        if taps is not None:
-            taps["z_q"], taps["d_vector"], taps["prenet.out"] = zq.clone(), dvec.clone(), pre.clone()
         cl = ch // 2 ** len(d["rates"])
         for si, st in enumerate(stages):
             cin, cout, J, sdn, k = st["cin"], st["cout"], st["J"], st["s"], st["k"]
@@ -652,8 +724,13 @@ class BiCodec(_Face):
         """bicodec.py:174-178: batch["ref_wav"] [B, L] (or [B, 1, L]) -> int32 [B, 1, token_num], the layout detokenize takes.
         taps (a dict) receives channel-last fp32 copies: "mel" [B, T, num_mels], "latent" [B, T, 1536], "perceiver" [B, N, dim]
         and "z" [B, N, len(fsq_levels)], the project_in output that the FSQ bound rounds."""
+        return self._global_tokens(batch["ref_wav"] if isinstance(batch, dict) else batch, taps)[0]
+
+    def _global_tokens(self, wav, taps=None, keep_latent=False):
+        """get_global_tokens on ref_wav -> (indices, the ECAPA latent as fp32 scratch [B*T, 1536] when taps or keep_latent is given,
+        else None, and its 3-term planes, T)"""
         G = self._prepare_global()
-        wav = self._check_wav(batch["ref_wav"] if isinstance(batch, dict) else batch)
+        wav = self._check_wav(wav)
         B = wav.shape[0]
         mel, x0, T = self._mel(G, wav)
         M, C, w = B * T, ECAPA_C, ECAPA_C // ECAPA_SCALE
@@ -682,9 +759,9 @@ class BiCodec(_Face):
             ops.se_apply(z, gate, x_in, B, T, C, out=x_out, planes=cat, ld=3 * C, col_off=bi * C)
             inp, in_ld, in_off = cat, 3 * C, bi * C
         latp = self._planes("ecapa_latent_p", (M, ECAPA_OUT), True)
-        lat32 = self._buf("ecapa_latent", (M, ECAPA_OUT)) if taps is not None else None
+        lat32 = self._buf("ecapa_latent", (M, ECAPA_OUT)) if taps is not None or keep_latent else None
         ops.gemm(cat, G["conv"], ECAPA_OUT, a_batch=1, a_rows_per_batch=M, a_ld=3 * C, m_per_batch=M, bias=G["conv_b"], act=ACT_RELU,
-                 out_f32=rowmap(lat32, ECAPA_OUT, M, 0) if taps is not None else None, out_planes=latp, out_planes_map=(ECAPA_OUT, M, 0))
+                 out_f32=rowmap(lat32, ECAPA_OUT, M, 0) if lat32 is not None else None, out_planes=latp, out_planes_map=(ECAPA_OUT, M, 0))
         # ---- PerceiverResampler (perceiver_encoder.py:339-350); context rows 0..N-1 = the current latents, N.. = proj_context(x)
         s = self.cfg["speaker"]
         N, D, dp, ip = s["token_num"], G["dim"], G["dp"], G["ip"]
@@ -720,7 +797,7 @@ class BiCodec(_Face):
         if taps is not None:
             taps.update(mel=mel.clone().reshape(B, T, -1), latent=lat32.clone().reshape(B, T, ECAPA_OUT), perceiver=xn.reshape(B, N, D),
                         z=zt.reshape(B, N, nl))
-        return idx
+        return idx, lat32, latp, T
 
     # ------------------------------------------------------------------ semantic tokens
     def _prepare_semantic(self):
@@ -787,5 +864,125 @@ class BiCodec(_Face):
             raise RuntimeError(f"BiCodec.tokenize needs both token paths: construct it with {', '.join(f + '=True' for f in missing)}")
         return self.get_semantic_tokens(batch), self.get_global_tokens(batch)
 
-    def forward(self, *a, **k):
-        raise RuntimeError("unified_audio_b200.BiCodec implements detokenize only (the decoder UniSE uses, model.py:193)")
+    # ------------------------------------------------------------------ forward (eval): postnet, x-vector, codebook usage
+    def _postnet_params(self):
+        return self.cfg.get("postnet", POSTNET_PARAMS)
+
+    def _prepare_forward(self):
+        if self._wf is not None:
+            return self._wf
+        dev = self._require_cuda()
+        p, pre = self._postnet_params(), self.cfg["prenet"]
+        if any(w % 64 for w in (p["input_channels"], p["vocos_dim"], p["vocos_intermediate_dim"], p["out_channels"])):
+            raise ValueError("BiCodec postnet widths must be multiples of 64")
+        if p["input_channels"] != pre["out_channels"]:
+            raise ValueError("postnet input_channels must equal the prenet's out_channels (the postnet reads the prenet output)")
+        keys = set(postnet_spec(self.cfg)) | set(xvector_spec(self.cfg))
+        sd = {k: v.detach().double().cpu() for k, v in self.state_dict().items() if k in keys}
+        sp = self.policy["prenet"]
+        f32 = {k: v.float().to(dev) for k, v in sd.items() if k.startswith("postnet.")}
+        # the postnet follows the prenet's precision group; SamplingBlock(1)'s 3 x folded into the downsample embeds, as the encoder's
+        F = dict(lin_pre=Planes.from_f32(f32["postnet.linear_pre.weight"], sp), lin_pre_b=f32["postnet.linear_pre.bias"].contiguous(),
+                 down=[_backbone_weights(f32, f"postnet.downsample.{i}.1.", 2, None, 3.0, sp) for i in range(len(p["sample_ratios"]))],
+                 bb=_backbone_weights(f32, "postnet.vocos_backbone.", p["vocos_num_layers"], None, 1.0, sp),
+                 lin=Planes.from_f32(f32["postnet.linear.weight"], sp), lin_b=f32["postnet.linear.bias"].contiguous())
+        # x-vector: linear1 split into its x part (first 1536 input channels) and its context part [mean | std]; eval BatchNorm1d
+        # folded into the final Linear in fp64: W' = W diag(g), b' = b + W (beta - mean g), g = gamma / sqrt(var + 1e-5)
+        E = "speaker_encoder.speaker_encoder."
+        w1 = sd[E + "pool.linear1.weight"][:, :, 0]
+        g = sd[E + "bn.weight"] / torch.sqrt(sd[E + "bn.running_var"] + 1e-5)
+        w = sd[E + "linear.weight"]
+
+        def pl(t):
+            return Planes.from_f32(t.float().contiguous().to(dev), True)
+
+        F.update(w1x=pl(w1[:, :ECAPA_OUT]), w1c=pl(w1[:, ECAPA_OUT:]), b1=sd[E + "pool.linear1.bias"].float().to(dev),
+                 w2=pl(sd[E + "pool.linear2.weight"][:, :, 0]), b2=sd[E + "pool.linear2.bias"].float().to(dev),
+                 wx=pl(w * g[None, :]), bx=(sd[E + "linear.bias"] + w @ (sd[E + "bn.bias"] - sd[E + "bn.running_mean"] * g)).float().to(dev))
+        self._wf = F
+        return F
+
+    def _postnet(self, pre, B, T):
+        """postnet(x) (bicodec.py:135, feat_decoder.py:81-97 without a condition) on the prenet output [B*T, input_channels] ->
+        fresh pred_feat [B, out_channels, T] (channel-first, the reference's layout)"""
+        F, p = self._prepare_forward(), self._postnet_params()
+        M, cin, dim, inter, cout = B * T, p["input_channels"], p["vocos_dim"], p["vocos_intermediate_dim"], p["out_channels"]
+        sp = self.policy["prenet"]
+        apl = self._planes("post_in_p", (M, cin), sp)
+        ops.split_f16(pre, apl) if sp else ops.rows_to_planes(pre, 1, M, cin, apl, cin, M, 0)
+        x = self._buf("post_x", (M, dim))
+        ops.gemm(apl, F["lin_pre"], dim, a_batch=1, a_rows_per_batch=M, a_ld=cin, m_per_batch=M, bias=F["lin_pre_b"],
+                 out_f32=rowmap(x, dim, M, 0))
+        for i, bw in enumerate(F["down"]):
+            x = self._backbone(bw, x, B, T, dim, inter, tag=f"_d{i}", scope="post_")
+        x = self._backbone(F["bb"], x, B, T, dim, inter, tag="_m", scope="post_")
+        xpl = self._planes("post_out_p", (M, dim), sp)
+        ops.split_f16(x, xpl) if sp else ops.rows_to_planes(x, 1, M, dim, xpl, dim, M, 0)
+        y = self._buf("post_y", (M, cout))
+        ops.gemm(xpl, F["lin"], cout, a_batch=1, a_rows_per_batch=M, a_ld=dim, m_per_batch=M, bias=F["lin_b"], out_f32=rowmap(y, cout, M, 0))
+        out = torch.empty(B, cout, T, device=pre.device)
+        ops.ssl_compress(y, B, T, cout, 0.0, True, out)          # power 0: a plain channel-first copy
+        return out
+
+    def _xvector(self, lat32, latp, B, T):
+        """ECAPA_TDNN's x-vector linear(bn(ASTP(latent))) (ecapa_tdnn.py:206-208, pooling_layers.py:134-144) from the fp32 latent
+        [B*T, 1536] and its planes -> fresh [B, out_dim].  Every contraction is a 3-term split."""
+        F = self._prepare_forward()
+        M, C, H, n = B * T, ECAPA_OUT, ASTP_BOTTLENECK, self.cfg["speaker"]["out_dim"]
+        # linear1 over [x; mean; std]: the context part once per clip (+ b1), the x part per frame, then tanh of their sum
+        ctx, cpl = self._buf("xv_ctx", (B, 2 * C)), self._planes("xv_ctx_p", (B, 2 * C), True)
+        ops.asp_context(lat32, B, T, C, ctx, cpl, 2 * C)
+        crow = self._buf("xv_ctx_row", (B, H))
+        ops.gemm(cpl, F["w1c"], H, a_batch=1, a_rows_per_batch=B, a_ld=2 * C, m_per_batch=B, bias=F["b1"], out_f32=rowmap(crow, H, B, 0))
+        h = self._buf("xv_h", (M, H))
+        ops.gemm(latp, F["w1x"], H, a_batch=1, a_rows_per_batch=M, a_ld=C, m_per_batch=M, out_f32=rowmap(h, H, M, 0))
+        hpl = self._planes("xv_h_p", (M, H), True)
+        ops.asp_tanh_planes(h, crow, B, T, H, hpl, H)
+        logits = self._buf("xv_logits", (M, C))
+        ops.gemm(hpl, F["w2"], C, a_batch=1, a_rows_per_batch=M, a_ld=H, m_per_batch=M, bias=F["b2"], out_f32=rowmap(logits, C, M, 0))
+        # attentive [mean | std] -> BatchNorm-folded Linear
+        pooled, ppl = self._buf("xv_pool", (B, 2 * C)), self._planes("xv_pool_p", (B, 2 * C), True)
+        ops.asp_pool(lat32, logits, B, T, C, pooled, ppl, 2 * C)
+        out = torch.empty(B, n, device=lat32.device)
+        ops.gemm(ppl, F["wx"], n, a_batch=1, a_rows_per_batch=B, a_ld=2 * C, m_per_batch=B, bias=F["bx"], out_f32=rowmap(out, n, B, 0))
+        return out
+
+    def forward(self, batch=None):
+        """BiCodec.forward in evaluation mode (bicodec.py:113-149): batch {"feat": [B, T, 1024], "ref_wav": [B, L] (or [B, 1, L]),
+        "wav": any tensor with B rows}, on the device -> the reference's dict:
+          recons [B, 1, T * hop], pred_feat [B, out_channels, T] (the postnet on the prenet output, before + d_vector), x_vector and
+          d_vector [B, out_dim], perplexity and cluster_size (0-d fp32: the codebook's perplexity and number of codes used in the
+          batch), vq_loss, audios = batch["wav"].unsqueeze(1), with_speaker_loss = False.
+        vq_loss is NaN, as the reference computes it in eval mode: the mean of two empty tensors (factorized_vector_quantize.py:121-131).
+        z_q and d_vector come from the gathers detokenize uses.  The reference's forward has z_q = out_project(z_e + (q - z_e)) and
+        its d_vector from the quantised latents, which differ from detokenize's by rounding only; with the gathers, forward(batch)
+        ["recons"] equals detokenize(*tokenize(batch)) bit for bit - the reference's own check (bicodec.py:235-257), made exact.
+        Needs full=True; refused in train mode (the FVQ losses, the cluster_size EMA and straight-through gradients are not built)."""
+        if not self.full:
+            raise RuntimeError("unified_audio_b200.BiCodec.forward needs the whole module: construct it with BiCodec(..., full=True) "
+                               "and load a checkpoint that carries postnet.* and the x-vector branch")
+        if self.training:
+            raise RuntimeError("unified_audio_b200.BiCodec.forward runs in evaluation mode only: call .eval() (the FVQ losses, the "
+                               "cluster_size EMA and straight-through gradients are not built)")
+        if not isinstance(batch, dict) or any(not isinstance(batch.get(k), torch.Tensor) for k in ("feat", "ref_wav", "wav")):
+            raise ValueError('BiCodec.forward takes a dict with tensors "feat", "ref_wav" and "wav"')
+        feat, wav = batch["feat"], batch["wav"]
+        if wav.device.type != "cuda":
+            raise RuntimeError("unified_audio_b200.BiCodec runs on CUDA only (no CPU fallback): wav is on the CPU")
+        ref = self._check_wav(batch["ref_wav"])
+        if wav.ndim < 1 or feat.ndim != 3 or not feat.shape[0] == ref.shape[0] == wav.shape[0]:
+            raise ValueError("feat [B, T, C], ref_wav and wav must have the same batch size B")
+        with torch.no_grad():
+            sem = self.get_semantic_tokens(feat)
+            glob, lat32, latp, Tm = self._global_tokens(ref, keep_latent=True)
+            B, T = sem.shape
+            x_vector = self._xvector(lat32, latp, B, Tm)
+            K = self.cfg["quantizer"]["codebook_size"]
+            perplexity, active = torch.empty((), device=wav.device), torch.empty((), device=wav.device)
+            ops.fvq_usage(sem.reshape(-1), K, self._buf("fvq_counts", (K,), torch.int32), perplexity, active)
+            pre, dvec = self._prenet(sem, glob)
+            pred_feat = self._postnet(pre, B, T)
+            recons = self._wave(pre, dvec, B, T)
+            return {"vq_loss": torch.full((), float("nan"), device=wav.device), "perplexity": perplexity, "cluster_size": active,
+                    "recons": recons, "pred_feat": pred_feat, "x_vector": x_vector, "d_vector": dvec.clone(),
+                    "audios": wav.unsqueeze(1), "with_speaker_loss": False}

@@ -209,6 +209,45 @@ fvq_tokenize_kernel(const float* __restrict__ z, long long M, int D, const float
   }
 }
 
+
+// FactorizedVectorQuantize.forward's usage statistics (factorized_vector_quantize.py:97-103): an int32 histogram of the indices
+// (integer atomics: the counts do not depend on the order), then one block reduces the K bins in a fixed order in fp64.
+constexpr int FVQ_USAGE_THREADS = 256;
+
+__global__ void fvq_histogram_kernel(const int64_t* __restrict__ idx, long long n, int K, int32_t* __restrict__ counts) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int64_t k = idx[i];
+    if (k >= 0 && k < K) atomicAdd(counts + k, 1);
+  }
+}
+
+__global__ void fvq_usage_kernel(const int32_t* __restrict__ counts, int K, long long n, float* __restrict__ perplexity,
+                                 float* __restrict__ active) {
+  __shared__ double s_h[FVQ_USAGE_THREADS];
+  __shared__ int s_a[FVQ_USAGE_THREADS];
+  double h = 0.0;
+  int a = 0;
+  for (int k = threadIdx.x; k < K; k += FVQ_USAGE_THREADS) {
+    const double p = (double)counts[k] / (double)n;
+    h += p * log(p + 1e-10);
+    a += counts[k] > 0;
+  }
+  s_h[threadIdx.x] = h;
+  s_a[threadIdx.x] = a;
+  __syncthreads();
+  for (int o = FVQ_USAGE_THREADS / 2; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+      s_h[threadIdx.x] += s_h[threadIdx.x + o];
+      s_a[threadIdx.x] += s_a[threadIdx.x + o];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    *perplexity = (float)exp(-s_h[0]);
+    *active = (float)s_a[0];
+  }
+}
+
 }  // namespace qb
 using namespace qb;
 
@@ -272,6 +311,19 @@ extern "C" int qb_rvq_decode(const int64_t* idx, const float* codebooks, int64_t
   if (M == 0) return 0;
   rvq_decode_kernel<<<(unsigned)M, 128, 0, (cudaStream_t)stream>>>(idx, codebooks, D, K, nq, out, out_ld, col_off);
   g_launches++;
+  QB_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int qb_fvq_usage(const int64_t* idx, int64_t n, int32_t K, int32_t* counts, float* perplexity, float* active, void* stream) {
+  QB_REQUIRE(idx && counts && perplexity && active, "fvq_usage: bad args");
+  QB_REQUIRE(n >= 1 && K >= 1, "fvq_usage: needs at least one index and one code (n %lld, K %d)", (long long)n, K);
+  cudaStream_t st = (cudaStream_t)stream;
+  QB_CHECK_CUDA(cudaMemsetAsync(counts, 0, (size_t)K * sizeof(int32_t), st));
+  const long long g = ceil_div(n, 256);
+  fvq_histogram_kernel<<<(unsigned)(g < 132 * 16 ? g : 132 * 16), 256, 0, st>>>(idx, n, K, counts);
+  fvq_usage_kernel<<<1, FVQ_USAGE_THREADS, 0, st>>>(counts, K, n, perplexity, active);
+  g_launches += 2;
   QB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

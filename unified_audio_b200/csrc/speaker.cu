@@ -3,7 +3,8 @@
 // (QuarkAudio-UniSE/model/bicodec/bicodec.py:174-178, 201-221; modules/speaker/*.py; modules/fsq/*.py).
 // Every convolution and linear of the path is a qb_gemm (3-term split); these kernels frame and take the magnitude of the
 // spectrum around the two-stage DFT GEMMs, form the Res2Net sums, compute squeeze-excitation, run the perceiver's cross
-// attention and GEGLU, and quantise.  All fp32 arithmetic, deterministic: no atomics, fixed reduction orders.
+// attention and GEGLU, and quantise; the ASTP kernels pool the ECAPA latent into the x-vector's statistics (ecapa_tdnn.py:195-210).
+// fp32 arithmetic, except the fp64 time sums of the SE mean and the pooling; deterministic: no atomics, fixed reduction orders.
 #include <atomic>
 
 #include "common.cuh"
@@ -232,6 +233,67 @@ __global__ void fsq_tokenize_kernel(const float* __restrict__ x, long long rows,
   if (lane == 0) idx[row] = index;
 }
 
+// ASTP with global context (pooling_layers.py:119-144), the x-vector branch of ECAPA_TDNN.forward (ecapa_tdnn.py:195-210).  One
+// thread per (clip, channel), channels on threadIdx so that every frame's read is coalesced; each thread walks the T frames of its
+// channel in order with fp64 accumulators, so the result does not depend on the launch shape and no atomics are used.
+constexpr int ASP_THREADS = 128;
+
+// context: mean_c and sqrt(var_c + 1e-7) with torch.var's unbiased divisor T - 1 (two passes: the mean, then the squared deviations)
+__global__ void asp_context_kernel(const float* __restrict__ x, int T, int C, float* __restrict__ out, __half* __restrict__ hi,
+                                   __half* __restrict__ lo, long long ld) {
+  const int c = blockIdx.x * ASP_THREADS + threadIdx.x, b = blockIdx.y;
+  if (c >= C) return;
+  const float* xc = x + (long long)b * T * C + c;
+  double s = 0.0;
+  for (int t = 0; t < T; ++t) s += (double)xc[(long long)t * C];
+  const double mean = s / T;
+  double q = 0.0;
+  for (int t = 0; t < T; ++t) {
+    const double d = (double)xc[(long long)t * C] - mean;
+    q = fma(d, d, q);
+  }
+  const float m = (float)mean, sd = (float)sqrt(q / (T - 1) + 1e-7);
+  out[(long long)b * 2 * C + c] = m;
+  out[(long long)b * 2 * C + C + c] = sd;
+  put_planes(hi, lo, b * ld + c, m);
+  put_planes(hi, lo, b * ld + C + c, sd);
+}
+
+// tanh(h[b*T + t, n] + row[b, n]) -> planes [B*T, ld], zero past N: linear1's x part (a GEMM over the frames) plus its context
+// part and bias (one row per clip), then the tanh (pooling_layers.py:138-139)
+__global__ void asp_tanh_planes_kernel(const float* __restrict__ h, const float* __restrict__ row, int T, int N, __half* __restrict__ hi,
+                                       __half* __restrict__ lo, long long ld) {
+  const long long r = blockIdx.x;
+  const float* hr = h + r * N;
+  const float* rr = row + (r / T) * N;
+  for (int n = threadIdx.x; n < ld; n += blockDim.x) put_planes(hi, lo, r * ld + n, n < N ? tanhf(hr[n] + rr[n]) : 0.f);
+}
+
+// attentive statistics (pooling_layers.py:140-143): alpha = softmax over T of the logits (maximum subtracted), mean = sum alpha x,
+// std = sqrt(max(sum alpha x^2 - mean^2, 1e-7)); exponentials and sums in fp64
+__global__ void asp_pool_kernel(const float* __restrict__ x, const float* __restrict__ logits, int T, int C, float* __restrict__ out,
+                                __half* __restrict__ hi, __half* __restrict__ lo, long long ld) {
+  const int c = blockIdx.x * ASP_THREADS + threadIdx.x, b = blockIdx.y;
+  if (c >= C) return;
+  const long long base = (long long)b * T * C + c;
+  float mx = -INFINITY;
+  for (int t = 0; t < T; ++t) mx = fmaxf(mx, logits[base + (long long)t * C]);
+  double se = 0.0, s1 = 0.0, s2 = 0.0;
+  for (int t = 0; t < T; ++t) {
+    const double e = exp((double)logits[base + (long long)t * C] - (double)mx);
+    const double v = (double)x[base + (long long)t * C];
+    se += e;
+    s1 = fma(e, v, s1);
+    s2 = fma(e * v, v, s2);
+  }
+  const double mean = s1 / se, var = s2 / se - mean * mean;
+  const float m = (float)mean, sd = (float)sqrt(fmax(var, 1e-7));
+  out[(long long)b * 2 * C + c] = m;
+  out[(long long)b * 2 * C + C + c] = sd;
+  put_planes(hi, lo, b * ld + c, m);
+  put_planes(hi, lo, b * ld + C + c, sd);
+}
+
 }  // namespace qb
 using namespace qb;
 
@@ -313,5 +375,30 @@ extern "C" int qb_fsq_tokenize(const float* x, int64_t rows, int32_t dim, const 
   }
   QB_REQUIRE(cb <= (double)(1 << 24), "fsq_tokenize: codebook larger than 2^24 entries");
   fsq_tokenize_kernel<<<(unsigned)ceil_div(rows, 8), 256, 0, (cudaStream_t)stream>>>(x, rows, dim, gamma, w_in, b_in, lv, idx, z, xn);
+  QB_LAUNCH_END();
+}
+
+extern "C" int qb_asp_context(const float* x, int64_t B, int64_t T, int32_t C, float* out, qb_half* hi, qb_half* lo, int64_t ld,
+                              void* stream) {
+  QB_REQUIRE(x && out && hi && B >= 1 && C >= 1 && 2 * (int64_t)C <= ld, "asp_context: bad args (ld must hold 2 C columns)");
+  QB_REQUIRE(T >= 2 && T <= INT32_MAX, "asp_context: the unbiased variance needs T >= 2 frames (got %lld)", (long long)T);
+  asp_context_kernel<<<dim3((unsigned)ceil_div(C, ASP_THREADS), (unsigned)B), ASP_THREADS, 0, (cudaStream_t)stream>>>(
+      x, (int)T, C, out, (__half*)hi, (__half*)lo, ld);
+  QB_LAUNCH_END();
+}
+
+extern "C" int qb_asp_tanh_planes(const float* h, const float* row, int64_t B, int64_t T, int32_t N, qb_half* hi, qb_half* lo, int64_t ld,
+                                  void* stream) {
+  QB_REQUIRE(h && row && hi && B >= 1 && T >= 1 && T <= INT32_MAX && N >= 1 && N <= ld, "asp_tanh_planes: bad args");
+  asp_tanh_planes_kernel<<<(unsigned)(B * T), 128, 0, (cudaStream_t)stream>>>(h, row, (int)T, N, (__half*)hi, (__half*)lo, ld);
+  QB_LAUNCH_END();
+}
+
+extern "C" int qb_asp_pool(const float* x, const float* logits, int64_t B, int64_t T, int32_t C, float* out, qb_half* hi, qb_half* lo,
+                           int64_t ld, void* stream) {
+  QB_REQUIRE(x && logits && out && hi && B >= 1 && T >= 1 && T <= INT32_MAX && C >= 1 && 2 * (int64_t)C <= ld,
+             "asp_pool: bad args (ld must hold 2 C columns)");
+  asp_pool_kernel<<<dim3((unsigned)ceil_div(C, ASP_THREADS), (unsigned)B), ASP_THREADS, 0, (cudaStream_t)stream>>>(
+      x, logits, (int)T, C, out, (__half*)hi, (__half*)lo, ld);
   QB_LAUNCH_END();
 }

@@ -325,6 +325,11 @@ def fvq_tokenize(z, M, D_in, w_in, b_in, codebook_n, K, cdim, idx, z_e=None):
     _lib.check(_lib.load().qb_fvq_tokenize(_p(z), M, D_in, _p(w_in), _p(b_in), _p(codebook_n), K, cdim, _p(idx), _p(z_e), _stream()))
 
 
+def fvq_usage(idx, K, counts, perplexity, active):
+    """idx int64 [n] -> perplexity and active-code count (0-d fp32 device tensors); counts: int32 [K] scratch"""
+    _lib.check(_lib.load().qb_fvq_usage(_p(idx), idx.numel(), K, _p(counts), _p(perplexity), _p(active), _stream()))
+
+
 def lm_qkv_prep(qkv, B, L, heads, pos0, cos, sin, q16, kc, vc, Lmax):
     _lib.check(_lib.load().qb_lm_qkv_prep(_p(qkv), B, L, heads, pos0, _p(cos), _p(sin), _p(q16), _p(kc), _p(vc), Lmax,
                                           _stream()))
@@ -480,6 +485,21 @@ def fsq_tokenize(x, rows, dim, gamma, w_in, b_in, levels, num_quantizers, idx, z
     lv = (C.c_int32 * len(levels))(*levels)
     _lib.check(_lib.load().qb_fsq_tokenize(_p(x), rows, dim, _p(gamma), _p(w_in), _p(b_in), len(levels), lv, num_quantizers, _p(idx),
                                            _p(z), _p(xn), _stream()))
+
+
+def asp_context(x, B, T, Cc, out, planes: Planes, ld):
+    """latent [B*T, Cc] -> [mean | unbiased std + 1e-7] fp32 [B, 2 Cc] and planes [B, ld]"""
+    _lib.check(_lib.load().qb_asp_context(_p(x), B, T, Cc, _p(out), _p(planes.hi), _p(planes.lo), ld, _stream()))
+
+
+def asp_tanh_planes(h, row, B, T, N, out: Planes, ld):
+    """tanh(h [B*T, N] + row [B, N] per clip) -> planes [B*T, ld]"""
+    _lib.check(_lib.load().qb_asp_tanh_planes(_p(h), _p(row), B, T, N, _p(out.hi), _p(out.lo), ld, _stream()))
+
+
+def asp_pool(x, logits, B, T, Cc, out, planes: Planes, ld):
+    """softmax-over-T attentive [mean | std] of x [B*T, Cc] -> fp32 [B, 2 Cc] and planes [B, ld]"""
+    _lib.check(_lib.load().qb_asp_pool(_p(x), _p(logits), B, T, Cc, _p(out), _p(planes.hi), _p(planes.lo), ld, _stream()))
 
 
 def lm_loss(logits, ld, M, V, targets, label_smoothing):
